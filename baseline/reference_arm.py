@@ -1,7 +1,7 @@
 """The reference arm of bench.py: the UNMODIFIED MeshDiffusion modules from baseline/_ref (lib/diffusion/models/ddpm_res64.py,
 sde_lib.py, sampling.py, configs/res64.py) driven through the reference's own public API -- mutils.create_model,
 sampling.get_sampling_fn -> pc_sampler -- on the host cores (`--impl reference`) or, as the stock-PyTorch-GPU baseline of
-the bench line, on the same B200. Nothing of this repository's package is imported here.
+the bench line, on the same GPU. Nothing of this repository's package is imported here.
 
 Run-time patches applied from the outside (SURVEY 8c), none of which touches the reference's arithmetic:
   * `ml_collections` is not installed: a minimal attribute-dict stand-in is put in sys.modules for configs/*.py;

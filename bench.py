@@ -9,20 +9,24 @@ A "step" is one denoising step of pc_sampler for one batch: U-Net evaluation + a
 [batch, 4, 64, 64, 64]. metric = sample-steps/s = batch * steps / time, whole job (sum over ranks).
 
 The HEADLINE is measured in the operand mode that meets north_star's parity contract (1e-3 against the reference's
-fp32 arithmetic): `bf16x3`, split-bf16 operands (hi*hi + hi*lo + lo*hi into the fp32 TMEM accumulator). The same line
+fp32 arithmetic): `bf16x3`, split-bf16 operands (hi*hi + hi*lo + lo*hi into the fp32 wgmma accumulator). The same line
 carries complete secondary legs (`legs`: value, e2e, roofline, clocks each) for `tf32` operands (the arithmetic class of
 the reference's own stock GPU path, 1.3e-3) and plain `bf16` operands (throughput mode, 1.2e-2).
 
   value     : device-resident loop (mdb_sampler_run: state, noise and coefficients never leave HBM), CUDA events.
   e2e       : same steps through the public Python API (model(x, labels) + fused update) with the state copied
               host->device from pinned memory before and device->host after EVERY step.
-  roofline  : the tcgen05 implicit-GEMM kernel: algorithmic FLOPs / CUDA-event time of exactly those launches inside
-              one forward, against the measured sustained bf16 cuBLAS peak (MEASURED_PEAKS.json) divided by the tensor
-              instructions the mode issues per product (1 bf16, 2 tf32, 3 bf16x3).
+  roofline  : the wgmma implicit-GEMM kernel: algorithmic FLOPs / CUDA-event time of exactly those launches inside
+              one forward, against the bf16 tensor peak (MEASURED_PEAKS.json if present, else the H100 SXM data sheet)
+              divided by the tensor instructions the mode issues per product (1 bf16, 2 tf32, 3 bf16x3).
   cpu_baseline       : the unmodified reference modules (baseline/_ref) on the host cores, B=1 (bounded sample).
-  torch_gpu_baseline : the same reference modules under stock PyTorch on the same B200 (TF32 default / strict fp32 /
+  torch_gpu_baseline : the same reference modules under stock PyTorch on the same GPU (TF32 default / strict fp32 /
                        bf16 autocast) -- the same-box stand-in for the "1x A100-equivalent PyTorch-GPU" figure.
   train     : BASELINE configs[2], one optimiser step of the PRODUCT training path (tools/bench_train.py), all ranks.
+
+--dump-outputs DIR writes what the timed device-resident loop of every operand mode returned after its last step (the
+state x and its mean x_mean) as DIR/<mode>_<name>.npy, float32: the same seeded sample of 2^21 elements of each array in
+every run, so that two builds can be compared output for output on identical inputs.
 """
 import argparse
 import json
@@ -47,8 +51,7 @@ PARITY = {"bf16x3": "fp32-class: full res64 net 4e-5 max-rel vs the fp32 oracle,
 
 
 def host_threads():
-    """oneDNN conv3d scales to ~32 threads on this host class and gets slower beyond (measured on the 128-core GPU box:
-    16 thr 6.7 s, 32 thr 6.1 s, 64 thr 8.3 s, 128 thr 46 s per res64 forward) -- use what is actually useful."""
+    """oneDNN conv3d stops scaling at a few dozen threads for this network and gets slower beyond; 32 at most."""
     return int(os.environ.get("MDB_CPU_THREADS", min(32, os.cpu_count() or 1)))
 
 
@@ -58,7 +61,8 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # H100 SXM data sheet (dense bf16, HBM3); a power-limited card reaches less
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -139,7 +143,19 @@ class Ctx:
         return t.item()
 
 
-def sampler_leg(ctx, precision, B, R, K, W, dump_profile=None, full_run=False):
+def dump_outputs(d, prefix, arrays, n=1 << 21):
+    """Each array as DIR/<prefix><name>.npy in float32: all of it, or the elements at the same seeded indices every run."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1).float()
+        if flat.numel() > n:
+            idx = np.sort(np.random.default_rng(0).choice(flat.numel(), n, replace=False))
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+        np.save(os.path.join(d, f"{prefix}{name}.npy"), flat.cpu().numpy())
+
+
+def sampler_leg(ctx, precision, B, R, K, W, dump_profile=None, full_run=False, dump_dir=None):
     """One operand mode: device-resident loop, end-to-end loop, roofline of the GEMM launches, clocks."""
     from meshdiffusion_b200.diffusion import sde_lib, sampling
     from meshdiffusion_b200.geometry.dmtet import grid_mask_from_tets
@@ -168,12 +184,14 @@ def sampler_leg(ctx, precision, B, R, K, W, dump_profile=None, full_run=False):
     clocks.start()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    native_steps(W, K)
+    x_mean = native_steps(W, K)
     e1.record()
     ctx.barrier()
     ms = ctx.max_over_ranks(e0.elapsed_time(e1))
     clk = clocks.stop()
     value = world * B * K / (ms * 1e-3)
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, f"{precision}_", {"x": x, "x_mean": x_mean})
 
     # ---- the complete 999-evaluation run (opt-in: minutes), so samples/s is measured rather than extrapolated
     full = None
@@ -228,13 +246,13 @@ def sampler_leg(ctx, precision, B, R, K, W, dump_profile=None, full_run=False):
         peaks, src = measured_peaks()
         flops = info["flops_per_sample"] * B
         # FLOPs of the non-conv GEMMs (attention, stem) are < 3 % of the total; the roofline is quoted on all launches of
-        # the tcgen05 kernel together: algorithmic FLOPs / their summed duration
+        # the wgmma kernel together: algorithmic FLOPs / their summed duration
         per = MMA_PER_PRODUCT[precision]
         peak = peaks["bf16_tflops_sustained"] / per
         ach = flops / (all_gemm_ms * 1e-3) / 1e12
         fwd_ms = sum(t for _, t in prof)
-        roofline = {"bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05 implicit-GEMM conv3d / NIN / attention)",
-                    "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": ncu_traffic(precision),
+        roofline = {"bound": "tensor", "kernel": "gemm_tc_kernel (wgmma implicit-GEMM conv3d / NIN / attention)",
+                    "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
                     "peak_source": f"{src} bf16_tflops_sustained" + (f" / {per:g} ({precision}: {per:g} bf16-rate tensor instructions per product)" if per != 1 else ""),
                     "issued_tflops": ach * per, "gemm_ms_per_forward": all_gemm_ms, "conv_ms_per_forward": conv_ms,
                     "forward_ms": fwd_ms, "non_gemm_share_of_forward": 1.0 - all_gemm_ms / fwd_ms,
@@ -250,25 +268,6 @@ def sampler_leg(ctx, precision, B, R, K, W, dump_profile=None, full_run=False):
     del model, net
     torch.cuda.empty_cache()
     return leg, mask
-
-
-def ncu_traffic(precision):
-    """dram read+write bytes per launch of the dominant launch type (128->128 conv @64^3) from the committed `ncu --set full`
-    capture of this mode (taken at batch 8; reported as captured, with its batch and source file), or null."""
-    name = {"bf16": "r02_ncu_conv_final_bf16.txt", "bf16x3": "r02_ncu_conv_final_bf16x3.txt", "tf32": "r02_ncu_conv_final_tf32.txt"}[precision]
-    path = os.path.join(ROOT, "profiles", name)
-    try:
-        rd = wr = None
-        for line in open(path):
-            if "dram__bytes_read.sum =" in line and rd is None:
-                v, u = line.split("=")[1].split()[:2]; rd = float(v) * (1e9 if u.startswith("G") else 1e6)
-            if "dram__bytes_write.sum =" in line and wr is None:
-                v, u = line.split("=")[1].split()[:2]; wr = float(v) * (1e9 if u.startswith("G") else 1e6)
-        es = 2 if precision == "bf16" else 4
-        return {"bytes_per_launch": rd + wr, "batch": 8, "launch": "conv3x3x3 128->128 @64^3", "source": f"profiles/{name} (static capture, not this run)",
-                "algorithmic_bytes_per_launch": 2 * 8 * 64 ** 3 * 128 * es + 27 * 128 * 128 * es * (1.5 if precision == "bf16x3" else 1)}
-    except Exception:
-        return None
 
 
 def _is_gemm(name):
@@ -306,7 +305,7 @@ def run_ours(args):
     legs, mask = {}, None
     for i, prec in enumerate(precisions):
         legs[prec], mask = sampler_leg(ctx, prec, B, R, K, W, dump_profile=args.dump_profile if i == 0 else None,
-                                       full_run=args.full_run and i == 0)
+                                       full_run=args.full_run and i == 0, dump_dir=args.dump_outputs)
         if ctx.rank == 0:  # progress on stderr (stdout carries only the final JSON line)
             print(f"[bench] {prec}: value {legs[prec]['value']:.2f} e2e {legs[prec]['e2e']['value']:.2f} {UNIT}, "
                   f"gemm frac {legs[prec]['roofline']['frac']:.3f}", file=sys.stderr, flush=True)
@@ -374,7 +373,7 @@ def run_reference(args):
     from baseline import reference_arm
     K, W = args.steps, args.warmup
     if not reference_arm.available():
-        print(json.dumps({"impl": "reference", "unavailable": "baseline/_ref is missing (built by __graft_entry__.build() where /root/reference exists)"}))
+        print(json.dumps({"impl": "reference", "unavailable": "baseline/_ref is missing (staged by __graft_entry__.build() where the reference tree is present)"}))
         return
     threads = host_threads()
     torch.set_num_threads(threads)
@@ -413,6 +412,8 @@ def main():
     ap.add_argument("--no-torch-gpu-baseline", action="store_true")
     ap.add_argument("--no-train-leg", action="store_true", help="skip the training-step measurement (tools/bench_train.py)")
     ap.add_argument("--dump-profile", default=None, help="write the per-launch CUDA-event times of one forward as JSON")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the timed loop of each operand mode computed in its last step as DIR/<mode>_<name>.npy")
     args = ap.parse_args()
     if args.batch is None:
         args.batch = 8 if args.res == 128 else 32
@@ -422,7 +423,7 @@ def main():
         run_reference(args)
         return
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: the hot path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs a CUDA GPU (H100): the hot path has no CPU fallback (use --impl reference for the CPU arm)")
     run_ours(args)
 
 

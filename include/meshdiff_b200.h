@@ -1,4 +1,4 @@
-/* meshdiff_b200 -- C ABI of the B200-native MeshDiffusion hot path.
+/* meshdiff_b200 -- C ABI of the H100-native MeshDiffusion hot path.
  *
  * The reference (lzzcd001/MeshDiffusion) has no FFI on this path: its seam is a set of Python callables
  * (SURVEY.md section 8b). Each entry point below names the reference callable it replaces. All pointers are raw

@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a shared library (no JIT cache: the .so must travel with the repo snapshot)."""
+"""In-tree build of the sm_90a shared library (no JIT cache: the .so must travel with the repo snapshot)."""
 import os
 import subprocess
 import sys
@@ -8,10 +8,15 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libmeshdiff_b200.so")
 SOURCES = ["gemm_host.cu", "wgrad_host.cu", "elementwise.cu", "backward.cu", "unet.cu", "unet_train.cu", "marching_tets.cu", "mesh_ops.cu", "train_ops.cu", "api.cu"]
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH_FLAGS + [
+    "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
+    "-Xptxas", "-v",  # the per-kernel report is where ptxas says it had to serialise wgmma (checked below)
 ]
+# ptxas reports that make a wgmma kernel issue one MMA at a time (it waits for each to finish before the next): a build that
+# would silently lose the MMA pipelining fails instead
+SERIALISED_WGMMA = ("C7510", "C7520")
 
 
 def _newest_mtime(paths):
@@ -42,15 +47,19 @@ def _build_locked(force, verbose):
     for s in srcs:
         o = os.path.join(LIBDIR, os.path.basename(s)[:-3] + ".o")
         objs.append(o)
-        cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", s, "-o", o]
+        cmd = [nvcc] + NVCC_FLAGS + ["-c", s, "-o", o]
         procs.append((cmd, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
     for cmd, p in procs:
         out, _ = p.communicate()
+        out = out.decode()
         if verbose or p.returncode != 0:
-            sys.stderr.write(out.decode())
+            sys.stderr.write(out)
         if p.returncode != 0:
             raise RuntimeError("nvcc failed: " + " ".join(cmd))
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-lcudart", "-ldl"]
+        serialised = [line for line in out.splitlines() if any(code in line for code in SERIALISED_WGMMA)]
+        if serialised:
+            raise RuntimeError("ptxas serialised wgmma in " + cmd[-3] + ":\n" + "\n".join(serialised))
+    cmd = [nvcc] + ARCH_FLAGS + ["-shared", "-o", LIB] + objs + ["-lcudart", "-ldl"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -36,8 +36,8 @@ __device__ __forceinline__ float dsilu(float y) {
   return s * fmaf(y, 1.f - s, 1.f);
 }
 
-// grid.x for the staged, grid-stride kernels: the whole grid is ONE full wave of `target` = 148 x (resident blocks per
-// SM) blocks -- a 608-block launch at 2 blocks/SM (296 resident) spends a third, nearly empty wave on 16 blocks.
+// grid.x for the staged, grid-stride kernels: the whole grid is ONE full wave of `target` = 132 x (resident blocks per
+// SM) blocks -- a launch a few blocks over one wave would spend a second, nearly empty wave on them.
 static inline int blocks_x(long long voxels, int k, int B, int target) {
   long long gx = (voxels + (long long)k * 4 - 1) / ((long long)k * 4);
   long long want = target / B;
@@ -207,7 +207,7 @@ void launch_gn_bwd_reduce(const GnBwdArgs& a, int B, cudaStream_t s) {
   int cv, k;
   gn_launch_shape(a, cv, k);
   const int C = a.C0 + a.C1;
-  const int gx = blocks_x(a.voxels, k, B, 296);
+  const int gx = blocks_x(a.voxels, k, B, 2 * 132);
   gn_bwd_reduce_kernel<<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
   MDB_LAUNCH_CHECK();
   gn_bwd_sums_kernel<<<(B * C + 255) / 256, 256, 0, s>>>(a.part, a.sums, gx, B * C);
@@ -347,7 +347,7 @@ void launch_gn_bwd_apply(const GnBwdArgs& a, int B, cudaStream_t s) {
   int cv, k;
   gn_launch_shape(a, cv, k);
   const int C = a.C0 + a.C1;
-  const int gx = blocks_x(a.voxels, k, B, 444);
+  const int gx = blocks_x(a.voxels, k, B, 3 * 132);
   static bool configured_dev[64] = {};  // the attribute is per device
   int dev = 0;
   cudaGetDevice(&dev);
@@ -505,7 +505,7 @@ void launch_colsum(const ColsumArgs& a, int B, cudaStream_t s) {
   const int cv = a.C / VEC;
   if (cv < 1 || cv > 256 || a.C % VEC != 0) throw std::runtime_error("mdb: unsupported channel count in colsum");
   const int k = 256 / cv;
-  const int gx = blocks_x(a.voxels, k, B, 592);
+  const int gx = blocks_x(a.voxels, k, B, 4 * 132);
   colsum_kernel<<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
   MDB_LAUNCH_CHECK();
   colsum_final_kernel<<<(a.C + 31) / 32, dim3(32, 8), 0, s>>>(a, gx, B);
@@ -515,7 +515,7 @@ void launch_colsum(const ColsumArgs& a, int B, cudaStream_t s) {
 // ------------------------------------------------------------------ resampling data movement
 static inline int grid_for(long long work_items, int threads) {
   long long b = (work_items + threads - 1) / threads;
-  const long long cap = 148LL * 8;
+  const long long cap = 132LL * 8;
   if (b > cap) b = cap;
   return b < 1 ? 1 : (int)b;
 }
@@ -643,7 +643,7 @@ __global__ void __launch_bounds__(256) softmax_bwd_rows_kernel(const float* __re
 }
 void launch_softmax_bwd_rows(const float* P, float* dP, long long rows, int L, cudaStream_t s) {
   if (L > 16 * 256) throw std::runtime_error("mdb: softmax row too long");
-  const int grid = (int)(rows < 148LL * 16 ? rows : 148LL * 16);
+  const int grid = (int)(rows < 132LL * 16 ? rows : 132LL * 16);
   softmax_bwd_rows_kernel<<<grid, 256, 0, s>>>(P, dP, rows, L);
   MDB_LAUNCH_CHECK();
 }

@@ -15,7 +15,7 @@ namespace mdb {
 
 static inline int grid_for(long long work_items, int threads) {
   long long b = (work_items + threads - 1) / threads;
-  const long long cap = 148LL * 8;
+  const long long cap = 132LL * 8;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
   return (int)b;
@@ -216,7 +216,7 @@ void launch_norm_act(const NormActArgs& a, int B, cudaStream_t s) {
   const int k = 256 / cv;  // voxels per block pass
   const int threads = cv * k;
   long long gx = (a.voxels + (long long)k * 4 - 1) / ((long long)k * 4);
-  const long long cap = (148LL * 8 + B - 1) / B;
+  const long long cap = (132LL * 8 + B - 1) / B;
   if (gx > cap) gx = cap;
   if (gx < 1) gx = 1;
   dim3 grid((unsigned)gx, (unsigned)B);
@@ -390,7 +390,7 @@ __global__ void softmax_rows_kernel(float* __restrict__ s, long long rows, int L
 }
 void launch_softmax_rows(float* s, long long rows, int L, int tf32, cudaStream_t st) {
   if (L > 16 * 256) throw std::runtime_error("mdb: softmax row too long");
-  const int grid = (int)(rows < 148LL * 16 ? rows : 148LL * 16);
+  const int grid = (int)(rows < 132LL * 16 ? rows : 132LL * 16);
   if (tf32 == 1) softmax_rows_kernel<1><<<grid, 256, 0, st>>>(s, rows, L);
   else if (tf32 == 2) softmax_rows_kernel<2><<<grid, 256, 0, st>>>(s, rows, L);
   else softmax_rows_kernel<0><<<grid, 256, 0, st>>>(s, rows, L);
@@ -546,7 +546,7 @@ void launch_tap_shift_sum(const void* P, long long ldp, int p_fp32, const float*
   if (Cout != 4) throw std::runtime_error("mdb: tap_shift_sum supports 4 output channels");
   const long long V = (long long)R * R * R;
   long long gx = (V + 255) / 256;
-  const long long cap = (148LL * 16 + B - 1) / B;
+  const long long cap = (132LL * 16 + B - 1) / B;
   if (gx > cap) gx = cap;
   dim3 grid((unsigned)gx, (unsigned)B);
   if (p_fp32) tap_shift_sum_kernel<true><<<grid, 256, 0, s>>>(P, ldp, bias, out, R, k);

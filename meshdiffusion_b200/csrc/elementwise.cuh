@@ -1,4 +1,4 @@
-// Bandwidth-bound kernels around the tcgen05 contractions: GroupNorm finalize/apply (+SiLU), nearest 2x upsample,
+// Bandwidth-bound kernels around the wgmma contractions: GroupNorm finalize/apply (+SiLU), nearest 2x upsample,
 // stem im2col, attention softmax / V transpose, time-embedding MLP, ancestral-sampling update.
 // All of these are HBM-roofline kernels: 16-byte vector accesses, grid-stride loops sized to the SM count.
 #pragma once

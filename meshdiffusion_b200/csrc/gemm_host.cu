@@ -1,4 +1,4 @@
-// Host-side builders for the tcgen05 implicit-GEMM kernel (see gemm_tc.cuh).
+// Host-side builders for the wgmma implicit-GEMM kernel (see gemm_tc.cuh).
 #include "gemm_host.h"
 #include "elementwise.cuh"
 #include <cstring>
@@ -46,15 +46,6 @@ void encode_map(CUtensorMap* m, Precision prec, int rank, void* base, const uint
   }
 }
 
-static int sm_count_or_default() {
-  int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
-    cudaGetLastError();
-    return 148;
-  }
-  return n;
-}
-
 int sm_count() {
   static int n = 0;
   if (!n) {
@@ -84,7 +75,7 @@ int plan_splits(int X, int Y, int Z, int B, int N, int cin_total, int taps, Prec
   const int tiles = tiles_m * ((N + block_n - 1) / block_n);
   const int ksteps = ((cin_total + kb_elems(prec) - 1) / kb_elems(prec)) * taps * (prec == kBF16X3 ? 3 : 1);
   if (tiles > 49 || ksteps < 48) return 1;
-  int S = 148 / tiles;
+  int S = kPlanSMs / tiles;
   if (S > 16) S = 16;
   if (S > ksteps / 8) S = ksteps / 8;
   return S < 2 ? 1 : S;
@@ -92,7 +83,7 @@ int plan_splits(int X, int Y, int Z, int B, int N, int cin_total, int taps, Prec
 
 void GemmOp::enable_splits(int S, float* scratch) {
   if (S <= 1) return;
-  if (pair || p.ocs != 1 || p.out_fp32 || p.bias_on_m || p.alpha != 1.f || p.res_fp32)
+  if (p.ocs != 1 || p.out_fp32 || p.bias_on_m || p.alpha != 1.f || p.res_fp32)
     throw std::runtime_error("mdb: split-K is only wired for plain NDHWC conv outputs");
   if (p.osx != (long long)p.N * parts(prec) || (p.res && p.rsx != (long long)p.N * parts(prec)))
     throw std::runtime_error("mdb: split-K needs dense [B][V][N] output / residual");
@@ -123,13 +114,6 @@ void GemmOp::set_output_strided(Precision pr, int X, int Y, int Z, int B, int N,
   p.N = N;
   block_n = N <= 32 ? 32 : 128;
   p.n_tiles_n = (N + block_n - 1) / block_n;
-  { const char* f = getenv("MDB_DBG_FLAGS"); p.dbg_flags = f ? atoi(f) : 0; }
-  {
-    // CTA pairs (tcgen05 cta_group::2) whenever there are enough M-tiles to keep all 74 pairs busy
-    const char* e = getenv("MDB_CTA_PAIRS");
-    const int tiles_m = p.tx * p.ty * p.tz * p.tb;
-    pair = block_n == 128 && tiles_m * p.n_tiles_n >= 2 * (sm_count_or_default() / 2) && !(e && e[0] == '0');
-  }
   p.out = out;
   p.osx = osx; p.osy = osy; p.osz = osz; p.osb = osb;
   p.out_fp32 = out_fp32 ? 1 : 0;
@@ -180,15 +164,7 @@ int GemmOp::add_amap(const Act& a, int halo, int sub, int px, int py, int pz, in
 void GemmOp::add_load_x(int tm_hi, int tm_lo, int nk, int rows, int jrows, int dx, int dy, int dz, int c0, int wsrc,
                         int wc0, int tap0, int tapj) {
   if (prec != kBF16X3) { add_load(tm_hi, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 0); return; }
-  if (pair) {
-    // CTA pairs: a (hi, lo) couple of stages -- (A hi, W hi) then (A lo, W lo) -- from which the MMA warp forms the three
-    // products itself (GemmSeg::x3pair): every operand byte crosses L2 -> SMEM once
-    add_load(tm_hi, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 0);
-    add_load(tm_lo, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 1);
-    return;
-  }
-  // K-extension form (single CTAs: small problems, split-K). Small terms first: (A lo, W hi) and (A hi, W lo) are ~2^-9
-  // of the leading product
+  // K-extension form. Small terms first: (A lo, W hi) and (A hi, W lo) are ~2^-9 of the leading product
   add_load(tm_lo, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 0);
   add_load(tm_hi, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 1);
   add_load(tm_hi, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 0);
@@ -349,7 +325,7 @@ void GemmOp::set_gn_backward(const void* x0, long long ld0, int c0, const void* 
 void GemmOp::encode_bmap(void* ptr, int K, int N, int batch, long long rsb, long long bsb) {
   uint64_t dims[3] = {(uint64_t)K, (uint64_t)N, (uint64_t)batch};
   uint64_t strides[2] = {(uint64_t)rsb, (uint64_t)bsb};
-  uint32_t box[3] = {(uint32_t)kb_elems(prec), (uint32_t)(pair ? block_n / 2 : block_n), 1};
+  uint32_t box[3] = {(uint32_t)kb_elems(prec), (uint32_t)block_n, 1};
   encode_map(&p.bmap, prec, 3, ptr, dims, strides, box);
 }
 
@@ -446,7 +422,7 @@ void GemmOp::repack(cudaStream_t stream) {
   const int KB = kb_elems(prec), n_loads = (int)loads.size();
   const long long total = 1LL * p.N * n_loads * (KB / 8);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kPlanSMs * 16) blocks = kPlanSMs * 16;
   if (prec == kTF32)
     pack_weights_kernel<1><<<blocks, 256, 0, stream>>>(d_loads, d_ks0, n_loads, args, p.N, ksteps, KB, d_wpacked);
   else if (prec == kBF16X3)
@@ -474,54 +450,29 @@ void GemmOp::finalize(cudaStream_t stream, bool pack) {
   p.loads = d_loads;
   p.n_loads = (int)loads.size();
   if (p.splits < 1) p.splits = 1;
-  // pipeline segments: runs of identical entries; plain (nk == 1) entries are paired two per stage. The stage size is the
-  // largest group of this op and the ring takes as many stages as fit in the 227 KB next to the epilogue scratch.
+  // pipeline segments: runs of identical entries, one entry (its A box and the weight tiles of its k-steps) per stage.
+  // The stage size is the largest group of this op and the ring takes as many stages as fit next to the epilogue scratch.
   {
-    const int btile = block_n * kRowBytes / (pair ? 2 : 1);
-    const int max_stage = pair ? (2 * 128 * kRowBytes + 2 * 64 * kRowBytes) : (kAStageBytes + 3 * 128 * kRowBytes);
-    const bool x3pair = pair && prec == kBF16X3;
-    {
-      // two M-tiles per CTA (weight tiles shared by both): bf16 / tf32 pair kernels with packed weights and enough tiles to
-      // fill every pair with 4-tile work items; MDB_M2=0 switches it off
-      const char* e = getenv("MDB_M2");
-      const int tiles_m = p.tx * p.ty * p.tz * p.tb;
-      m2 = pair && prec != kBF16X3 && !b_from_act && block_n == 128 && !(e && e[0] == '0') &&
-           (long long)tiles_m * p.n_tiles_n >= 4LL * (sm_count_or_default() / 2);
-    }
+    const int btile = block_n * kRowBytes;
+    const int max_stage = kAStageBytes + 3 * 128 * kRowBytes;
     stage_need = 0;
     p.n_segs = 0;
-    auto push = [&](int n_groups, int epg, const LoadEntry& e, int couple) {
-      if (n_groups <= 0) return;
-      if (p.n_segs >= kMaxSegs) throw std::runtime_error("mdb: too many pipeline segments");
-      GemmSeg sg{};
-      sg.n_groups = n_groups; sg.epg = epg; sg.nk = e.nk;
-      sg.a_bytes = e.rows * kRowBytes;
-      sg.a_stride = (sg.a_bytes + 1023) / 1024 * 1024;
-      sg.jbytes = e.jrows * kRowBytes;
-      sg.x3pair = couple;
-      const int need = m2 ? 2 * sg.a_stride + e.nk * btile : epg * (sg.a_stride + e.nk * btile);
-      if (need > (m2 ? kMaxDynSmem / 2 : max_stage)) throw std::runtime_error("mdb: pipeline group exceeds the stage size");
-      if (need > stage_need) stage_need = need;
-      p.segs[p.n_segs++] = sg;
-      p.total_groups += n_groups;
-    };
     p.total_groups = 0;
     size_t i = 0;
     while (i < loads.size()) {
       size_t j = i;
       while (j < loads.size() && loads[j].nk == loads[i].nk && loads[j].rows == loads[i].rows && loads[j].jrows == loads[i].jrows) ++j;
-      const int run = (int)(j - i);
-      if (x3pair) {
-        if (run % 2 != 0) throw std::runtime_error("mdb: X3 stage couples need an even run of entries");
-        push(run, 1, loads[i], 1);
-      } else if (m2) {
-        push(run, 1, loads[i], 0);  // one entry per group: its box for both sub-tiles + the shared weight tiles
-      } else if (loads[i].nk == 1 && 2 * (loads[i].rows * kRowBytes + btile) <= max_stage) {
-        push(run / 2, 2, loads[i], 0);
-        push(run % 2, 1, loads[i], 0);
-      } else {
-        push(run, 1, loads[i], 0);
-      }
+      if (p.n_segs >= kMaxSegs) throw std::runtime_error("mdb: too many pipeline segments");
+      GemmSeg sg{};
+      sg.n_groups = (int)(j - i); sg.nk = loads[i].nk;
+      sg.a_bytes = loads[i].rows * kRowBytes;
+      sg.a_stride = (sg.a_bytes + 1023) / 1024 * 1024;
+      sg.jbytes = loads[i].jrows * kRowBytes;
+      const int need = sg.a_stride + sg.nk * btile;
+      if (need > max_stage) throw std::runtime_error("mdb: pipeline group exceeds the stage size");
+      if (need > stage_need) stage_need = need;
+      p.segs[p.n_segs++] = sg;
+      p.total_groups += sg.n_groups;
       i = j;
     }
   }
@@ -538,31 +489,18 @@ void GemmOp::finalize(cudaStream_t stream, bool pack) {
   MDB_CUDA_CHECK(cudaStreamSynchronize(stream));
 }
 
-template <int BN, bool TF32, bool CG2, bool GNB = false, bool X3 = false, bool M2 = false>
+template <int BN, bool TF32, bool GNB = false, bool X3 = false>
 static void launch_impl(const GemmParams& p, int grid, cudaStream_t stream) {
   static bool configured[64] = {};  // the attribute is per device
-  auto kern = gemm_tc_kernel<BN, TF32, CG2, GNB, X3, M2>;
-  const int smem = GemmCfg<BN, CG2>::kFixedBytes + p.n_stages * p.stage_bytes;
+  auto kern = gemm_tc_kernel<BN, TF32, GNB, X3>;
+  const int smem = GemmCfg<BN>::kFixedBytes + p.n_stages * p.stage_bytes;
   int dev = 0;
   MDB_CUDA_CHECK(cudaGetDevice(&dev));
   if (dev >= 64 || !configured[dev]) {
     MDB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
     if (dev < 64) configured[dev] = true;
   }
-  if (CG2) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    MDB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, p));
-  } else {
-    kern<<<grid, kGemmThreads, smem, stream>>>(p);
-  }
+  kern<<<grid, kGemmThreads, smem, stream>>>(p);
   MDB_CUDA_CHECK(cudaGetLastError());
 }
 
@@ -570,11 +508,9 @@ void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
   GemmParams p = this->p;
   {
     // operand ring of this op: stage = its largest pipeline group, as many stages as the 227 KB allow
-    const int fixed = 1024 + 24 * block_n * 4 + (2 * kMaxStages + 4) * 8 + 16;  // GemmCfg<block_n, *>::kFixedBytes
+    const int fixed = block_n == 32 ? GemmCfg<32>::kFixedBytes : GemmCfg<128>::kFixedBytes;
     p.stage_bytes = (stage_need + 1023) / 1024 * 1024;
     int ns = (kMaxDynSmem - fixed) / p.stage_bytes;
-    // measured (profiles/r02_bench_stages_4_vs_5.txt): a fifth 42 KB stage fits for the halo convolutions but is 1-2 %
-    // SLOWER in all three operand modes than four -- the feed is bounded by L2 -> SMEM bytes per MMA, not by bytes in flight
     int cap = 4;
     if (const char* e = getenv("MDB_MAX_STAGES")) { const int c = atoi(e); if (c >= 2) cap = c; }
     if (ns > cap) ns = cap;
@@ -589,42 +525,23 @@ void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
   if (out_override) p.out = out_override;
   const int tiles_m = p.tx * p.ty * p.tz * p.tb;
   const bool tf = prec == kTF32;
+  const int total = tiles_m * p.n_tiles_n * (p.splits > 1 ? p.splits : 1);
+  const int grid = total < sm_count() ? total : sm_count();
   if (gnb) {
     if (tf || p.splits > 1) throw std::runtime_error("mdb: GroupNorm-backward epilogue: bf16, no split-K");
     p.gnb_drop_thresh = rt_drop_thresh; p.gnb_drop_scale = rt_drop_scale; p.gnb_seed = rt_seed;
-    if (pair) {
-      const int work = (m2 ? (tiles_m + 3) / 4 : (tiles_m + 1) / 2) * p.n_tiles_n;
-      const int pairs = sm_count() / 2;
-      if (m2) launch_impl<128, false, true, true, false, true>(p, 2 * (work < pairs ? work : pairs), stream);
-      else launch_impl<128, false, true, true>(p, 2 * (work < pairs ? work : pairs), stream);
-    } else {
-      const int total = tiles_m * p.n_tiles_n;
-      const int grid = total < sm_count() ? total : sm_count();
-      if (block_n == 32) launch_impl<32, false, false, true>(p, grid, stream); else launch_impl<128, false, false, true>(p, grid, stream);
-    }
+    if (block_n == 32) launch_impl<32, false, true>(p, grid, stream); else launch_impl<128, false, true>(p, grid, stream);
     return;
   }
   const bool x3 = prec == kBF16X3;
-  if (pair) {
-    const int work = (m2 ? (tiles_m + 3) / 4 : (tiles_m + 1) / 2) * p.n_tiles_n;
-    const int pairs = sm_count() / 2;
-    const int grid = 2 * (work < pairs ? work : pairs);
-    if (m2) { if (tf) launch_impl<128, true, true, false, false, true>(p, grid, stream); else launch_impl<128, false, true, false, false, true>(p, grid, stream); }
-    else if (tf) launch_impl<128, true, true>(p, grid, stream);
-    else if (x3) launch_impl<128, false, true, false, true>(p, grid, stream);
-    else launch_impl<128, false, true>(p, grid, stream);
-    return;
-  }
-  const int total = tiles_m * p.n_tiles_n * (p.splits > 1 ? p.splits : 1);
-  int grid = total < sm_count() ? total : sm_count();
   if (block_n == 32) {
-    if (tf) launch_impl<32, true, false>(p, grid, stream);
-    else if (x3) launch_impl<32, false, false, false, true>(p, grid, stream);
-    else launch_impl<32, false, false>(p, grid, stream);
+    if (tf) launch_impl<32, true>(p, grid, stream);
+    else if (x3) launch_impl<32, false, false, true>(p, grid, stream);
+    else launch_impl<32, false>(p, grid, stream);
   } else {
-    if (tf) launch_impl<128, true, false>(p, grid, stream);
-    else if (x3) launch_impl<128, false, false, false, true>(p, grid, stream);
-    else launch_impl<128, false, false>(p, grid, stream);
+    if (tf) launch_impl<128, true>(p, grid, stream);
+    else if (x3) launch_impl<128, false, false, true>(p, grid, stream);
+    else launch_impl<128, false>(p, grid, stream);
   }
   if (p.splits > 1) {
     SplitReduceArgs a{};

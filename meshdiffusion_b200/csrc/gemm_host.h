@@ -1,4 +1,4 @@
-// Host-side construction of tcgen05 implicit-GEMM operations: TMA tensor maps, load tables, packed weights.
+// Host-side construction of wgmma implicit-GEMM operations: TMA tensor maps, load tables, packed weights.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -19,7 +19,7 @@ namespace mdb {
   } while (0)
 
 // kBF16X3 ("split bf16"): every fp32 value v is carried as a bf16 pair hi = bf16(v), lo = bf16(v - hi) and every product
-// is evaluated as hi*hi + hi*lo + lo*hi into the same fp32 TMEM accumulator (three kind::f16 MMAs per k-step; the
+// is evaluated as hi*hi + hi*lo + lo*hi into the same fp32 accumulator (three bf16 MMAs per k-step; the
 // dropped lo*lo term is 2^-16 relative) -- fp32-class results (the mode that meets the 1e-3 parity contract) at
 // one third of the bf16 tensor rate. An X3 tensor with a logical row pitch of `ld` channels occupies 2*ld bf16 per
 // voxel: hi parts at [0, ld), lo parts at [ld, 2*ld). All pitches handed to GemmOp / Act stay LOGICAL.
@@ -63,8 +63,6 @@ class GemmOp {
   GemmParams p{};
   Precision prec = kBF16;
   int block_n = 128;
-  bool pair = false;  // CTA-pair kernel (cta_group::2)
-  bool m2 = false;    // pair kernel with two M-tiles per CTA sharing the staged weight tiles (decided by finalize)
   int splits = 1;     // split-K factor (small problems: few tiles, long K)
   std::vector<LoadEntry> loads;
   std::vector<WSrc> wsrcs;
@@ -155,6 +153,9 @@ class GemmOp {
 };
 
 int sm_count();
+// SMs the split-K plans and grid caps are sized for (the H100 SXM's 132). A constant (not the device query) so that the
+// GPU-less sizing pass and the real pass agree on every scratch size.
+constexpr int kPlanSMs = 132;
 void encode_map(CUtensorMap* m, Precision prec, int rank, void* base, const uint64_t* dims,
                 const uint64_t* strides_bytes /*rank-1*/, const uint32_t* box);
 // Split-K factor for a conv-like op (pure function of the shapes, so the dry planning pass and the real pass agree).

@@ -343,7 +343,7 @@ __global__ void __launch_bounds__(256) mt_grad_kernel(const int2* __restrict__ e
   if (gsdf) gsdf[(size_t)b * Nv + v] = gs;
 }
 
-static int grid1d(int n) { int g = (n + 255) / 256; return g > 148 * 4 ? 148 * 4 : (g < 1 ? 1 : g); }
+static int grid1d(int n) { int g = (n + 255) / 256; return g > 132 * 4 ? 132 * 4 : (g < 1 ? 1 : g); }
 
 }  // namespace mdbmt
 

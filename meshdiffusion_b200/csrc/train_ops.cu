@@ -215,7 +215,7 @@ int mdb_ddpm_loss(const float* pred, const float* noise, const float* mask, doub
   const double coef = 1.0 / ((double)B * C * V) * ((double)V / mask_sum);
   TR_CHECK(cudaMemsetAsync(scratch, 0, sizeof(double), s));
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   ddpm_loss_kernel<<<(unsigned)blocks, 256, 0, s>>>(pred, noise, mask, coef, scratch, grad_pred, V, total);
   store_scalar_kernel<<<1, 1, 0, s>>>(scratch, loss_out);
   TR_CHECK(cudaGetLastError());
@@ -227,7 +227,7 @@ int mdb_ddpm_perturb(const float* x0, const float* noise, const float* mask, con
   TR_API_BEGIN
   const long long total = (long long)B * C * V;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   ddpm_perturb_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x0, noise, mask, sqrt_ac, sqrt_1mac, out, V, (long long)C * V, total);
   TR_CHECK(cudaGetLastError());
   TR_API_END
@@ -301,7 +301,7 @@ int mdb_allreduce_grads(void* nccl_comm, float* grads, long long numel, int worl
   const int rc = fn(grads, grads, (size_t)numel, ncclFloat32, ncclSum, nccl_comm, (cudaStream_t)stream);
   if (rc != 0) throw std::runtime_error("mdb: ncclAllReduce failed with code " + std::to_string(rc));
   if (world_size > 1) {
-    scale_kernel<<<148 * 8, 256, 0, (cudaStream_t)stream>>>(grads, 1.f / (float)world_size, numel);
+    scale_kernel<<<132 * 8, 256, 0, (cudaStream_t)stream>>>(grads, 1.f / (float)world_size, numel);
     TR_CHECK(cudaGetLastError());
   }
   TR_API_END

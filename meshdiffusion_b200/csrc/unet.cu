@@ -167,7 +167,7 @@ TensP UNet::gn(const std::string& pname, const std::vector<TensP>& ins, bool sil
   return y;
 }
 
-// ResnetBlockDDPM (layers.py:646-689). The NIN shortcut (when in_ch != out_ch) is accumulated into Conv_1's TMEM
+// ResnetBlockDDPM (layers.py:646-689). The NIN shortcut (when in_ch != out_ch) is accumulated into Conv_1's
 // accumulator as extra k-steps over the raw inputs, so the shortcut add is free.
 TensP UNet::resblock(const std::vector<TensP>& ins, int out_ch, int midx) {
   const std::string pre = "all_modules." + std::to_string(midx) + ".";

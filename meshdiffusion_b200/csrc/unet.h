@@ -1,5 +1,5 @@
 // Score-network engine: builds the DDPM 3-D U-Net (reference lib/diffusion/models/ddpm_res64.py:41-199,
-// ddpm_res128.py:43-215, layers.py:573-689) as a static plan of tcgen05 GEMM ops + bandwidth kernels over a
+// ddpm_res128.py:43-215, layers.py:573-689) as a static plan of wgmma GEMM ops + bandwidth kernels over a
 // liveness-packed HBM arena, and replays it per denoising step.
 #pragma once
 #include <functional>
@@ -27,7 +27,7 @@ struct UNetConfig {
   int stem_ksize = 3;   // 3 (res64) or 5 (res128)
   int use_pos_bias = 1; // ddpm_res64.py:148 adds pos_layer(coords*0) == its bias; res128 does not
   int max_batch = 1;
-  int precision = 0;    // 0 = bf16 operands, 1 = tf32 operands (fp32 accumulate in TMEM either way)
+  int precision = 0;    // 0 = bf16 operands, 1 = tf32 operands (fp32 accumulate either way)
   int training = 0;     // 1: keep the activations backward needs and build the backward plan (bf16 only)
 };
 

@@ -1,6 +1,6 @@
 // Backward plan of the score network: what torch autograd executes for the reference's `loss.backward()`
 // (lib/diffusion/losses.py:104-139) over DDPMRes64/128 (ddpm_res64.py:126-199, layers.py:573-689), emitted as a static
-// list of tcgen05 data-gradient GEMMs (gemm_tc.cuh), tcgen05 weight-gradient contractions (wgrad_tc.cuh) and
+// list of wgmma data-gradient GEMMs (gemm_tc.cuh), wgmma weight-gradient contractions (wgrad_tc.cuh) and
 // bandwidth kernels (backward.cu). Every forward builder records an emitter on a tape; build() runs the tape in
 // reverse, so tensor lifetimes of the whole forward+backward step are packed into one arena by the same first-fit
 // planner as the inference engine.
@@ -241,7 +241,7 @@ GradView UNet::emit_conv_dgrad(const std::string& name, const GradView& dy, int 
   return dx;
 }
 
-// [N] = sum_i srcs[i] . ws[i]  (1x1x1 products accumulated in one TMEM accumulator) (+ addend)
+// [N] = sum_i srcs[i] . ws[i]  (1x1x1 products accumulated in one accumulator) (+ addend)
 GradView UNet::emit_pointwise(const std::string& name, const std::vector<Act>& srcs, const std::vector<WSrc>& ws, int N, int R,
                               const GradView* addend, GnFuse* fuse) {
   GradView dx = new_grad(N, R);

@@ -1,4 +1,4 @@
-// Host-side builders for the tcgen05 weight-gradient kernel (see wgrad_tc.cuh) and its split-K reduction.
+// Host-side builders for the wgmma weight-gradient kernel (see wgrad_tc.cuh) and its split-K reduction.
 #define MDB_WGRAD_KERNEL_IMPL
 #include "wgrad_host.h"
 #include <cstdlib>
@@ -16,9 +16,7 @@ WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int st
     tiles = ((long long)B * X * Y * Z + 127) / 128;
   } else {
     pl.geo = pick_geometry(X, Y, Z);
-    pl.halo = stride == 1 && pl.geo.bz == 1 && pl.geo.bb == 1 && pl.geo.bx % 8 == 0 &&
-              pl.geo.bx * (pl.geo.by + 2) <= kWgXRowsMax && Y >= pl.geo.by;
-    pl.n_groups = pl.halo ? 9 : 27;
+    pl.n_groups = 27;
     pl.taps = 27;
     tiles = 1LL * ((X + pl.geo.bx - 1) / pl.geo.bx) * ((Y + pl.geo.by - 1) / pl.geo.by) * ((Z + pl.geo.bz - 1) / pl.geo.bz) *
             ((B + pl.geo.bb - 1) / pl.geo.bb);
@@ -47,28 +45,17 @@ void WgradOp::init(const Act& dy, const Act& x, int ksize, int stride, const Wgr
   p.taps = plan_.taps;
   p.Mp = plan_.m_tiles * 128; p.Np = plan_.n_tiles * 128;
   p.partial = scratch;
-  { const char* f = getenv("MDB_WG_DBG"); p.dbg = f ? atoi(f) : 0; }
   p.n_groups = plan_.n_groups;
-  const int xrows = plan_.halo ? p.bx * (p.by + 2) : 128;
-  p.x_chunk_bytes = xrows * kRowBytes;
-  p.tap_shift16 = plan_.halo ? (p.bx * kRowBytes) >> 4 : 0;
   int g = 0;
   if (plan_.flat) {
-    p.groups[g++] = WgradGroup{0, 0, 0, 0, 1, {0, 0, 0}};
-  } else if (plan_.halo) {
-    for (int kz = 0; kz < 3; ++kz)
-      for (int kx = 0; kx < 3; ++kx) {
-        WgradGroup gr{0, (int8_t)(kx - 1), -1, (int8_t)(kz - 1), 3, {0, 0, 0}};
-        for (int ky = 0; ky < 3; ++ky) gr.tap[ky] = (int8_t)((kz * 3 + ky) * 3 + kx);
-        p.groups[g++] = gr;
-      }
+    p.groups[g++] = WgradGroup{0, 0, 0, 0, 0, {0, 0, 0}};
   } else {
     for (int kz = 0; kz < 3; ++kz)
       for (int ky = 0; ky < 3; ++ky)
         for (int kx = 0; kx < 3; ++kx) {
           const int8_t tap = (int8_t)((kz * 3 + ky) * 3 + kx);
-          if (stride == 1) p.groups[g++] = WgradGroup{0, (int8_t)(kx - 1), (int8_t)(ky - 1), (int8_t)(kz - 1), 1, {tap, 0, 0}};
-          else p.groups[g++] = WgradGroup{(int8_t)((kx & 1) | ((ky & 1) << 1) | ((kz & 1) << 2)), (int8_t)(kx >> 1), (int8_t)(ky >> 1), (int8_t)(kz >> 1), 1, {tap, 0, 0}};
+          if (stride == 1) p.groups[g++] = WgradGroup{0, (int8_t)(kx - 1), (int8_t)(ky - 1), (int8_t)(kz - 1), tap, {0, 0, 0}};
+          else p.groups[g++] = WgradGroup{(int8_t)((kx & 1) | ((ky & 1) << 1) | ((kz & 1) << 2)), (int8_t)(kx >> 1), (int8_t)(ky >> 1), (int8_t)(kz >> 1), tap, {0, 0, 0}};
         }
   }
   flops = 2.0 * dy.voxels() * dy.B * (double)M_ * N_ * plan_.taps;
@@ -95,7 +82,7 @@ const WgradParams& WgradOp::params_for(int B) {
   } else {
     p.tx = (dy_.X + p.bx - 1) / p.bx; p.ty = (dy_.Y + p.by - 1) / p.by; p.tz = (dy_.Z + p.bz - 1) / p.bz;
     p.tb = (B + p.bb - 1) / p.bb;
-    auto enc = [&](CUtensorMap* m, const Act& a, int halo, int sub, int px, int py, int pz) {
+    auto enc = [&](CUtensorMap* m, const Act& a, int sub, int px, int py, int pz) {
       char* base = static_cast<char*>(a.ptr);
       const long long sx = a.row() * es, sy = sx * a.X, sz = sy * a.Y, sb = sz * a.Z;
       dims[0] = a.C; dims[4] = B;
@@ -107,14 +94,14 @@ const WgradParams& WgradOp::params_for(int B) {
         strides[0] = sx * sub; strides[1] = sy * sub; strides[2] = sz * sub; strides[3] = sb;
         base += px * sx + py * sy + pz * sz;
       }
-      box[0] = 64; box[1] = p.bx; box[2] = p.by + halo; box[3] = p.bz; box[4] = p.bb;
+      box[0] = 64; box[1] = p.bx; box[2] = p.by; box[3] = p.bz; box[4] = p.bb;
       encode_map(m, kBF16, 5, base, dims, strides, box);
     };
-    enc(&p.ymap, dy_, 0, 1, 0, 0, 0);
+    enc(&p.ymap, dy_, 1, 0, 0, 0);
     if (stride_ == 1) {
-      enc(&p.xmap[0], x_, plan_.halo ? 2 : 0, 1, 0, 0, 0);
+      enc(&p.xmap[0], x_, 1, 0, 0, 0);
     } else {
-      for (int par = 0; par < 8; ++par) enc(&p.xmap[par], x_, 0, 2, par & 1, (par >> 1) & 1, (par >> 2) & 1);
+      for (int par = 0; par < 8; ++par) enc(&p.xmap[par], x_, 2, par & 1, (par >> 1) & 1, (par >> 2) & 1);
     }
   }
   const long long tiles = 1LL * p.tx * p.ty * p.tz * p.tb;
@@ -149,7 +136,7 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(WgradReduceArgs a) {
 void launch_wgrad_reduce(const WgradReduceArgs& a, cudaStream_t s) {
   const long long total = (long long)a.M * a.N * a.taps;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kPlanSMs * 16) blocks = kPlanSMs * 16;
   wgrad_reduce_kernel<<<(unsigned)blocks, 256, 0, s>>>(a);
   MDB_CUDA_CHECK(cudaGetLastError());
 }

@@ -1,4 +1,4 @@
-// Host-side construction of tcgen05 weight-gradient operations (see wgrad_tc.cuh).
+// Host-side construction of wgmma weight-gradient operations (see wgrad_tc.cuh).
 #pragma once
 #include <map>
 #include "gemm_host.h"
@@ -15,13 +15,9 @@ struct WgradOut {
   int m_valid = 0, n_valid = 0;  // rows / columns actually written (0 = all channels of the operands)
 };
 
-// SMs the split-K plan is sized for. A constant (not the device query) so that the GPU-less sizing pass and the real
-// pass agree on every scratch size.
-constexpr int kPlanSMs = 148;
-
 struct WgradPlan {
   int m_tiles = 0, n_tiles = 0, n_groups = 0, taps = 0, max_splits = 1;
-  bool halo = false, flat = false;
+  bool flat = false;
   Geometry geo{};
   size_t scratch_bytes = 0;
 };

@@ -1,37 +1,36 @@
-// tcgen05 weight-gradient kernel for sm_100a (training path: the dW half of nn.Conv3d / NIN / Linear backward,
+// wgmma weight-gradient kernel for sm_90a (training path: the dW half of nn.Conv3d / NIN / Linear backward,
 // i.e. what autograd computes for the reference's `loss.backward()` in lib/diffusion/losses.py:104-139).
 //
 //   G[tap][m][n] = sum over positions p of  dY[p][m] * X[p + off(tap)][n]
 //
 // Both operands are NDHWC activations, so the contraction index (the voxel) is the SLOW axis of both tiles: the tiles
-// are fed to the tensor cores as MN-major operands (UMMA descriptors with the 64-channel chunk stride in LBO and the
-// 8-voxel group stride in SBO; a_major = b_major = 1 in the instruction descriptor) -- no transposed copy of any
-// activation exists. A CTA owns ONE (Cout tile, Cin tile, tap group) and a contiguous range of voxel tiles; its up to
-// three 128x128 fp32 accumulators (the ky = -1,0,+1 taps of one (kz,kx) column, served by ONE halo load of X) stay in
-// TMEM for the whole range and are written once, as a split-K partial, at the end. Partials are summed in a fixed
-// order by wgrad_reduce_kernel (deterministic gradients), which also scatters into the reference's OIDHW layout.
+// are fed to the tensor cores as MN-major operands (wgmma descriptors with the 64-channel block stride in LBO and the
+// 8-voxel group stride in SBO, transpose flags set) -- no transposed copy of any activation exists. A CTA owns ONE
+// (Cout tile, Cin tile, tap) and a contiguous range of voxel tiles; its 128x128 fp32 accumulator stays in registers for
+// the whole range -- each consumer warpgroup holds 64 of the 128 rows -- and is written once, as a split-K partial, at the
+// end. (One tap per CTA: three taps sharing a halo load of X would need 192 accumulator registers per thread, more than a
+// thread can hold next to its addressing.) Partials are summed in a fixed order by wgrad_reduce_kernel (deterministic
+// gradients), which also scatters into the reference's OIDHW layout.
 //
-// Warp roles (256 threads): w0 = TMA producer, w1 = MMA issuer, w2 = TMEM allocator, w4..7 = final drain.
+// Warp roles (384 threads): warpgroup 0 = TMA producer (warp 0), warpgroups 1-2 = MMA + drain.
 #pragma once
 #include "gemm_tc.cuh"
 
 namespace mdb {
 
-constexpr int kWgThreads = 256;
+constexpr int kWgThreads = 384;
 constexpr int kWgStages = 3;
 constexpr int kWgYChunkBytes = 128 * kRowBytes;           // 64 channels x 128 voxels
-constexpr int kWgXRowsMax = 144;                          // 8 x (16 + 2 halo rows)
-constexpr int kWgXChunkBytesMax = kWgXRowsMax * kRowBytes;  // 18432
-constexpr int kWgStageBytes = 2 * kWgYChunkBytes + 2 * kWgXChunkBytesMax;  // 69632
-constexpr int kWgSmemBytes = 1024 + kWgStages * kWgStageBytes + (2 * kWgStages + 1) * 8 + 16;
+constexpr int kWgStageBytes = 4 * kWgYChunkBytes;         // dY and X: two 64-channel chunks each
+constexpr int kWgSmemBytes = 1024 + kWgStages * kWgStageBytes + 2 * kWgStages * 8;
 constexpr int kWgMaxGroups = 27;
 constexpr int kWgMaxXMaps = 8;
 
 struct WgradGroup {
   int8_t xmap;        // which X tensor map (stride-2 convs: the parity sub-grid of this tap)
   int8_t dx, dy, dz;  // coordinate offset of the X box relative to the dY tile origin
-  int8_t ntaps;       // 1, or 3 (halo reuse along y)
-  int8_t tap[3];      // output tap index of each accumulator
+  int8_t tap;         // output tap index
+  int8_t pad[3];
 };
 static_assert(sizeof(WgradGroup) == 8, "WgradGroup must be 8 bytes");
 
@@ -44,37 +43,20 @@ struct WgradParams {
   int tx, ty, tz, tb;   // voxel tile counts
   int m_tiles, n_tiles;
   int splits;           // CTAs sharing one (m tile, n tile, group): contiguous ranges of voxel tiles
-  int x_chunk_bytes;    // one 64-channel X box
-  int tap_shift16;      // smem advance (bytes >> 4) between the taps of a group
   int taps;             // taps of the whole operation (partial layout)
   int Mp, Np;           // padded extents (multiples of 128)
   float* partial;       // [splits][taps][Mp][Np]
-  int dbg;              // bring-up switch (MDB_WG_DBG): bit 0 swaps the roles of LBO and SBO in the operand descriptors
 };
 
 #ifdef MDB_WGRAD_KERNEL_IMPL  // the kernel itself is compiled in wgrad_host.cu only
-__device__ __forceinline__ uint32_t desc_lo_lbo(uint32_t saddr, uint32_t lbo_bytes) {
-  return ((saddr & 0x3FFFFu) >> 4) | ((lbo_bytes >> 4) << 16);
-}
-
-// explicit-descriptor MMA (bring-up path only)
-__device__ __forceinline__ void umma_full(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "mov.b64 da, {%1, %5};\n\tmov.b64 db, {%2, %6};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t}"
-      :: "r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(a_hi), "r"(b_hi) : "memory");
-}
-
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ WgradParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWgStages * kWgStageBytes);
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + 2 * kWgStages + 1);
   const uint32_t stage0 = smem_u32(smem);
-  const uint32_t full = smem_u32(bars), empty = full + 8 * kWgStages, done = empty + 8 * kWgStages;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t full = smem_u32(bars), empty = full + 8 * kWgStages;
+  // (broadcast from lane 0, so the compiler can treat the warpgroup branches as warp-uniform)
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
 
   // work item of this CTA
   int w = blockIdx.x;
@@ -93,104 +75,77 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     tma_prefetch_desc(&p.xmap[grp.xmap]);
   }
   if (warp == 1 && lane == 0) {
-    for (int i = 0; i < kWgStages; ++i) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 1); }
-    mbar_init(done, 1);
+    for (int i = 0; i < kWgStages; ++i) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 2); }
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 2) tmem_alloc<512>(smem_u32(s_tmem));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  if (*s_tmem != 0) {
-    if (threadIdx.x == 0) printf("mdb: unexpected TMEM base %u\n", *s_tmem);
-    __trap();
-  }
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    uint32_t st = 0, ph = 0;
-    const uint32_t bytes = 2 * kWgYChunkBytes + 2 * p.x_chunk_bytes;
-    for (int t = t_lo; t < t_hi; ++t) {
-      int r = t;
-      const int x0 = (r % p.tx) * p.bx; r /= p.tx;
-      const int y0 = (r % p.ty) * p.by; r /= p.ty;
-      const int z0 = (r % p.tz) * p.bz; r /= p.tz;
-      const int b0 = r * p.bb;
-      mbar_wait(empty + 8 * st, ph ^ 1);
-      if (elect_one()) {
-        const uint32_t bar = full + 8 * st;
-        const uint32_t sbase = stage0 + st * kWgStageBytes;
-        mbar_expect_tx(bar, bytes);
-        tma_load_5d(&p.ymap, bar, sbase, m0, x0, y0, z0, b0);
-        tma_load_5d(&p.ymap, bar, sbase + kWgYChunkBytes, m0 + 64, x0, y0, z0, b0);
-        const uint32_t xb = sbase + 2 * kWgYChunkBytes;
-        tma_load_5d(&p.xmap[grp.xmap], bar, xb, n0, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
-        tma_load_5d(&p.xmap[grp.xmap], bar, xb + p.x_chunk_bytes, n0 + 64, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
+  if (warp < 4) {
+    setmaxnreg_dec<kRegsProducer>();
+    if (warp == 0) {
+      // ------------------------------------------------------------------ TMA producer
+      uint32_t st = 0, ph = 0;
+      const uint32_t bytes = kWgStageBytes;
+      for (int t = t_lo; t < t_hi; ++t) {
+        int r = t;
+        const int x0 = (r % p.tx) * p.bx; r /= p.tx;
+        const int y0 = (r % p.ty) * p.by; r /= p.ty;
+        const int z0 = (r % p.tz) * p.bz; r /= p.tz;
+        const int b0 = r * p.bb;
+        mbar_wait(empty + 8 * st, ph ^ 1);
+        if (elect_one()) {
+          const uint32_t bar = full + 8 * st;
+          const uint32_t sbase = stage0 + st * kWgStageBytes;
+          mbar_expect_tx(bar, bytes);
+          tma_load_5d(&p.ymap, bar, sbase, m0, x0, y0, z0, b0);
+          tma_load_5d(&p.ymap, bar, sbase + kWgYChunkBytes, m0 + 64, x0, y0, z0, b0);
+          const uint32_t xb = sbase + 2 * kWgYChunkBytes;
+          tma_load_5d(&p.xmap[grp.xmap], bar, xb, n0, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
+          tma_load_5d(&p.xmap[grp.xmap], bar, xb + kWgYChunkBytes, n0 + 64, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
+        }
+        __syncwarp();
+        if (++st == kWgStages) { st = 0; ph ^= 1; }
       }
-      __syncwarp();
-      if (++st == kWgStages) { st = 0; ph ^= 1; }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = make_idesc(false, 128, 128) | (1u << 15) | (1u << 16);  // A and B MN-major
+  } else {
+    setmaxnreg_inc<kRegsConsumer>();
+    // ------------------------------------------------------------------ MMA: warpgroup wg owns rows [64*wg, 64*wg + 64)
+    const int wg = (warp - 4) >> 2, wt = threadIdx.x & 127;
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     uint32_t st = 0, ph = 0;
+    int prev = -1;
     for (int t = t_lo; t < t_hi; ++t) {
       mbar_wait(full + 8 * st, ph);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sbase = stage0 + st * kWgStageBytes;
-        const uint32_t a0 = desc_lo_lbo(sbase, kWgYChunkBytes);
-        const uint32_t b0 = desc_lo_lbo(sbase + 2 * kWgYChunkBytes, p.x_chunk_bytes);
-        const uint32_t first = t != t_lo ? 1u : 0u;
-        if (p.dbg & 1) {
-          const uint32_t hi_common = (1u << 14) | (2u << 29);
-          const uint32_t a_sw = desc_lo_lbo(sbase, 1024), b_sw = desc_lo_lbo(sbase + 2 * kWgYChunkBytes, 1024);
-          for (int j = 0; j < grp.ntaps; ++j)
-            for (int c = 0; c < 8; ++c)
-              umma_full(j * 128, a_sw + c * 128, hi_common | (kWgYChunkBytes >> 4), b_sw + j * p.tap_shift16 + c * 128,
-                        hi_common | (p.x_chunk_bytes >> 4), idesc, c > 0 ? 1u : first);
-        } else {
-          for (int j = 0; j < grp.ntaps; ++j) {
-            const uint32_t bj = b0 + j * p.tap_shift16;
+      const uint32_t sbase = stage0 + st * kWgStageBytes;
+      // A = this warpgroup's 64-channel dY block (one MN block); B = both 64-channel X blocks, LBO apart
+      const uint64_t a0 = make_wgmma_desc(sbase + wg * kWgYChunkBytes, kWgYChunkBytes, 1024);
+      const uint64_t b0 = make_wgmma_desc(sbase + 2 * kWgYChunkBytes, kWgYChunkBytes, 1024);
+      fence_operands(acc);
+      wgmma_fence();
 #pragma unroll
-            for (int c = 0; c < 8; ++c)  // 16 voxels (two 8-row swizzle atoms = 2048 B) per instruction
-              umma_lo<false>(j * 128, a0 + c * 128, bj + c * 128, idesc, c > 0 ? 1u : first);
-          }
-        }
-        umma_commit(empty + 8 * st);
-      }
-      __syncwarp();
+      for (int c = 0; c < 8; ++c)  // 16 voxels (two 8-row swizzle groups = 2048 B) per instruction
+        wgmma_m64n128k16_bf16<1, 1>(acc, a0 + c * 128, b0 + c * 128, 1u);
+      wgmma_commit();
+      fence_operands(acc);
+      wgmma_wait<1>();
+      if (prev >= 0 && wt == 0) mbar_arrive(empty + 8 * prev);
+      prev = (int)st;
       if (++st == kWgStages) { st = 0; ph ^= 1; }
     }
-    if (elect_one()) umma_commit(done);
-    __syncwarp();
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ drain: TMEM -> fp32 partial
-    mbar_wait(done, 0);
-    tc_fence_after();
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    for (int j = 0; j < grp.ntaps; ++j) {
-      float* dst = p.partial + (((long long)split * p.taps + grp.tap[j]) * p.Mp + m0 + row) * p.Np + n0;
-#pragma unroll 1
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t rr[32];
-        tmem_ld32((static_cast<uint32_t>(q * 32) << 16) + j * 128 + ch * 32, rr);
-        tmem_ld_wait();
+    wgmma_wait<0>();
+    fence_operands(acc);
+    // ------------------------------------------------------------------ drain: registers -> fp32 partial
+    // register 4i+{0,1} = (row l/4, cols 8i + 2(l%4) + {0,1}), 4i+{2,3} = the same columns 8 rows further down
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2), col = 2 * (lane & 3);
+    float* dst = p.partial + (((long long)split * p.taps + grp.tap) * p.Mp + m0 + row) * p.Np + n0 + col;
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
-          reinterpret_cast<float4*>(dst + ch * 32)[i] = make_float4(__uint_as_float(rr[4 * i]), __uint_as_float(rr[4 * i + 1]),
-                                                                     __uint_as_float(rr[4 * i + 2]), __uint_as_float(rr[4 * i + 3]));
-      }
+    for (int i = 0; i < 16; ++i) {
+      *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(acc[4 * i], acc[4 * i + 1]);
+      *reinterpret_cast<float2*>(dst + 8 * p.Np + 8 * i) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<512>(0);
   }
 }
 

@@ -8,7 +8,7 @@
 * `step_fn(state, batch, clear_grad, update_param)`: gradients of successive micro-batches add up (no division),
   `state['step']` and the EMA advance on EVERY micro-step, evaluation runs under the EMA weights.
 
-The network forward and backward run inside the sm_100a engine; `loss.backward()` reaches it through one autograd node
+The network forward and backward run inside the sm_90a engine; `loss.backward()` reaches it through one autograd node
 (models/ddpm.py::_ScoreNetFn). The arithmetic around it runs in the library's optimiser-side kernels (train_ops.py):
 the forward perturbation and the masked l2 loss + its gradient (mdb_ddpm_perturb / mdb_ddpm_loss, one autograd node),
 clip_grad_norm_ as a coefficient (mdb_grad_clip_coef) and Adam + the EMA update in ONE pass over the parameters

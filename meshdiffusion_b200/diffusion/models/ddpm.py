@@ -1,10 +1,10 @@
-"""Score networks `ddpm_res64` / `ddpm_res128` backed by the sm_100a engine.
+"""Score networks `ddpm_res64` / `ddpm_res128` backed by the sm_90a engine.
 
 Drop-in for the reference's DDPMRes64 / DDPMRes128 (lib/diffusion/models/ddpm_res64.py:39-199,
 ddpm_res128.py:41-215): same registered names, same `model(x, labels)` call, same parameter names and shapes
 (so reference checkpoints load with `load_state_dict`), same `.mask` / `.coords` / `sigmas` entries. The module
 holds the fp32 master parameters as ordinary torch Parameters; the forward pass runs entirely inside
-libmeshdiff_b200.so (tcgen05 implicit-GEMM convolutions + fused bandwidth kernels). There is no PyTorch or CPU
+libmeshdiff_b200.so (wgmma implicit-GEMM convolutions + fused bandwidth kernels). There is no PyTorch or CPU
 fallback: calling the model without the native library and a CUDA device raises.
 """
 import ctypes
@@ -198,7 +198,7 @@ class ScoreNet(nn.Module):
         if self._handle is not None and batch <= self._engine_batch:
             return
         if device.type != "cuda":
-            raise _native.NativeError("the score network runs only on a CUDA (sm_100a) device; there is no CPU path")
+            raise _native.NativeError("the score network runs only on a CUDA (sm_90a) device; there is no CPU path")
         self.release_engine()
         mb = max(batch, self.max_batch)
         cfg = _config_c(self.arch, mb, self.precision)
@@ -221,7 +221,7 @@ class ScoreNet(nn.Module):
         if self._train_handle is not None and batch <= self._train_batch:
             return
         if device.type != "cuda":
-            raise _native.NativeError("the score network trains only on a CUDA (sm_100a) device; there is no CPU path")
+            raise _native.NativeError("the score network trains only on a CUDA (sm_90a) device; there is no CPU path")
         if self._train_handle is not None:
             L.mdb_unet_destroy(self._train_handle)
             self._train_handle = None
@@ -443,7 +443,7 @@ class ScoreNet(nn.Module):
 
     def forward(self, x, labels):
         if not x.is_cuda:
-            raise _native.NativeError("the score network runs only on a CUDA (sm_100a) device; there is no CPU path")
+            raise _native.NativeError("the score network runs only on a CUDA (sm_90a) device; there is no CPU path")
         L = _native.lib()
         x = x.float().contiguous()
         labels = labels.to(device=x.device, dtype=torch.float32).contiguous()

@@ -4,7 +4,7 @@ Host loop with the reference's structure: model / EMA / Adam, auto-resume from `
 grid mask written into `score_model.module.mask`, micro-batching through `training.iter_size`, logging every
 `log_freq`, pre-emption checkpoint every `snapshot_freq_for_preemption`, numbered checkpoints every `snapshot_freq`.
 
-Forward AND backward of the score network run inside the sm_100a engine (bf16 operands, fp32 master weights /
+Forward AND backward of the score network run inside the sm_90a engine (bf16 operands, fp32 master weights /
 gradients / Adam / EMA); `loss.backward()` reaches it through one autograd node (models/ddpm.py); the loss arithmetic,
 clipping, Adam and the EMA run in the library's optimiser-side kernels (train_ops.py). Data parallelism is one process
 per GPU (torchrun), replacing the reference's nn.DataParallel (models/utils.py:95): replicas start from identical

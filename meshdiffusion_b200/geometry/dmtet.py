@@ -1,4 +1,4 @@
-"""Marching tetrahedra on the sm_100a kernels, behind the reference's `DMTet()(pos_nx3, sdf_n, tet_fx4)` call
+"""Marching tetrahedra on the sm_90a kernels, behind the reference's `DMTet()(pos_nx3, sdf_n, tet_fx4)` call
 (nvdiffrec/lib/geometry/dmtet.py:32-163), plus the grid -> tet-vertex gather of nvdiffrec/eval.py:389-419 and the
 vertex placement of dmtet.py:293-304. Integer outputs are int64 and bit-exact with the reference's ordering.
 """

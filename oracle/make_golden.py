@@ -30,6 +30,17 @@ ensure_ml_collections()
 from oracle import unet_oracle, sampler_oracle, mt_oracle, synth  # noqa: E402
 
 
+
+def savez_lzma(path, **arrays):
+    """np.savez_compressed with LZMA instead of deflate (np.load reads both): keeps the larger fixtures under 1 MB."""
+    import io
+    import zipfile
+    with zipfile.ZipFile(path, "w", compression=zipfile.ZIP_LZMA) as zf:
+        for k, v in arrays.items():
+            buf = io.BytesIO()
+            np.lib.format.write_array(buf, np.asanyarray(v), allow_pickle=False)
+            zf.writestr(k + ".npy", buf.getvalue())
+
 def import_reference():
     sys.path.insert(0, REF)
     torch.Tensor.cuda = lambda self, *a, **k: self  # reference hard-codes .cuda() in table construction
@@ -340,7 +351,7 @@ def golden_marching_tets():
         cases[case + "_uvs_head"] = r[2][:64]
         cases[case + "_uvs_tail"] = r[2][-64:]
         cases[case + "_uvs_sum"] = np.array([r[2].astype(np.float64).sum()])
-    np.savez_compressed(os.path.join(GOLD, "marching_tets_64.npz"), **cases)
+    savez_lzma(os.path.join(GOLD, "marching_tets_64.npz"), **cases)
     golden_marching_tets_grad(mt, verts, idx)
     golden_marching_tets_128(mt)
     # grid mask derivable from the tet grid (data/get_tet_mask.py): check against the shipped mask

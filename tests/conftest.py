@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run through gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (H100)")
 
 
 def pytest_collection_modifyitems(config, items):

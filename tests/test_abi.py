@@ -1,4 +1,4 @@
-"""CPU: the shared library builds for sm_100a, loads, and exports every symbol the header declares (no compute)."""
+"""CPU: the shared library builds for sm_90a, loads, and exports every symbol the header declares (no compute)."""
 import ctypes
 import os
 import re
@@ -23,8 +23,9 @@ def test_library_exports_every_declared_symbol():
     assert L.mdb_version() == 100
 
 
-def test_sass_contains_tcgen05_and_tma():
-    """The .so must carry Blackwell tensor-core / TMA SASS (UTC*MMA, UTMALDG, LDTM), i.e. it really is the sm_100a path."""
+def test_sass_contains_wgmma_and_tma():
+    """The .so must carry Hopper warpgroup-MMA / TMA SASS (HGMMA, UTMALDG) and no other architecture, i.e. it really is the
+    sm_90a path."""
     import shutil
     import subprocess
     from meshdiffusion_b200 import _native
@@ -34,8 +35,9 @@ def test_sass_contains_tcgen05_and_tma():
         import pytest
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", _native.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM"):
+    archs = set(re.findall(r"arch = (sm_\w+)", sass))
+    assert archs == {"sm_90a"}, archs
+    for mnemonic in ("HGMMA", "UTMALDG"):
         assert mnemonic in sass, f"{mnemonic} missing from the SASS"
 
 

@@ -1,4 +1,4 @@
-"""Training path parity on the GPU: the tcgen05 weight-gradient kernel, the data-gradient convolutions, GroupNorm
+"""Training path parity on the GPU: the wgmma weight-gradient kernel, the data-gradient convolutions, GroupNorm
 backward and the whole score-network backward, against torch autograd in true fp32 (the reference computes its
 gradients with `loss.backward()`, lib/diffusion/losses.py:104-139).
 

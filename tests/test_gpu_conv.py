@@ -1,7 +1,7 @@
-"""Parity of the tcgen05 implicit-GEMM convolution against torch's fp32 conv3d (TF32 disabled) on the same inputs.
+"""Parity of the wgmma implicit-GEMM convolution against torch's fp32 conv3d (TF32 disabled) on the same inputs.
 
 Tolerances (max |diff| / max |ref|): tf32 operands 2e-3, bf16 operands 2e-2 -- operand rounding only, the
-accumulation is fp32 in TMEM in both modes; split bf16 ("bf16x3": hi*hi + hi*lo + lo*hi, the dropped lo*lo term is
+accumulation is fp32 in registers in both modes; split bf16 ("bf16x3": hi*hi + hi*lo + lo*hi, the dropped lo*lo term is
 2^-16 of a product; the 5^3 head case sums 16 000 products per output) 1e-4.
 """
 import pytest

@@ -1,4 +1,4 @@
-"""Score-network parity: the sm_100a engine vs (a) the committed golden vectors produced by the REFERENCE modules on
+"""Score-network parity: the sm_90a engine vs (a) the committed golden vectors produced by the REFERENCE modules on
 CPU fp32 (oracle/make_golden.py), (b) the oracle evaluated on the GPU in true fp32 at the full res64 size.
 
 Tolerances are on max|diff|/max|ref| and relative L2. Split bf16 operands ("bf16x3", the parity-grade mode): 1e-3, the

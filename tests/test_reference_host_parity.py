@@ -1,7 +1,11 @@
-"""CPU: host-side pieces of the drop-in surface compared with the REFERENCE's own code (baseline/_ref, run in a subprocess so
-its `configs` / `lib` packages never meet this repository's): config trees key by key, registered predictor / corrector /
-model names, the VP-SDE tables and `marginal_prob`, the EMA recursion, the optimiser construction and the warm-up / clip
-arithmetic of `optimization_manager` (lib/diffusion/losses.py:26-52)."""
+"""CPU: host-side pieces of the drop-in surface compared with the REFERENCE's own code: config trees key by key, registered
+predictor / corrector / model names, the VP-SDE tables and `marginal_prob`, the EMA recursion, the optimiser construction and
+the warm-up / clip arithmetic of `optimization_manager` (lib/diffusion/losses.py:26-52).
+
+The reference's answers are stored in tests/golden/reference_host_parity.json.gz. They were produced by REF_SIDE below, run on the
+unmodified reference modules in a subprocess (so its `configs` / `lib` packages never meet this repository's);
+`python tests/test_reference_host_parity.py` regenerates the file where the reference is staged under baseline/_ref."""
+import gzip
 import json
 import os
 import subprocess
@@ -84,19 +88,24 @@ print("REF_DONE")
 '''
 
 
-def _have_reference():
-    return os.path.exists(os.path.join(ROOT, "baseline", "_ref", "lib", "diffusion", "sampling.py"))
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_host_parity.json.gz")
+
+
+def regenerate():
+    import tempfile
+    with tempfile.TemporaryDirectory() as d:
+        out = os.path.join(d, "ref.json")
+        r = subprocess.run([sys.executable, "-c", REF_SIDE, ROOT, out], capture_output=True, text=True, timeout=600,
+                           env=dict(os.environ, OMP_NUM_THREADS="4"))
+        assert r.returncode == 0 and "REF_DONE" in r.stdout, r.stdout + r.stderr
+        with open(out, "rb") as f, gzip.GzipFile(GOLDEN, "wb", mtime=0) as g:
+            g.write(f.read())
 
 
 @pytest.fixture(scope="module")
-def ref(tmp_path_factory):
-    if not _have_reference():
-        pytest.skip("baseline/_ref not staged (python baseline/install_reference.py)")
-    out = str(tmp_path_factory.mktemp("ref") / "ref.json")
-    r = subprocess.run([sys.executable, "-c", REF_SIDE, ROOT, out], capture_output=True, text=True, timeout=600,
-                       env=dict(os.environ, OMP_NUM_THREADS="4"))
-    assert r.returncode == 0 and "REF_DONE" in r.stdout, r.stdout + r.stderr
-    return json.load(open(out))
+def ref():
+    with gzip.open(GOLDEN, "rt") as f:
+        return json.load(f)
 
 
 def _flat(c, pre=""):
@@ -212,3 +221,7 @@ def test_initialisers_match_the_reference_layer_by_layer(ref):
             assert abs(float(v.abs().max()) / r["absmax"] - 1.0) < max(0.05, 20.0 / n), (k, float(v.abs().max()), r["absmax"])
         checked += 1
     assert checked > 30
+
+
+if __name__ == "__main__":
+    regenerate()

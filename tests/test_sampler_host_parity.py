@@ -1,7 +1,9 @@
 """CPU: the host loop of the sampler -- every registered predictor / corrector pair, the partial (`cond_gen`) branch with the
 reference's (B,B,...) initial-broadcast quirk and `freeze_iters`, and `return_traj` -- is BITWISE equal to the REFERENCE's own
-`get_sampling_fn -> pc_sampler` (lib/diffusion/sampling.py:83-132,357-487, run from baseline/_ref in a subprocess) when both
-drive the same stub score model with the same seed. (On a CUDA tensor with the native network the configured
+`get_sampling_fn -> pc_sampler` (lib/diffusion/sampling.py:83-132,357-487) when both drive the same stub score model with the
+same seed. The reference's outputs are stored in tests/golden/sampler_host_parity.pt; REF_SIDE below produced them from the
+unmodified reference modules in a subprocess, and `python tests/test_sampler_host_parity.py` regenerates the file where the
+reference is staged under baseline/_ref. (On a CUDA tensor with the native network the configured
 ancestral + none pair takes the fused path instead; that path is pinned against reference goldens in tests/test_gpu_sampler.py.)"""
 import os
 import subprocess
@@ -71,19 +73,18 @@ print("REF_DONE")
 '''
 
 
-def _have_reference():
-    return os.path.exists(os.path.join(ROOT, "baseline", "_ref", "lib", "diffusion", "sampling.py"))
+GOLDEN = os.path.join(ROOT, "tests", "golden", "sampler_host_parity.pt")
+
+
+def regenerate():
+    r = subprocess.run([sys.executable, "-c", REF_SIDE, ROOT, GOLDEN], capture_output=True, text=True, timeout=900,
+                       env=dict(os.environ, OMP_NUM_THREADS="4"))
+    assert r.returncode == 0 and "REF_DONE" in r.stdout, r.stdout + r.stderr
 
 
 @pytest.fixture(scope="module")
-def ref(tmp_path_factory):
-    if not _have_reference():
-        pytest.skip("baseline/_ref not staged (python baseline/install_reference.py)")
-    out = str(tmp_path_factory.mktemp("ref") / "samplers.pt")
-    r = subprocess.run([sys.executable, "-c", REF_SIDE, ROOT, out], capture_output=True, text=True, timeout=900,
-                       env=dict(os.environ, OMP_NUM_THREADS="4"))
-    assert r.returncode == 0 and "REF_DONE" in r.stdout, r.stdout + r.stderr
-    return torch.load(out, map_location="cpu", weights_only=False)
+def ref():
+    return torch.load(GOLDEN, map_location="cpu", weights_only=False)
 
 
 _ns = {}
@@ -117,3 +118,7 @@ def test_host_sampler_loop_is_bitwise_the_reference(ref, variant):
     else:
         assert out.shape == want.shape and torch.isfinite(want).all()
         assert torch.equal(out, want), f"{name}: max |diff| {(out - want).abs().max().item():.3e}"
+
+
+if __name__ == "__main__":
+    regenerate()

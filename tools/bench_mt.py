@@ -1,4 +1,4 @@
-"""Marching-tetrahedra + mesh post-op throughput (BASELINE.json configs[4] tail: grids -> meshes), one B200.
+"""Marching-tetrahedra + mesh post-op throughput (BASELINE.json configs[4] tail: grids -> meshes), one GPU.
 
     python tools/bench_mt.py [--resolution 64] [--batch 32] [--steps 20]
 
@@ -83,7 +83,7 @@ def main():
     print(json.dumps({"metric": "marching-tet extraction", "resolution": args.resolution, "batch": B, "tets": F, "tet_vertices": Nv,
                       "unique_edges": mt.n_edges, "faces_per_batch": faces, **res,
                       "roofline": {"bound": "hbm", "algorithmic_bytes_per_batch": alg_bytes,
-                                   "achieved_GBps": alg_bytes / (ms * 1e-3) / 1e9, "peak_GBps": 6571.0,
+                                   "achieved_GBps": alg_bytes / (ms * 1e-3) / 1e9, "peak_GBps": 3350.0,  # H100 SXM data sheet (HBM3)
                                    "note": "latency / host-sync dominated at these sizes: the count pass returns per-sample sizes to the host"}}))
 
 

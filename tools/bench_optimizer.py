@@ -35,7 +35,7 @@ def main():
     n = off
     opt = train_ops.FusedAdam(params, lr=2e-5, betas=(0.9, 0.999), eps=1e-8)
     ema = ExponentialMovingAverage(params, decay=0.9999)
-    peak = 6571.2
+    peak = 3350.0  # GB/s, H100 SXM data sheet (HBM3)
     try:
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
     except Exception:
@@ -60,7 +60,7 @@ def main():
                                 ("ema alone", lambda: ema.update(params), 12)):
         ms = timed(fn)
         gbs = n * bytes_per / (ms * 1e-3) / 1e9
-        res[name] = {"ms": ms, "GBps": gbs, "frac_of_measured_hbm_peak": gbs / peak}
+        res[name] = {"ms": ms, "GBps": gbs, "frac_of_hbm_peak": gbs / peak}
     print(json.dumps({"parameters": n, "tensors": len(params), "hbm_peak_GBps": peak, "includes": "host-side launch overhead of the Python wrapper (pointer-table cache hit)", **res}))
 
 

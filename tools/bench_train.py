@@ -9,7 +9,8 @@ losses.get_step_fn (native perturb + loss node, engine forward / backward throug
 overlapped with the backward pass, FusedAdam with clip coefficient + EMA in one pass). One optimiser step = `iters`
 micro-batches of `batch` grids per GPU. Prints ONE JSON line: samples/s over all ranks, the device-time split (CUDA events
 around the product methods; `allreduce` is the EXPOSED wait of the optimiser on the side-stream reductions) and the achieved
-tensor-core rate (forward + backward GEMM FLOPs / their device time) against the measured sustained bf16 peak.
+tensor-core rate (forward + backward GEMM FLOPs / their device time) against the bf16 peak (MEASURED_PEAKS.json if present,
+else the H100 SXM data sheet).
 """
 import argparse
 import ctypes
@@ -145,7 +146,7 @@ def run(batch=16, iters=4, steps=3, warmup=1, config="res64", dropout=0.1, no_ov
     _native.check(L.mdb_unet_info(net._train_handle, ctypes.byref(fl), None, None, None))
     _native.check(L.mdb_unet_train_info(net._train_handle, ctypes.byref(bf), ctypes.byref(nb), ctypes.byref(numel)))
     samples = args.steps * args.iters * B * world
-    peak = 1418.0
+    peak = 989.0  # TFLOP/s, H100 SXM data sheet (dense bf16)
     try:
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops_sustained"])
     except Exception:

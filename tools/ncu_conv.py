@@ -1,6 +1,6 @@
-"""One convolution through the C ABI, for `ncu` captures of the tcgen05 kernel:
+"""One convolution through the C ABI, for profiler captures of the wgmma implicit-GEMM kernel, e.g.:
 
-    ncu --set full --clock-control none --import-source on -k regex:gemm_tc -s 1 -c 1 -o gpurun_out/prof \
+    ncu --set full --import-source on -k regex:gemm_tc -s 1 -c 1 -o conv_prof \
         python tools/ncu_conv.py <bf16|tf32|bf16x3> <B> <Cin> <Cout> <R> [reps]
 """
 import os

@@ -1,5 +1,5 @@
 """Context number (not a bench arm): the reference's op sequence (oracle restatement = the same torch ops the reference
-modules issue: conv3d / group_norm / silu / einsum / softmax / interpolate / cat) on the same B200 with stock PyTorch:
+modules issue: conv3d / group_norm / silu / einsum / softmax / interpolate / cat) on the same GPU with stock PyTorch:
 fp32 with TF32 convs (torch's default, what the reference runs) and bf16 autocast. Stand-in for the "1xA100-equivalent
 PyTorch-GPU" figure of the north star (the reference publishes no number)."""
 import json, os, sys, time

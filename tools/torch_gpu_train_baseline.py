@@ -1,5 +1,5 @@
 """Context number (not a bench arm): forward + backward of the reference's op sequence with stock PyTorch autograd on the
-same B200 (bf16 autocast, and fp32 with TF32 convolutions = torch's default, what the reference's trainer runs), next to
+same GPU (bf16 autocast, and fp32 with TF32 convolutions = torch's default, what the reference's trainer runs), next to
 which tools/bench_train.py's fwd+bwd time can be read. Uses the oracle restatement as the stock-torch model."""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
