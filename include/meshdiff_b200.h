@@ -39,7 +39,8 @@ typedef struct mdb_unet_config {
   int precision;           /* 0 = bf16 operands, 1 = tf32 operands, 2 = split bf16 ("bf16x3": every value is a (hi, lo)
                               bf16 pair and every product hi*hi + hi*lo + lo*hi -- fp32-class results, the mode that
                               meets the 1e-3 parity contract); fp32 accumulation in all three */
-  int training;            /* 1 = also build the backward plan (bf16 operands only) and keep what it needs */
+  int training;            /* 1 = also build the backward plan and keep what it needs; precision 0 (bf16) or 2 (split bf16:
+                              fp32-class gradients at about a third of the tensor rate); tf32 is refused */
 } mdb_unet_config;
 
 int mdb_unet_create(const mdb_unet_config* cfg, mdb_unet** out);
@@ -197,6 +198,10 @@ int mdb_groupnorm_act(const void* x, const long long* stats, const float* gamma,
  * dx (nullable, stride 1 only): bf16 [B][Z][Y][X][Cin]. Synchronises. */
 int mdb_conv3d_backward(const void* dy, const void* x, const float* w, int batch, int cin, int cout, int z, int y_,
                         int x_, int ksize, int stride, float* dw, void* dx, void* stream);
+/* The same with an operand mode: precision 0 = bf16 (= mdb_conv3d_backward), 2 = split bf16 (dy, x and dx rows of 2C
+ * bf16: the hi parts of the C channels, then their lo parts, as in mdb_conv3d). */
+int mdb_conv3d_backward_prec(const void* dy, const void* x, const float* w, int batch, int cin, int cout, int z, int y_,
+                             int x_, int ksize, int stride, float* dw, void* dx, int precision, void* stream);
 /* Backward of mdb_groupnorm_act (bf16): da = dL/dy [B][V][C] -> dx [B][V][C], dgamma / dbeta fp32 [C]. `add`
  * (nullable, [B][V][C]) is summed into dx. Dropout (p, seed) as in mdb_unet_set_dropout. `da` is used as scratch
  * (overwritten with the pre-activation gradient). Synchronises. */
@@ -204,6 +209,12 @@ int mdb_groupnorm_act_backward(const void* x, const long long* stats, const floa
                                void* da, const void* add, void* dx, float* dgamma, float* dbeta, int batch,
                                long long voxels, int channels, int silu, float dropout_p, unsigned long long seed,
                                void* stream);
+/* The same with an operand mode: precision 0 = bf16 (= mdb_groupnorm_act_backward), 2 = split bf16 (x, da, add and dx
+ * rows of 2C bf16, hi parts then lo parts). */
+int mdb_groupnorm_act_backward_prec(const void* x, const long long* stats, const float* gamma, const float* beta,
+                                    void* da, const void* add, void* dx, float* dgamma, float* dbeta, int batch,
+                                    long long voxels, int channels, int silu, float dropout_p, unsigned long long seed,
+                                    int precision, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Marching tetrahedra. Replaces DMTet.__call__ (nvdiffrec/lib/geometry/dmtet.py:105-163; tables :34-54, map_uv

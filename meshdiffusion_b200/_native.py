@@ -84,6 +84,8 @@ SIGNATURES = {
     "mdb_groupnorm_act": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _ll, _i, _i, _i, _vp]),
     "mdb_conv3d_backward": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "mdb_groupnorm_act_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _i, _i, _f, _u64, _vp]),
+    "mdb_conv3d_backward_prec": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
+    "mdb_groupnorm_act_backward_prec": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _i, _i, _f, _u64, _i, _vp]),
     "mdb_marching_tets_prepare": (_i, [_vp, _i, _i, _i, ctypes.POINTER(_vp)]),
     "mdb_marching_tets_destroy": (None, [_vp]),
     "mdb_marching_tets_info": (_i, [_vp, ctypes.POINTER(_i), ctypes.POINTER(_i)]),

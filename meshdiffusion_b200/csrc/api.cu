@@ -306,19 +306,26 @@ int mdb_groupnorm_act(const void* x, const long long* stats, const float* gamma,
 
 int mdb_conv3d_backward(const void* dy, const void* x, const float* w, int B, int cin, int cout, int z, int y_, int x_,
                         int ksize, int stride, float* dw, void* dx, void* stream) {
+  return mdb_conv3d_backward_prec(dy, x, w, B, cin, cout, z, y_, x_, ksize, stride, dw, dx, 0, stream);
+}
+
+int mdb_conv3d_backward_prec(const void* dy, const void* x, const float* w, int B, int cin, int cout, int z, int y_, int x_,
+                             int ksize, int stride, float* dw, void* dx, int precision, void* stream) {
   MDB_API_BEGIN
   cudaStream_t s = (cudaStream_t)stream;
+  const Precision pr = precision_from_int(precision);
+  if (pr == kTF32) throw std::runtime_error("mdb: conv3d backward takes bf16 (0) or bf16x3 (2) operands");
   const int xo = x_ / stride, yo = y_ / stride, zo = z / stride;
   Act ady; ady.ptr = const_cast<void*>(dy); ady.C = cout; ady.X = xo; ady.Y = yo; ady.Z = zo; ady.B = B;
   Act ax; ax.ptr = const_cast<void*>(x); ax.C = cin; ax.X = x_; ax.Y = y_; ax.Z = z; ax.B = B;
   if (dw) {
     const int T = ksize * ksize * ksize;
-    const WgradPlan pl = plan_wgrad(xo, yo, zo, B, cout, cin, ksize, stride);
+    const WgradPlan pl = plan_wgrad(xo, yo, zo, B, cout, cin, ksize, stride, pr == kBF16X3);
     float* scratch = nullptr;
     MDB_CUDA_CHECK(cudaMalloc(&scratch, pl.scratch_bytes));
     WgradOut o; o.ptr = dw; o.sm = (long long)cin * T; o.sn = T; o.st = 1;
     WgradOp op;
-    op.init(ady, ax, ksize, stride, o, scratch);
+    op.init(ady, ax, ksize, stride, o, scratch, pr);
     op.launch(s, B, false);
     MDB_CUDA_CHECK(cudaStreamSynchronize(s));
     cudaFree(scratch);
@@ -326,7 +333,7 @@ int mdb_conv3d_backward(const void* dy, const void* x, const float* w, int B, in
   if (dx) {
     if (stride != 1) throw std::runtime_error("mdb: conv3d data gradient entry point supports stride 1");
     GemmOp g;
-    g.set_output(kBF16, x_, y_, z, B, cin, dx, cin, false);
+    g.set_output(pr, x_, y_, z, B, cin, dx, cin, false);
     if (ksize == 1) { WSrc ws{w, 1, (long long)cin, 0, cout}; g.add_pointwise_w({ady}, &ws); }
     else g.add_conv_dgrad(ady, w, cin, ksize);
     g.finalize(s, true);
@@ -339,8 +346,16 @@ int mdb_conv3d_backward(const void* dy, const void* x, const float* w, int B, in
 int mdb_groupnorm_act_backward(const void* x, const long long* stats, const float* gamma, const float* beta, void* da,
                                const void* add, void* dx, float* dgamma, float* dbeta, int B, long long V, int C, int silu,
                                float dropout_p, unsigned long long seed, void* stream) {
+  return mdb_groupnorm_act_backward_prec(x, stats, gamma, beta, da, add, dx, dgamma, dbeta, B, V, C, silu, dropout_p, seed, 0, stream);
+}
+
+int mdb_groupnorm_act_backward_prec(const void* x, const long long* stats, const float* gamma, const float* beta, void* da,
+                                    const void* add, void* dx, float* dgamma, float* dbeta, int B, long long V, int C, int silu,
+                                    float dropout_p, unsigned long long seed, int precision, void* stream) {
   MDB_API_BEGIN
   cudaStream_t s = (cudaStream_t)stream;
+  const Precision pr = precision_from_int(precision);
+  if (pr == kTF32) throw std::runtime_error("mdb: GroupNorm backward takes bf16 (0) or bf16x3 (2) operands");
   float *part = nullptr, *sums = nullptr;
   MDB_CUDA_CHECK(cudaMalloc(&part, (size_t)kBwdPartRows(B) * C * 2 * sizeof(float)));
   MDB_CUDA_CHECK(cudaMalloc(&sums, (size_t)B * C * 2 * sizeof(float)));
@@ -350,6 +365,7 @@ int mdb_groupnorm_act_backward(const void* x, const long long* stats, const floa
   a.drop_thresh = (int)lround((double)dropout_p * 65536.0); a.drop_scale = dropout_p > 0.f ? 1.f / (1.f - dropout_p) : 1.f; a.seed = seed;
   a.part = part; a.sums = sums; a.dgamma = dgamma; a.dbeta = dbeta; a.accumulate = 0;
   a.dx = dx; a.add0 = add; a.add0_ld = C;
+  a.x3 = pr == kBF16X3 ? 1 : 0;
   launch_gn_bwd_reduce(a, B, s);
   launch_gn_bwd_apply(a, B, s);
   MDB_CUDA_CHECK(cudaStreamSynchronize(s));

@@ -309,7 +309,8 @@ void GemmOp::set_residual(const void* res, long long ldr, long long batch_stride
 
 void GemmOp::set_gn_backward(const void* x0, long long ld0, int c0, const void* x1, long long ld1, const void* consts, int silu,
                              float* part) {
-  if (prec != kBF16 || p.out_fp32 || p.ocs != 1) throw std::runtime_error("mdb: the GroupNorm-backward epilogue is built for bf16 NDHWC outputs");
+  if (prec == kTF32 || p.out_fp32 || p.ocs != 1)
+    throw std::runtime_error("mdb: the GroupNorm-backward epilogue is built for bf16 / split-bf16 NDHWC outputs");
   if (p.N % 32 != 0 || (x1 && c0 % 32 != 0)) throw std::runtime_error("mdb: GroupNorm-backward epilogue needs 32-channel aligned sources");
   if (splits > 1) throw std::runtime_error("mdb: GroupNorm-backward epilogue cannot be combined with split-K");
   gnb = true;
@@ -317,6 +318,12 @@ void GemmOp::set_gn_backward(const void* x0, long long ld0, int c0, const void* 
   p.rsx = ld0; p.rsy = ld0 * p.X; p.rsz = ld0 * p.X * p.Y; p.rsb = ld0 * p.X * p.Y * p.Z;
   p.res1 = x1; p.res_c0 = x1 ? c0 : p.N;
   p.r1sx = ld1; p.r1sy = ld1 * p.X; p.r1sz = ld1 * p.X * p.Y; p.r1sb = ld1 * p.X * p.Y * p.Z;
+  p.res_lo_off = 0; p.res1_lo_off = 0;
+  if (prec == kBF16X3) {  // (hi, lo) rows: physical pitches twice the logical ones, lo parts one logical row behind
+    p.res_lo_off = ld0; p.res1_lo_off = ld1;
+    p.rsx *= 2; p.rsy *= 2; p.rsz *= 2; p.rsb *= 2;
+    p.r1sx *= 2; p.r1sy *= 2; p.r1sz *= 2; p.r1sb *= 2;
+  }
   p.gnb_c = reinterpret_cast<const float4*>(consts);
   p.gnb_silu = silu;
   p.gnb_part = part;
@@ -528,9 +535,13 @@ void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
   const int total = tiles_m * p.n_tiles_n * (p.splits > 1 ? p.splits : 1);
   const int grid = total < sm_count() ? total : sm_count();
   if (gnb) {
-    if (tf || p.splits > 1) throw std::runtime_error("mdb: GroupNorm-backward epilogue: bf16, no split-K");
+    if (tf || p.splits > 1) throw std::runtime_error("mdb: GroupNorm-backward epilogue: bf16 or split bf16, no split-K");
     p.gnb_drop_thresh = rt_drop_thresh; p.gnb_drop_scale = rt_drop_scale; p.gnb_seed = rt_seed;
-    if (block_n == 32) launch_impl<32, false, true>(p, grid, stream); else launch_impl<128, false, true>(p, grid, stream);
+    if (prec == kBF16X3) {
+      if (block_n == 32) launch_impl<32, false, true, true>(p, grid, stream); else launch_impl<128, false, true, true>(p, grid, stream);
+    } else {
+      if (block_n == 32) launch_impl<32, false, true>(p, grid, stream); else launch_impl<128, false, true>(p, grid, stream);
+    }
     return;
   }
   const bool x3 = prec == kBF16X3;

@@ -123,7 +123,7 @@ class GemmOp {
   void set_out_col_stride(long long ocs) { p.ocs = ocs; }
   void set_residual(const void* res, long long ldr, long long batch_stride, bool fp32);
   void set_stats(long long* stats) { p.stats = stats; }
-  // GroupNorm-backward epilogue (training data gradients, bf16): the GEMM result is dL/da of a GroupNorm(+SiLU)(+dropout)
+  // GroupNorm-backward epilogue (training data gradients, bf16 or split bf16 with logical pitches): the GEMM result is dL/da of a GroupNorm(+SiLU)(+dropout)
   // whose INPUT is the channel concatenation of x0 (c0 channels, row pitch ld0) and x1; `consts` = [B][N] float4 from
   // launch_gn_consts; `part` = [gnb_rows()][N][2] per-tile partials for launch_gnb_tile_reduce. Dropout of the layer is
   // supplied per launch through rt_drop_*.

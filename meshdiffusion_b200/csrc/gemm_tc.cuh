@@ -104,6 +104,7 @@ struct GemmParams {
   // dy = da*drop*act'(y) and per-tile column partials of (sum dy, sum dy*xhat) for the GroupNorm backward.
   const void* res1;
   long long r1sx, r1sy, r1sz, r1sb;
+  long long res1_lo_off;  // X3: lo parts of the res1 rows (res rows: res_lo_off)
   int res_c0;
   const float4* gnb_c;  // [Bn][N] {hsc, hsh, rs, nm}: y/2 = x*hsc + hsh, xhat = x*rs + nm
   int gnb_silu;
@@ -139,7 +140,9 @@ __device__ __forceinline__ uint64_t kdesc(uint32_t saddr) { return make_wgmma_de
 // GNB: GroupNorm-backward epilogue (see GemmParams::gnb_c) -- a separate instantiation, so the inference kernels'
 // code is untouched.
 // X3: split-bf16 operands (see Precision::kBF16X3): the main loop is unchanged (the three partial products are extra
-// k-steps of the load table); the epilogue reads residuals and stores outputs as (hi, lo) bf16 pairs.
+// k-steps of the load table); the epilogue reads residuals and stores outputs as (hi, lo) bf16 pairs. GNB && X3 reads
+// the GroupNorm input as hi + lo, stores dy as (hi, lo) and takes the SiLU derivative from ex2/rcp (tanh.approx's 2^-11
+// would cap the gradient accuracy near 5e-4).
 template <int BLOCK_N, bool TF32, bool GNB = false, bool X3 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   using Cfg = GemmCfg<BLOCK_N>;
@@ -358,6 +361,11 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
           const uint4* rp = reinterpret_cast<const uint4*>(base + off);
 #pragma unroll
           for (int i = 0; i < 4; ++i) rbuf[i] = __ldg(rp + i);
+          if constexpr (X3) {
+            const uint4* rl = reinterpret_cast<const uint4*>(base + off + (second ? p.res1_lo_off : p.res_lo_off));
+#pragma unroll
+            for (int i = 0; i < 4; ++i) rbuf[4 + i] = __ldg(rl + i);
+          }
           return;
         }
         if (TF32 || p.res_fp32) {
@@ -431,7 +439,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
             for (int i = 0; i < 32; ++i) {
               const float4 kc = __ldg(cc + i);
               const __nv_bfloat16 xb = reinterpret_cast<const __nv_bfloat16*>(rbuf)[i];
-              const float xv = __bfloat162float(xb);
+              float xv = __bfloat162float(xb);
+              if constexpr (X3) xv += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(rbuf + 4)[i]);
               float d = v[i];
               if (p.gnb_drop_thresh > 0) {
                 const unsigned r16 = (unsigned)((hsh[i >> 2] >> (16 * (i & 3))) & 0xFFFFu);
@@ -439,9 +448,17 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
               }
               if (p.gnb_silu) {
                 const float h = fmaf(xv, kc.x, kc.y);
-                float th;
-                asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(h));
-                d *= fmaf(0.5f, h * fmaf(-th, th, 1.f), fmaf(0.5f, th, 0.5f));
+                if constexpr (X3) {
+                  // silu'(y) = s(1 + y(1 - s)), s = sigmoid(y) = 1 / (1 + 2^(-y log2 e)), y = 2h
+                  float e, sg;
+                  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(h * -2.8853900817779268f));
+                  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(sg) : "f"(1.f + e));
+                  d *= sg * fmaf(2.f * h, 1.f - sg, 1.f);
+                } else {
+                  float th;
+                  asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(h));
+                  d *= fmaf(0.5f, h * fmaf(-th, th, 1.f), fmaf(0.5f, th, 0.5f));
+                }
               }
               v[i] = d;
               q2[i] = d * fmaf(xv, kc.z, kc.w);

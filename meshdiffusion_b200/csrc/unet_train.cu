@@ -4,6 +4,9 @@
 // bandwidth kernels (backward.cu). Every forward builder records an emitter on a tape; build() runs the tape in
 // reverse, so tensor lifetimes of the whole forward+backward step are packed into one arena by the same first-fit
 // planner as the inference engine.
+// Operand modes: bf16, or split bf16 (kBF16X3): gradient tensors then use the (hi | lo) row layout of X3 activations --
+// a buffer of logical pitch ld holds 2 ld bf16 per voxel -- so every GemmOp / WgradOp / bandwidth kernel takes them
+// through the same logical pitches and channel offsets as in bf16.
 #include "unet.h"
 #include <cmath>
 #include <cstdlib>
@@ -18,7 +21,7 @@ void UNet::free_act(const TensP& t) {
 GradView UNet::new_grad(int C, int R) {
   GradView g;
   g.buf = std::make_shared<GradBuf>();
-  g.buf->off = arena_.alloc((size_t)cfg_.max_batch * R * R * R * C * 2);
+  g.buf->off = arena_.alloc((size_t)cfg_.max_batch * R * R * R * C * esize(prec_) * parts(prec_));
   g.buf->refs = 1;
   g.ptr = dry_ ? nullptr : arena_base_ + g.buf->off;
   g.ld = C; g.C = C;
@@ -28,7 +31,7 @@ GradView UNet::new_grad(int C, int R) {
 GradView UNet::grad_view(const GradView& g, int c0, int C) {
   GradView v = g;
   v.buf->refs++;
-  v.ptr = dry_ ? nullptr : (char*)g.ptr + (size_t)c0 * 2;
+  v.ptr = dry_ ? nullptr : (char*)g.ptr + (size_t)c0 * esize(prec_);  // (X3: offset into the hi parts; lo parts follow at ld)
   v.C = C;
   if (g.colsum) v.colsum = g.colsum + c0;
   return v;
@@ -150,6 +153,7 @@ void UNet::emit_colsum(const std::string& name, const GradView& t, int R, float*
     a.t = t.ptr; a.ld = t.ld; a.C = t.C; a.voxels = (long long)R * R * R;
     a.part = (float*)part.ptr; a.per = per; a.per_ld = per_ld;
     a.from_per = t.colsum; a.from_ld = t.cs_ld;
+    a.x3 = prec_ == kBF16X3 ? 1 : 0;
     add_bwd(name, [=](cudaStream_t s, int B) {
       ColsumArgs c = a;
       c.total0 = g0 >= 0 ? rt_grads_ + g0 : nullptr;
@@ -165,12 +169,12 @@ void UNet::emit_colsum(const std::string& name, const GradView& t, int R, float*
 // G[tap][m][n] = sum_p dy[p][m] x[p+tap][n] scattered to the parameter gradient at `goff` with `layout` strides
 void UNet::emit_wgrad(const std::string& name, const Act& dy, const Act& x, int ksize, int stride, long long goff,
                       const WgradOut& layout) {
-  const WgradPlan pl = plan_wgrad(dy.X, dy.Y, dy.Z, dy.B, dy.C, x.C, ksize, stride);
+  const WgradPlan pl = plan_wgrad(dy.X, dy.Y, dy.Z, dy.B, dy.C, x.C, ksize, stride, prec_ == kBF16X3);
   Tmp sc = tmp_alloc(pl.scratch_bytes);
   if (!dry_) {
     auto op = std::make_unique<WgradOp>();
     op->name = name;
-    op->init(dy, x, ksize, stride, layout, (float*)sc.ptr);
+    op->init(dy, x, ksize, stride, layout, (float*)sc.ptr, prec_);
     WgradOp* raw = op.get();
     wgrads_.push_back(std::move(op));
     const bool fixed = dy.B == 1 && cfg_.max_batch != 1;  // batch-reduced operand (mask_layer)
@@ -292,6 +296,7 @@ GradView UNet::emit_gn_backward(const std::string& pname, const std::vector<Tens
     a.add0 = add0 ? add0->ptr : nullptr; a.add0_ld = add0 ? add0->ld : 0;
     a.add1 = add1 ? add1->ptr : nullptr; a.add1_ld = add1 ? add1->ld : 0;
     a.cs_part = (float*)cs_part.ptr; a.cs_per = dx.colsum;
+    a.x3 = prec_ == kBF16X3 ? 1 : 0;
     const long long gw = G(pname + ".weight"), gb = G(pname + ".bias");
     auto with_rt = [this, a, gw, gb, drop_layer]() {
       GnBwdArgs c = a;
@@ -414,6 +419,7 @@ void UNet::tape_attn(TensP x, TensP hn, TensP qkv, TensP S, TensP O, TensP out, 
       return a;
     };
     const float alpha = 1.0f / std::sqrt((float)C);
+    const int es = esize(prec_), P = parts(prec_), x3 = prec_ == kBF16X3 ? 1 : 0;
     GradView dqkv = new_grad(3 * C, R);
     // dP[q][k] = dOo[q][:] . v[k][:]   (fp32, softmax backward then runs in place)
     Tmp dS = tmp_alloc((size_t)mb * V * V * 4);
@@ -421,52 +427,58 @@ void UNet::tape_attn(TensP x, TensP hn, TensP qkv, TensP S, TensP O, TensP out, 
       GemmOp* g = new_bwd_gemm(nm + ".dP");
       g->set_output_strided(prec_, V, 1, 1, mb, V, dS.ptr, V, 0, 0, (long long)V * V, true);
       g->add_pointwise({mat(dOo.ptr, C, C)}, nullptr, true);
-      g->set_b_activation((char*)qkv->ptr + (size_t)2 * C * 2, C, V, mb, 3 * C, (long long)V * 3 * C);
+      g->set_b_activation((char*)qkv->ptr + (size_t)2 * C * es, C, V, mb, 3 * C, (long long)V * 3 * C);
       g->finalize(0, false);
       add_bwd(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
     }
     // dv[k][c] = sum_q P[q][k] dOo[q][c]
-    Tmp PT = tmp_alloc((size_t)mb * V * V * 2);
-    Tmp dOT = tmp_alloc((size_t)mb * C * V * 2);
+    // (X3: P rows hold V hi then V lo parts; transposed rows are [V hi | V lo] again, one transpose per part)
+    Tmp PT = tmp_alloc((size_t)mb * V * V * es * P);
+    Tmp dOT = tmp_alloc((size_t)mb * C * V * es * P);
     if (!dry_) {
-      const void* sp = S->ptr; void* pt = PT.ptr; const void* dop = dOo.ptr; void* dot = dOT.ptr;
+      const void* sp = S->ptr; char* pt = (char*)PT.ptr; const void* dop = dOo.ptr; char* dot = (char*)dOT.ptr;
       add_bwd(nm + ".PT", [=](cudaStream_t s, int B) {
-        launch_transpose_vc(sp, 2 * V, 0, pt, B, V, V, 0, s);
-        launch_transpose_vc(dop, C, 0, dot, B, V, C, 0, s);
+        for (int part = 0; part < P; ++part) {
+          launch_transpose_vc(sp, 2 * V, part * V, pt + (size_t)part * V * es, B, V, V, 0, s, (long long)P * V);
+          launch_transpose_vc(dop, (long long)P * C, part * C, dot + (size_t)part * V * es, B, V, C, 0, s, (long long)P * V);
+        }
       });
       GemmOp* g = new_bwd_gemm(nm + ".dv");
-      g->set_output_strided(prec_, V, 1, 1, mb, C, (char*)dqkv.ptr + (size_t)2 * C * 2, 3 * C, 0, 0, (long long)V * 3 * C, false);
+      g->set_output_strided(prec_, V, 1, 1, mb, C, (char*)dqkv.ptr + (size_t)2 * C * es, 3 * C, 0, 0, (long long)V * 3 * C, false);
       g->add_pointwise({mat(PT.ptr, V, V)}, nullptr, true);
       g->set_b_activation(dOT.ptr, V, C, mb, V, (long long)C * V);
       g->finalize(0, false);
       add_bwd(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
       float* dsp = (float*)dS.ptr; const float* pp = (const float*)S->ptr;
-      add_bwd(nm + ".softmax_bwd", [=](cudaStream_t s, int B) { launch_softmax_bwd_rows(pp, dsp, (long long)B * V, V, s); });
+      add_bwd(nm + ".softmax_bwd", [=](cudaStream_t s, int B) { launch_softmax_bwd_rows(pp, dsp, (long long)B * V, V, s, x3); });
     }
     tmp_free(PT);
     tmp_free(dOT);
     unref(dOo);
     free_act(S);
     // dq = alpha dS . k ; dk = alpha dS^T . q
-    Tmp kT = tmp_alloc((size_t)mb * C * V * 2);
-    Tmp qT = tmp_alloc((size_t)mb * C * V * 2);
-    Tmp dST = tmp_alloc((size_t)mb * V * V * 2);
+    Tmp kT = tmp_alloc((size_t)mb * C * V * es * P);
+    Tmp qT = tmp_alloc((size_t)mb * C * V * es * P);
+    Tmp dST = tmp_alloc((size_t)mb * V * V * es * P);
     if (!dry_) {
-      const void* qp = qkv->ptr; void* ktp = kT.ptr; void* qtp = qT.ptr; const void* dsp = dS.ptr; void* dstp = dST.ptr;
+      const void* qp = qkv->ptr; char* ktp = (char*)kT.ptr; char* qtp = (char*)qT.ptr; const void* dsp = dS.ptr; char* dstp = (char*)dST.ptr;
       add_bwd(nm + ".kT", [=](cudaStream_t s, int B) {
-        launch_transpose_vc(qp, 3 * C, C, ktp, B, V, C, 0, s);
-        launch_transpose_vc(qp, 3 * C, 0, qtp, B, V, C, 0, s);
-        launch_transpose_vc(dsp, 2 * V, 0, dstp, B, V, V, 0, s);
+        for (int part = 0; part < P; ++part) {  // qkv rows: [3C hi | 3C lo]; dS rows: V hi then V lo bf16
+          launch_transpose_vc(qp, 3LL * C * P, C + part * 3 * C, ktp + (size_t)part * V * es, B, V, C, 0, s, (long long)P * V);
+          launch_transpose_vc(qp, 3LL * C * P, part * 3 * C, qtp + (size_t)part * V * es, B, V, C, 0, s, (long long)P * V);
+          launch_transpose_vc(dsp, 2 * V, part * V, dstp + (size_t)part * V * es, B, V, V, 0, s, (long long)P * V);
+        }
       });
       GemmOp* g = new_bwd_gemm(nm + ".dq");
       g->set_output_strided(prec_, V, 1, 1, mb, C, dqkv.ptr, 3 * C, 0, 0, (long long)V * 3 * C, false);
-      g->add_pointwise({mat(dS.ptr, V, 2 * V)}, nullptr, true);
+      // dS as the A operand: bf16 at the start of rows of V fp32 slots (logical pitch 2V), or X3 (hi | lo) rows filling them
+      g->add_pointwise({mat(dS.ptr, V, x3 ? V : 2 * V)}, nullptr, true);
       g->set_b_activation(kT.ptr, V, C, mb, V, (long long)C * V);
       g->set_alpha(alpha);
       g->finalize(0, false);
       add_bwd(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
       GemmOp* g2 = new_bwd_gemm(nm + ".dk");
-      g2->set_output_strided(prec_, V, 1, 1, mb, C, (char*)dqkv.ptr + (size_t)C * 2, 3 * C, 0, 0, (long long)V * 3 * C, false);
+      g2->set_output_strided(prec_, V, 1, 1, mb, C, (char*)dqkv.ptr + (size_t)C * es, 3 * C, 0, 0, (long long)V * 3 * C, false);
       g2->add_pointwise({mat(dST.ptr, V, V)}, nullptr, true);
       g2->set_b_activation(qT.ptr, V, C, mb, V, (long long)C * V);
       g2->set_alpha(alpha);
@@ -518,7 +530,8 @@ void UNet::tape_downsample(TensP x, TensP out, int midx) {
     GradView z = new_grad(C, Ri);
     if (!dry_) {
       const void* src = dO.ptr; void* dst = z.ptr;
-      add_bwd(nm + ".zero_stuff", [=](cudaStream_t s, int B) { launch_zero_stuff2x(src, dst, B, Ro, C, s); });
+      const int Cp = C * parts(prec_);  // X3: a row is 2C bf16 (hi | lo), moved as it is
+      add_bwd(nm + ".zero_stuff", [=](cudaStream_t s, int B) { launch_zero_stuff2x(src, dst, B, Ro, Cp, s); });
     }
     GradView prev = x->grad;
     GradView dx = emit_conv_dgrad(nm + ".dgrad", z, Ri, w, C, prev.valid() ? &prev : nullptr);
@@ -546,8 +559,8 @@ void UNet::tape_upsample(TensP x, TensP up, TensP out, int midx) {
     unref(out->grad);
     GradView dx = new_grad(C, x->R);
     if (!dry_) {
-      const void* src = dup.ptr; void* dst = dx.ptr; const int r = x->R;
-      add_bwd(nm + ".downsum", [=](cudaStream_t s, int B) { launch_downsum2x(src, dst, B, r, C, s); });
+      const void* src = dup.ptr; void* dst = dx.ptr; const int r = x->R; const int x3 = prec_ == kBF16X3 ? 1 : 0;
+      add_bwd(nm + ".downsum", [=](cudaStream_t s, int B) { launch_downsum2x(src, dst, B, r, C, s, x3); });
     }
     unref(dup);
     if (x->grad.valid()) throw std::runtime_error("mdb: upsample input already has a gradient");
@@ -566,10 +579,11 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
     // h0 = conv(x) + b + pos_layer.bias + mask_layer(mask): the three biases receive the same column sum
     emit_colsum("stem.dbias", dh, R0, nullptr, 0, G("all_modules.2.bias"), cfg_.use_pos_bias ? G("pos_layer.bias") : -1, G("mask_layer.bias"));
     // stem weight: dW[co][ci*T + tap] = sum_v dh[v][co] im2col(x)[v][ci*T + tap]  (im2col recomputed)
-    Tmp A0 = tmp_alloc((size_t)cfg_.max_batch * V0 * Kpad * 2);
+    const int es = esize(prec_), P = parts(prec_), mode = (int)prec_;
+    Tmp A0 = tmp_alloc((size_t)cfg_.max_batch * V0 * Kpad * es * P);
     if (!dry_) {
       void* a0 = A0.ptr;
-      add_bwd("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, 0, s); });
+      add_bwd("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, mode, s); });
     }
     {
       Act xa; xa.ptr = A0.ptr; xa.C = Kpad; xa.X = xa.Y = xa.Z = R0; xa.B = cfg_.max_batch;
@@ -578,10 +592,10 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
     }
     tmp_free(A0);
     // mask_layer weight: the mask is shared by the batch -> reduce dh over the batch first
-    Tmp hs = tmp_alloc((size_t)V0 * nf * 2);
+    Tmp hs = tmp_alloc((size_t)V0 * nf * es * P);
     if (!dry_) {
-      const void* src = dh.ptr; void* dst = hs.ptr;
-      add_bwd("stem.batch_sum", [=](cudaStream_t s, int B) { launch_batch_sum(src, dst, B, V0 * nf, s); });
+      const void* src = dh.ptr; void* dst = hs.ptr; const int x3 = prec_ == kBF16X3 ? 1 : 0;
+      add_bwd("stem.batch_sum", [=](cudaStream_t s, int B) { launch_batch_sum(src, dst, B, V0 * nf, s, nf, x3); });
     }
     {
       Act da; da.ptr = hs.ptr; da.C = nf; da.X = da.Y = da.Z = R0; da.B = 1;
@@ -607,10 +621,11 @@ void UNet::tape_head(TensP h, TensP a, const std::string& gn_name, const std::st
     // im2col of dL/dout ([voxel][co*T + tap'], reading dout at v + off(tap')) serves both gradients:
     //   dW[co][c][T-1-tap'] = sum_v a[v][c] Ad[v][co*T + tap'],   da[v][c] = sum_k Ad[v][k] W[co][c][T-1-tap']
     const int Kp = ((Cin * T + 63) / 64) * 64;
-    Tmp Ad = tmp_alloc((size_t)cfg_.max_batch * V0 * Kp * 2);
+    const int mode = (int)prec_;
+    Tmp Ad = tmp_alloc((size_t)cfg_.max_batch * V0 * Kp * esize(prec_) * parts(prec_));
     if (!dry_) {
       void* ad = Ad.ptr;
-      add_bwd("head.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_dout_, ad, B, Cin, R0, k, Kp, 0, s); });
+      add_bwd("head.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_dout_, ad, B, Cin, R0, k, Kp, mode, s); });
     }
     Act ada; ada.ptr = Ad.ptr; ada.C = Kp; ada.X = ada.Y = ada.Z = R0; ada.B = cfg_.max_batch;
     {

@@ -5,17 +5,29 @@
 
 namespace mdb {
 
-WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int stride) {
+// X3 stages carry hi and lo parts of half the voxels: the forward tile with its slowest axis of extent > 1 halved
+static Geometry half_geometry(Geometry g) {
+  if (g.bb > 1) g.bb /= 2;
+  else if (g.bz > 1) g.bz /= 2;
+  else if (g.by > 1) g.by /= 2;
+  else g.bx /= 2;
+  return g;
+}
+
+WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int stride, bool x3) {
   WgradPlan pl;
   if (ksize != 1 && ksize != 3) throw std::runtime_error("mdb: wgrad supports 1x1x1 and 3x3x3 kernels");
   pl.flat = ksize == 1;
+  const int vox = x3 ? 64 : 128;
   long long tiles;
   if (pl.flat) {
-    pl.geo = {128, 1, 1, 1};
+    pl.geo = {vox, 1, 1, 1};
     pl.n_groups = 1; pl.taps = 1;
-    tiles = ((long long)B * X * Y * Z + 127) / 128;
+    tiles = ((long long)B * X * Y * Z + vox - 1) / vox;
   } else {
     pl.geo = pick_geometry(X, Y, Z);
+    if (x3) pl.geo = half_geometry(pl.geo);
+    if (pl.geo.bx * pl.geo.by * pl.geo.bz * pl.geo.bb != vox) throw std::runtime_error("mdb: unsupported wgrad tile geometry");
     pl.n_groups = 27;
     pl.taps = 27;
     tiles = 1LL * ((X + pl.geo.bx - 1) / pl.geo.bx) * ((Y + pl.geo.by - 1) / pl.geo.by) * ((Z + pl.geo.bz - 1) / pl.geo.bz) *
@@ -32,10 +44,12 @@ WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int st
   return pl;
 }
 
-void WgradOp::init(const Act& dy, const Act& x, int ksize, int stride, const WgradOut& out, float* scratch) {
+void WgradOp::init(const Act& dy, const Act& x, int ksize, int stride, const WgradOut& out, float* scratch, Precision prec) {
+  if (prec == kTF32) throw std::runtime_error("mdb: weight gradients are built for bf16 or split-bf16 operands");
   dy_ = dy; x_ = x; ksize_ = ksize; stride_ = stride; out_ = out;
+  x3_ = prec == kBF16X3;
   M_ = dy.C; N_ = x.C;
-  plan_ = plan_wgrad(dy.X, dy.Y, dy.Z, dy.B, M_, N_, ksize, stride);
+  plan_ = plan_wgrad(dy.X, dy.Y, dy.Z, dy.B, M_, N_, ksize, stride, x3_);
   if (ksize == 3 && stride == 1 && (x.X != dy.X || x.Y != dy.Y || x.Z != dy.Z)) throw std::runtime_error("mdb: wgrad extent mismatch");
   if (ksize == 3 && stride == 2 && (x.X != 2 * dy.X || x.Y != 2 * dy.Y || x.Z != 2 * dy.Z)) throw std::runtime_error("mdb: stride-2 wgrad extent mismatch");
   if (ksize == 1 && x.voxels() != dy.voxels()) throw std::runtime_error("mdb: pointwise wgrad extent mismatch");
@@ -66,25 +80,28 @@ const WgradParams& WgradOp::params_for(int B) {
   if (it != cache_.end()) return it->second;
   WgradParams p = base_;
   const long long es = 2;
+  const long long parts = x3_ ? 2 : 1;  // X3: physical row = hi parts | lo parts; part 1 maps start one logical row in
   uint64_t dims[5], strides[4];
   uint32_t box[5];
   if (plan_.flat) {
     const long long rows = (long long)B * dy_.voxels();
-    p.tx = (int)((rows + 127) / 128); p.ty = p.tz = p.tb = 1;
-    auto enc = [&](CUtensorMap* m, const Act& a) {
+    const int vox = p.bx;
+    p.tx = (int)((rows + vox - 1) / vox); p.ty = p.tz = p.tb = 1;
+    auto enc = [&](CUtensorMap* m, const Act& a, int part) {
       dims[0] = a.C; dims[1] = rows; dims[2] = dims[3] = dims[4] = 1;
-      strides[0] = a.row() * es; strides[1] = strides[0] * rows; strides[2] = strides[1]; strides[3] = strides[1];
-      box[0] = 64; box[1] = 128; box[2] = box[3] = box[4] = 1;
-      encode_map(m, kBF16, 5, a.ptr, dims, strides, box);
+      strides[0] = a.row() * es * parts; strides[1] = strides[0] * rows; strides[2] = strides[1]; strides[3] = strides[1];
+      box[0] = 64; box[1] = vox; box[2] = box[3] = box[4] = 1;
+      encode_map(m, kBF16, 5, static_cast<char*>(a.ptr) + part * a.row() * es, dims, strides, box);
     };
-    enc(&p.ymap, dy_);
-    enc(&p.xmap[0], x_);
+    enc(&p.ymap, dy_, 0);
+    enc(&p.xmap[0], x_, 0);
+    if (x3_) { enc(&p.ymap_lo, dy_, 1); enc(&p.xmap_lo[0], x_, 1); }
   } else {
     p.tx = (dy_.X + p.bx - 1) / p.bx; p.ty = (dy_.Y + p.by - 1) / p.by; p.tz = (dy_.Z + p.bz - 1) / p.bz;
     p.tb = (B + p.bb - 1) / p.bb;
-    auto enc = [&](CUtensorMap* m, const Act& a, int sub, int px, int py, int pz) {
-      char* base = static_cast<char*>(a.ptr);
-      const long long sx = a.row() * es, sy = sx * a.X, sz = sy * a.Y, sb = sz * a.Z;
+    auto enc = [&](CUtensorMap* m, const Act& a, int sub, int px, int py, int pz, int part) {
+      char* base = static_cast<char*>(a.ptr) + part * a.row() * es;
+      const long long sx = a.row() * es * parts, sy = sx * a.X, sz = sy * a.Y, sb = sz * a.Z;
       dims[0] = a.C; dims[4] = B;
       if (sub == 1) {
         dims[1] = a.X; dims[2] = a.Y; dims[3] = a.Z;
@@ -97,11 +114,14 @@ const WgradParams& WgradOp::params_for(int B) {
       box[0] = 64; box[1] = p.bx; box[2] = p.by; box[3] = p.bz; box[4] = p.bb;
       encode_map(m, kBF16, 5, base, dims, strides, box);
     };
-    enc(&p.ymap, dy_, 1, 0, 0, 0);
-    if (stride_ == 1) {
-      enc(&p.xmap[0], x_, 1, 0, 0, 0);
-    } else {
-      for (int par = 0; par < 8; ++par) enc(&p.xmap[par], x_, 2, par & 1, (par >> 1) & 1, (par >> 2) & 1);
+    for (int part = 0; part < (int)parts; ++part) {
+      enc(part ? &p.ymap_lo : &p.ymap, dy_, 1, 0, 0, 0, part);
+      CUtensorMap* xm = part ? p.xmap_lo : p.xmap;
+      if (stride_ == 1) {
+        enc(&xm[0], x_, 1, 0, 0, 0, part);
+      } else {
+        for (int par = 0; par < 8; ++par) enc(&xm[par], x_, 2, par & 1, (par >> 1) & 1, (par >> 2) & 1, part);
+      }
     }
   }
   const long long tiles = 1LL * p.tx * p.ty * p.tz * p.tb;
@@ -149,11 +169,13 @@ void WgradOp::launch(cudaStream_t s, int B, bool accumulate, float* out_ptr) {
   MDB_CUDA_CHECK(cudaGetDevice(&dev));
   bool& configured = configured_dev[dev < 64 ? dev : 63];
   if (!configured || dev >= 63) {
-    MDB_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes));
+    MDB_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes));
+    MDB_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes));
     configured = true;
   }
   const int grid = p.m_tiles * p.n_tiles * p.n_groups * p.splits;
-  wgrad_tc_kernel<<<grid, kWgThreads, kWgSmemBytes, s>>>(p);
+  if (x3_) wgrad_tc_kernel<true><<<grid, kWgThreads, kWgSmemBytes, s>>>(p);
+  else wgrad_tc_kernel<false><<<grid, kWgThreads, kWgSmemBytes, s>>>(p);
   MDB_CUDA_CHECK(cudaGetLastError());
   WgradReduceArgs r{};
   r.partial = p.partial; r.splits = p.splits; r.taps = p.taps; r.Mp = p.Mp; r.Np = p.Np; r.M = out_.m_valid ? out_.m_valid : M_; r.N = out_.n_valid ? out_.n_valid : N_;

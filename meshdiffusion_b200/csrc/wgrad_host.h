@@ -22,7 +22,8 @@ struct WgradPlan {
   size_t scratch_bytes = 0;
 };
 // dY extents (X,Y,Z,B) = output positions of the forward op; M = dY channels, N = X-operand channels.
-WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int stride);
+// x3: split-bf16 operands (64-voxel tiles).
+WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int stride, bool x3 = false);
 
 class WgradOp {
  public:
@@ -30,7 +31,8 @@ class WgradOp {
   double flops = 0;
   // dy: [B][Z][Y][X][M] (C = M), x: the forward op's input activation (C = N; for stride 2 at twice the extents).
   // ksize 1 (pointwise; any stride-1 geometry, positions are flattened) or 3 (stride 1 pad 1, or stride 2 pad-high).
-  void init(const Act& dy, const Act& x, int ksize, int stride, const WgradOut& out, float* scratch);
+  // prec: kBF16, or kBF16X3 for split-bf16 dy / x (logical pitches, rows of hi | lo parts)
+  void init(const Act& dy, const Act& x, int ksize, int stride, const WgradOut& out, float* scratch, Precision prec = kBF16);
   // accumulate: out += G instead of out = G (micro-batch gradient accumulation)
   void launch(cudaStream_t s, int B, bool accumulate, float* out_ptr = nullptr);
   const WgradPlan& plan() const { return plan_; }
@@ -40,6 +42,7 @@ class WgradOp {
   WgradParams base_{};
   Act dy_, x_;
   int ksize_ = 1, stride_ = 1, M_ = 0, N_ = 0;
+  bool x3_ = false;
   WgradOut out_;
   std::map<int, WgradParams> cache_;  // tensor maps encoded for a given runtime batch
   const WgradParams& params_for(int B);

@@ -12,6 +12,10 @@
 // thread can hold next to its addressing.) Partials are summed in a fixed order by wgrad_reduce_kernel (deterministic
 // gradients), which also scatters into the reference's OIDHW layout.
 //
+// Split-bf16 operands (X3 instantiation, Precision::kBF16X3): dY and X are (hi, lo) bf16 pairs and the contraction is
+// dYlo.Xhi + dYhi.Xlo + dYhi.Xhi into the same register accumulator (lo.lo dropped, 2^-16 relative). A stage then
+// carries the hi and lo parts of both operands for HALF the voxels (64-voxel boxes): still 64 KB, still three stages.
+//
 // Warp roles (384 threads): warpgroup 0 = TMA producer (warp 0), warpgroups 1-2 = MMA + drain.
 #pragma once
 #include "gemm_tc.cuh"
@@ -21,7 +25,7 @@ namespace mdb {
 constexpr int kWgThreads = 384;
 constexpr int kWgStages = 3;
 constexpr int kWgYChunkBytes = 128 * kRowBytes;           // 64 channels x 128 voxels
-constexpr int kWgStageBytes = 4 * kWgYChunkBytes;         // dY and X: two 64-channel chunks each
+constexpr int kWgStageBytes = 4 * kWgYChunkBytes;         // dY and X: two 64-channel chunks each (X3: hi and lo, 64 voxels)
 constexpr int kWgSmemBytes = 1024 + kWgStages * kWgStageBytes + 2 * kWgStages * 8;
 constexpr int kWgMaxGroups = 27;
 constexpr int kWgMaxXMaps = 8;
@@ -37,9 +41,11 @@ static_assert(sizeof(WgradGroup) == 8, "WgradGroup must be 8 bytes");
 struct WgradParams {
   CUtensorMap ymap;
   CUtensorMap xmap[kWgMaxXMaps];
+  CUtensorMap ymap_lo;                // X3: the lo parts of dY / X (same boxes, one logical row behind the hi parts)
+  CUtensorMap xmap_lo[kWgMaxXMaps];
   WgradGroup groups[kWgMaxGroups];
   int n_groups;
-  int bx, by, bz, bb;   // voxel tile (product 128)
+  int bx, by, bz, bb;   // voxel tile (product 128; X3: 64)
   int tx, ty, tz, tb;   // voxel tile counts
   int m_tiles, n_tiles;
   int splits;           // CTAs sharing one (m tile, n tile, group): contiguous ranges of voxel tiles
@@ -49,7 +55,11 @@ struct WgradParams {
 };
 
 #ifdef MDB_WGRAD_KERNEL_IMPL  // the kernel itself is compiled in wgrad_host.cu only
+template <bool X3>
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ WgradParams p) {
+  // one 64-channel block of one operand part; stage = [dY blocks][dY lo blocks][X blocks][X lo blocks] (lo: X3 only)
+  constexpr int CH = X3 ? kWgYChunkBytes / 2 : kWgYChunkBytes;
+  constexpr int KS = CH / 2048;  // 16-voxel wgmma k-steps per stage
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWgStages * kWgStageBytes);
@@ -73,6 +83,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.ymap);
     tma_prefetch_desc(&p.xmap[grp.xmap]);
+    if (X3) { tma_prefetch_desc(&p.ymap_lo); tma_prefetch_desc(&p.xmap_lo[grp.xmap]); }
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kWgStages; ++i) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 2); }
@@ -99,10 +110,18 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
           const uint32_t sbase = stage0 + st * kWgStageBytes;
           mbar_expect_tx(bar, bytes);
           tma_load_5d(&p.ymap, bar, sbase, m0, x0, y0, z0, b0);
-          tma_load_5d(&p.ymap, bar, sbase + kWgYChunkBytes, m0 + 64, x0, y0, z0, b0);
-          const uint32_t xb = sbase + 2 * kWgYChunkBytes;
+          tma_load_5d(&p.ymap, bar, sbase + CH, m0 + 64, x0, y0, z0, b0);
+          if (X3) {
+            tma_load_5d(&p.ymap_lo, bar, sbase + 2 * CH, m0, x0, y0, z0, b0);
+            tma_load_5d(&p.ymap_lo, bar, sbase + 3 * CH, m0 + 64, x0, y0, z0, b0);
+          }
+          const uint32_t xb = sbase + (X3 ? 4 : 2) * CH;
           tma_load_5d(&p.xmap[grp.xmap], bar, xb, n0, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
-          tma_load_5d(&p.xmap[grp.xmap], bar, xb + kWgYChunkBytes, n0 + 64, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
+          tma_load_5d(&p.xmap[grp.xmap], bar, xb + CH, n0 + 64, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
+          if (X3) {
+            tma_load_5d(&p.xmap_lo[grp.xmap], bar, xb + 2 * CH, n0, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
+            tma_load_5d(&p.xmap_lo[grp.xmap], bar, xb + 3 * CH, n0 + 64, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
+          }
         }
         __syncwarp();
         if (++st == kWgStages) { st = 0; ph ^= 1; }
@@ -121,12 +140,22 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
       mbar_wait(full + 8 * st, ph);
       const uint32_t sbase = stage0 + st * kWgStageBytes;
       // A = this warpgroup's 64-channel dY block (one MN block); B = both 64-channel X blocks, LBO apart
-      const uint64_t a0 = make_wgmma_desc(sbase + wg * kWgYChunkBytes, kWgYChunkBytes, 1024);
-      const uint64_t b0 = make_wgmma_desc(sbase + 2 * kWgYChunkBytes, kWgYChunkBytes, 1024);
+      // (X3: hi blocks at 0 / 4 CH, lo blocks at 2 CH / 6 CH)
+      const uint64_t a0 = make_wgmma_desc(sbase + wg * CH, CH, 1024);
+      const uint64_t b0 = make_wgmma_desc(sbase + (X3 ? 4 : 2) * CH, CH, 1024);
       fence_operands(acc);
       wgmma_fence();
+      if constexpr (X3) {
+        // small terms first: dYlo.Xhi, dYhi.Xlo, then dYhi.Xhi
+        const uint64_t al = make_wgmma_desc(sbase + (2 + wg) * CH, CH, 1024);
+        const uint64_t bl = make_wgmma_desc(sbase + 6 * CH, CH, 1024);
 #pragma unroll
-      for (int c = 0; c < 8; ++c)  // 16 voxels (two 8-row swizzle groups = 2048 B) per instruction
+        for (int c = 0; c < KS; ++c) wgmma_m64n128k16_bf16<1, 1>(acc, al + c * 128, b0 + c * 128, 1u);
+#pragma unroll
+        for (int c = 0; c < KS; ++c) wgmma_m64n128k16_bf16<1, 1>(acc, a0 + c * 128, bl + c * 128, 1u);
+      }
+#pragma unroll
+      for (int c = 0; c < KS; ++c)  // 16 voxels (two 8-row swizzle groups = 2048 B) per instruction
         wgmma_m64n128k16_bf16<1, 1>(acc, a0 + c * 128, b0 + c * 128, 1u);
       wgmma_commit();
       fence_operands(acc);

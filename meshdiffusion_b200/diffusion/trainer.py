@@ -169,6 +169,8 @@ def train(config):
     iter_size = config.training.iter_size
     num_train_steps = config.training.n_iters
     gen = torch.Generator(device=device).manual_seed(int(config.get("seed", 42)) + rank)
+    if rank == 0:
+        logging.info("Training operand mode: %s (training.compute_dtype).", score_model.module.train_precision)
     logging.info("Starting training loop at step %d.", initial_step // iter_size)
     for step in range(initial_step // iter_size, num_train_steps + 1):
         tmp_loss = 0.0

@@ -100,25 +100,38 @@ def sampler_update(eps, x, noise, mask, beta, std, seed=0, offset=0):
     return x, x_mean
 
 
-def conv3d_backward(dy, x, weight, stride=1, want_dw=True, want_dx=True):
-    """bf16 NDHWC conv3d backward: dy [B,Zo,Yo,Xo,Cout], x [B,Z,Y,X,Cin], weight fp32 OIDHW -> (dw fp32 OIDHW, dx bf16)."""
+def conv3d_backward(dy, x, weight, stride=1, want_dw=True, want_dx=True, precision="bf16"):
+    """NDHWC conv3d backward: dy [B,Zo,Yo,Xo,Cout], x [B,Z,Y,X,Cin], weight fp32 OIDHW -> (dw fp32 OIDHW, dx).
+
+    precision 'bf16' (bf16 tensors) or 'bf16x3' (split bf16: rows of 2C, see to_ndhwc); dx has the dtype / layout of x."""
     L = _native.lib()
+    if precision not in ("bf16", "bf16x3"):
+        raise ValueError("conv3d_backward: precision must be 'bf16' or 'bf16x3'")
     assert dy.dtype == torch.bfloat16 and x.dtype == torch.bfloat16 and dy.is_contiguous() and x.is_contiguous()
     B, Z, Y, X, Cin = x.shape
+    parts = 2 if precision == "bf16x3" else 1
+    Cin //= parts
     Cout, k = weight.shape[0], weight.shape[2]
+    assert weight.shape[1] == Cin and dy.shape[-1] == Cout * parts
     w = weight.detach().float().contiguous()
     dw = torch.zeros_like(w) if want_dw else None
     dx = torch.empty_like(x) if want_dx else None
-    _native.check(L.mdb_conv3d_backward(_native.ptr(dy), _native.ptr(x), _native.ptr(w), B, Cin, Cout, Z, Y, X, k, stride,
-                                        _native.ptr(dw), _native.ptr(dx), _native.current_stream()))
+    _native.check(L.mdb_conv3d_backward_prec(_native.ptr(dy), _native.ptr(x), _native.ptr(w), B, Cin, Cout, Z, Y, X, k, stride,
+                                             _native.ptr(dw), _native.ptr(dx), PRECISIONS[precision], _native.current_stream()))
     return dw, dx
 
 
-def groupnorm_act_backward(x, stats, gamma, beta, da, add=None, silu=True, dropout_p=0.0, seed=0):
-    """Backward of groupnorm_act (bf16): returns (dx bf16 [B,...,C], dgamma fp32 [C], dbeta fp32 [C])."""
+def groupnorm_act_backward(x, stats, gamma, beta, da, add=None, silu=True, dropout_p=0.0, seed=0, precision="bf16"):
+    """Backward of groupnorm_act: returns (dx [B,...,C], dgamma fp32 [C], dbeta fp32 [C]).
+
+    precision 'bf16' (bf16 tensors) or 'bf16x3' (x, da, add and dx as split-bf16 rows of 2C, see to_ndhwc)."""
     L = _native.lib()
+    if precision not in ("bf16", "bf16x3"):
+        raise ValueError("groupnorm_act_backward: precision must be 'bf16' or 'bf16x3'")
     B, C = x.shape[0], x.shape[-1]
     V = x.numel() // (B * C)
+    if precision == "bf16x3":
+        C //= 2
     stats = stats_to_words(stats)
     g = gamma.detach().float().contiguous()
     bt = beta.detach().float().contiguous()
@@ -126,7 +139,8 @@ def groupnorm_act_backward(x, stats, gamma, beta, da, add=None, silu=True, dropo
     dg = torch.empty(C, device=x.device, dtype=torch.float32)
     db = torch.empty(C, device=x.device, dtype=torch.float32)
     da = da.clone()  # the kernel pair overwrites dL/dy with the pre-activation gradient
-    _native.check(L.mdb_groupnorm_act_backward(_native.ptr(x), _native.ptr(stats), _native.ptr(g), _native.ptr(bt), _native.ptr(da),
-                                               _native.ptr(add), _native.ptr(dx), _native.ptr(dg), _native.ptr(db), B, V, C,
-                                               1 if silu else 0, float(dropout_p), int(seed), _native.current_stream()))
+    _native.check(L.mdb_groupnorm_act_backward_prec(_native.ptr(x), _native.ptr(stats), _native.ptr(g), _native.ptr(bt),
+                                                    _native.ptr(da), _native.ptr(add), _native.ptr(dx), _native.ptr(dg),
+                                                    _native.ptr(db), B, V, C, 1 if silu else 0, float(dropout_p), int(seed),
+                                                    PRECISIONS[precision], _native.current_stream()))
     return dx, dg, db

@@ -1,7 +1,8 @@
 """Training-step throughput of the PRODUCT training path (BASELINE.json configs[2]: res64 train, synthetic 4x64^3 grids,
-bf16 operands, fp32 master weights + Adam + EMA, data-parallel gradient mean).
+bf16 operands by default or split bf16 with --precision bf16x3, fp32 master weights + Adam + EMA, data-parallel gradient
+mean).
 
-    python tools/bench_train.py [--batch 16] [--iters 4] [--steps 3] [--warmup 1]
+    python tools/bench_train.py [--batch 16] [--iters 4] [--steps 3] [--warmup 1] [--precision bf16|bf16x3]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P tools/bench_train.py ...
 
 The step that is timed is the one `main_diffusion.py --mode=train` runs: trainer.build_state / trainer.make_train_step ->
@@ -10,7 +11,7 @@ overlapped with the backward pass, FusedAdam with clip coefficient + EMA in one 
 micro-batches of `batch` grids per GPU. Prints ONE JSON line: samples/s over all ranks, the device-time split (CUDA events
 around the product methods; `allreduce` is the EXPOSED wait of the optimiser on the side-stream reductions) and the achieved
 tensor-core rate (forward + backward GEMM FLOPs / their device time) against the bf16 peak (MEASURED_PEAKS.json if present,
-else the H100 SXM data sheet).
+else the H100 SXM data sheet), divided by 3 for the split-bf16 plan (three bf16 MMAs per product).
 """
 import argparse
 import ctypes
@@ -25,11 +26,11 @@ os.environ.setdefault("NCCL_DEBUG", "WARN")
 import torch  # noqa: E402
 
 
-def run(batch=16, iters=4, steps=3, warmup=1, config="res64", dropout=0.1, no_overlap=False, profile=None):
+def run(batch=16, iters=4, steps=3, warmup=1, config="res64", dropout=0.1, no_overlap=False, profile=None, precision="bf16"):
     """Runs the measurement on every rank (joins the NCCL group if the caller has not) and returns the JSON line as a dict
     on rank 0 (None elsewhere). bench.py calls this in-process for its `train` leg."""
     args = argparse.Namespace(batch=batch, iters=iters, steps=steps, warmup=warmup, config=config, dropout=dropout,
-                              no_overlap=no_overlap, profile=profile)
+                              no_overlap=no_overlap, profile=profile, precision=precision)
     import torch.distributed as dist
     from configs import res64, res128
     from meshdiffusion_b200 import _native
@@ -51,6 +52,7 @@ def run(batch=16, iters=4, steps=3, warmup=1, config="res64", dropout=0.1, no_ov
         cfg.data.image_size, cfg.model.nf, cfg.model.ch_mult = 16, 32, (1, 2)
         cfg.model.num_res_blocks, cfg.model.attn_resolutions = 1, (8,)
     cfg.model.compute_dtype = "bf16"
+    cfg.training.compute_dtype = args.precision
     cfg.model.dropout = args.dropout
     cfg.training.iter_size = args.iters
     cfg.device = dev
@@ -151,6 +153,8 @@ def run(batch=16, iters=4, steps=3, warmup=1, config="res64", dropout=0.1, no_ov
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops_sustained"])
     except Exception:
         pass
+    if args.precision == "bf16x3":
+        peak /= 3.0  # three bf16 MMAs per split-bf16 product
     tc_ms = split["fwd"] + split["bwd"]
     achieved = (fl.value + bf.value) * args.steps * args.iters * B / (tc_ms * 1e-3) / 1e12 if tc_ms > 0 else None
     if args.profile and rank == 0:
@@ -167,9 +171,9 @@ def run(batch=16, iters=4, steps=3, warmup=1, config="res64", dropout=0.1, no_ov
     result = None
     if rank == 0:
         result = ({
-            "metric": "training samples/s (res64 4x64^3 grids, bf16 operands, fp32 master/Adam/EMA)", "value": samples / (ms * 1e-3),
+            "metric": f"training samples/s (res64 4x64^3 grids, {args.precision} operands, fp32 master/Adam/EMA)", "value": samples / (ms * 1e-3),
             "unit": "samples/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
-            "higher_is_better": True, "scaling": "weak", "dtype": "bf16", "data": "synthetic",
+            "higher_is_better": True, "scaling": "weak", "dtype": args.precision, "data": "synthetic",
             "path": "product: trainer.make_train_step -> losses.get_step_fn -> FusedAdam(+EMA); all-reduce " +
                     ("blocking" if args.no_overlap else f"bucketed ({len(net._grad_buckets()) if world > 1 else 0} buckets) and overlapped with backward"),
             "config": {"workload": f"{args.config}.py train, micro-batch {B} x {args.iters} per GPU, dropout {args.dropout}, clip 1.0, Adam + EMA",
@@ -196,8 +200,9 @@ def main():
     ap.add_argument("--dropout", type=float, default=0.1)
     ap.add_argument("--no-overlap", action="store_true", help="one blocking all-reduce after the backward pass instead of buckets")
     ap.add_argument("--profile", default=None, help="write per-launch device times of one forward+backward as JSON")
+    ap.add_argument("--precision", default="bf16", choices=["bf16", "bf16x3"], help="operand mode of the training plan")
     a = ap.parse_args()
-    out = run(a.batch, a.iters, a.steps, a.warmup, a.config, a.dropout, a.no_overlap, a.profile)
+    out = run(a.batch, a.iters, a.steps, a.warmup, a.config, a.dropout, a.no_overlap, a.profile, a.precision)
     if out is not None:
         print(json.dumps(out))
 
