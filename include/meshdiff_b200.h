@@ -263,6 +263,29 @@ int mdb_mesh_compute_tangents(const float* v_pos, const long long* t_pos_idx, co
                               const float* v_nrm, const long long* t_nrm_idx, int n_nrm, int n_faces, float* v_tng,
                               long long* scratch, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Point-cloud metrics of generated shapes (MMD / COV / 1-NNA over the Chamfer distance). No reference counterpart: the
+ * reference's fitting code calls kaolin's sample_points / chamfer_distance (nvdiffrec/lib/geometry/dmtet.py:455-457).
+ */
+/* Area-weighted surface sampling of n_meshes meshes packed like mdb_marching_tets_extract's output: verts fp32 [V][3],
+ * faces int64 [F][3] with indices local to their mesh (not checked here: the caller validates them), vert_off device int64
+ * [n_meshes], face_off device int64 [n_meshes + 1] (exclusive sums, face_off[n_meshes] = F). Face areas
+ * 0.5 |(b-a) x (c-a)| and their per-mesh inclusive prefix sum (the CDF) are fp64 in face order; cdf: device scratch of F
+ * doubles. Point j of mesh b takes uniforms (u, r1, r2) in [0, 1) from uniforms [n_meshes][n_points][3] or, when it is NULL,
+ * from Philox(seed, subsequence (first_id + b) * n_points + j, offset 0) (24 high bits of each of the first three outputs
+ * times 2^-24); its face is the smallest k with cdf[k] > u * total and its position
+ * (1 - sqrt r1) a + sqrt r1 (1 - r2) b + sqrt r1 r2 c -> points fp32 [n_meshes][n_points][3]. A mesh with no faces or zero
+ * total area gets n_written[b] = 0 (device int32 [n_meshes]; n_points otherwise) and none of its points are written. */
+int mdb_mesh_sample_points(const float* verts, const long long* faces, const long long* vert_off, const long long* face_off,
+                           int n_meshes, int n_points, const float* uniforms, unsigned long long seed, long long first_id,
+                           double* cdf, float* points, int* n_written, void* stream);
+/* out[i][j] = CD(A_i, B_j) fp64 [nA][nB] for A fp32 [nA][N][3], B fp32 [nB][M][3]:
+ * CD(X, Y) = mean_x min_y d(x, y) + mean_y min_x d(x, y), d = fmaf(dz, dz, fmaf(dy, dy, dx * dx)) in fp32 (the
+ * squared-distance, sum-of-two-means convention of kaolin's chamfer_distance). Bitwise reproducible and batch-invariant;
+ * CD(X, Y) and CD(Y, X) are bitwise equal. B == NULL: self matrix of A (nB, M ignored), only i < j computed and mirrored,
+ * diagonal exactly 0. The N + M per-point minima of a pair live in shared memory: N + M up to about 50 000 points. */
+int mdb_chamfer_matrix(const float* A, int nA, int N, const float* B, int nB, int M, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

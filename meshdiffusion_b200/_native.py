@@ -96,6 +96,8 @@ SIGNATURES = {
     "mdb_marching_tets_extract": (_i, [_vp, _vp, _ll, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mdb_marching_tets_vertex_ids": (_i, [_vp, _i, _vp, _vp]),
     "mdb_marching_tets_backward": (_i, [_vp, _vp, _ll, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mdb_mesh_sample_points": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _u64, _ll, _vp, _vp, _vp, _vp]),
+    "mdb_chamfer_matrix": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp]),
 }
 
 
