@@ -285,6 +285,17 @@ int mdb_mesh_sample_points(const float* verts, const long long* faces, const lon
  * CD(X, Y) and CD(Y, X) are bitwise equal. B == NULL: self matrix of A (nB, M ignored), only i < j computed and mirrored,
  * diagonal exactly 0. The N + M per-point minima of a pair live in shared memory: N + M up to about 50 000 points. */
 int mdb_chamfer_matrix(const float* A, int nA, int N, const float* B, int nB, int M, double* out, void* stream);
+/* out[i][j] = EMD(A_i, B_j) fp64 [nA][nB] for A fp32 [nA][N][3], B fp32 [nB][N][3] (equal sizes):
+ * EMD(X, Y) = min over bijections pi of (1/N) sum_i |x_i - y_pi(i)| (Euclidean, not squared), with
+ * |d| = sqrt((dx*dx + dy*dy) + dz*dz) in fp32, each operation rounded. Forward auction with epsilon-scaling, one CTA per
+ * pair: every entry is the mean cost of a bijection, at most eps above the optimum over those fp32 costs.
+ * gap[i][j] = out[i][j] minus the dual lower bound (sum_i min_j (c_ij + p_j) - sum_j p_j) / N of the final prices: a
+ * certificate that out[i][j] - optimum <= gap[i][j] <= eps. eps must be at least 2^-18 times the diagonal of the pair's
+ * joint bounding box (fp32 prices resolve it); a pair below that floor gets NaN in both outputs, a pair that needs more than
+ * 2^18 auction rounds gets out = NaN and gap = +inf. Coordinates must be finite (not checked here: the caller checks them).
+ * Bitwise reproducible and batch-invariant. B == NULL: self matrix of A (nB ignored), only i < j computed and mirrored,
+ * diagonal exactly 0 with gap 0. About 35 N bytes of shared memory per pair: N up to about 6000 points. */
+int mdb_emd_matrix(const float* A, int nA, const float* B, int nB, int N, float eps, double* out, double* gap, void* stream);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,10 @@ distance (geometry/pointcloud.py) between those clouds:
 * COV-CD  = |{argmin over Y in R of CD(X, Y) : X in G}| / |R|;
 * 1-NNA-CD = over G and R together, the share of shapes whose nearest other shape is in their own set (0.5 is ideal).
 
-Ties go to the lowest index: in R for the argmin, in the concatenated order [G..., R...] for 1-NNA.
+Ties go to the lowest index: in R for the argmin, in the concatenated order [G..., R...] for 1-NNA. With
+`eval.metric_emd` set, the same three metrics are also computed over the Earth Mover's distance (`mmd_emd`, `cov_emd`,
+`1nna_emd`, ...), each EMD solved to within EMD_EPS of the optimum; `emd_max_gap` is the largest certified gap over the
+three EMD matrices.
 """
 import glob
 import json
@@ -27,10 +30,12 @@ from ..geometry import pointcloud
 
 # grids per marching-tets launch while the sets are streamed through; only the point clouds stay on the device
 _CHUNK = 8
+# the EMD entries' tolerance: at most this far above the optimum (sampled shapes span ~1.2 units, EMD values 1e-2..1e-1)
+EMD_EPS = 1e-5
 
 
-def metrics_from_matrices(d_gr, d_gg, d_rr):
-    """The three metrics from CD matrices G x R, G x G and R x R (numpy float64)."""
+def metrics_from_matrices(d_gr, d_gg, d_rr, suffix="cd"):
+    """The three metrics from distance matrices G x R, G x G and R x R (numpy float64); keys end in `_<suffix>`."""
     d_gr, d_gg, d_rr = (np.asarray(d, dtype=np.float64) for d in (d_gr, d_gg, d_rr))
     ng, nr = d_gr.shape
     mmd = float(d_gr.min(axis=0).mean())
@@ -39,12 +44,13 @@ def metrics_from_matrices(d_gr, d_gg, d_rr):
     np.fill_diagonal(full, np.inf)
     label = np.concatenate([np.zeros(ng, bool), np.ones(nr, bool)])
     same = label[full.argmin(axis=1)] == label
-    return {"mmd_cd": mmd, "cov_cd": cov, "1nna_cd": float(same.mean()),
-            "1nna_cd_gen": float(same[:ng].mean()), "1nna_cd_ref": float(same[ng:].mean())}
+    return {f"mmd_{suffix}": mmd, f"cov_{suffix}": cov, f"1nna_{suffix}": float(same.mean()),
+            f"1nna_{suffix}_gen": float(same[:ng].mean()), f"1nna_{suffix}_ref": float(same[ng:].mean())}
 
 
-def generation_metrics(gen_points, ref_points):
-    """gen_points [nG, N, 3], ref_points [nR, N, 3] (CUDA, fp32) -> metrics dict (+ `matrix_seconds`)."""
+def generation_metrics(gen_points, ref_points, emd=False):
+    """gen_points [nG, N, 3], ref_points [nR, N, 3] (CUDA, fp32) -> metrics dict (+ `matrix_seconds`). emd: also the
+    metrics over the EMD (+ `emd_max_gap`, `emd_seconds`)."""
     if gen_points.shape[0] < 1 or ref_points.shape[0] < 1 or gen_points.shape[0] + ref_points.shape[0] < 2:
         raise ValueError("need at least one generated and one reference shape")
     torch.cuda.synchronize(gen_points.device)
@@ -56,6 +62,16 @@ def generation_metrics(gen_points, ref_points):
     seconds = time.perf_counter() - t0
     out = metrics_from_matrices(d_gr.cpu().numpy(), d_gg.cpu().numpy(), d_rr.cpu().numpy())
     out["matrix_seconds"] = seconds
+    if emd:
+        torch.cuda.synchronize(gen_points.device)
+        t0 = time.perf_counter()
+        (e_gr, g_gr), (e_gg, g_gg), (e_rr, g_rr) = (pointcloud.emd_matrix(gen_points, ref_points, EMD_EPS),
+                                                    pointcloud.emd_matrix(gen_points, eps=EMD_EPS),
+                                                    pointcloud.emd_matrix(ref_points, eps=EMD_EPS))
+        torch.cuda.synchronize(gen_points.device)
+        out["emd_seconds"] = time.perf_counter() - t0
+        out.update(metrics_from_matrices(e_gr.cpu().numpy(), e_gg.cpu().numpy(), e_rr.cpu().numpy(), suffix="emd"))
+        out["emd_max_gap"] = max(float(g.max()) for g in (g_gr, g_gg, g_rr))
     return out
 
 
@@ -110,11 +126,16 @@ def eval_metrics(config):
     sample_seconds = time.perf_counter() - t0
     logging.info("eval_metrics: %d generated (%d empty), %d reference (%d empty) shapes, %d points each",
                  gen.shape[0], n_empty_gen, ref.shape[0], n_empty_ref, n_points)
-    m = generation_metrics(gen, ref)
+    emd = bool(config.eval.get("metric_emd", False))
+    m = generation_metrics(gen, ref, emd=emd)
     out = {k: m[k] for k in ("mmd_cd", "cov_cd", "1nna_cd", "1nna_cd_gen", "1nna_cd_ref")}
     out.update(n_gen=int(gen.shape[0]), n_ref=int(ref.shape[0]), n_empty_gen=n_empty_gen, n_empty_ref=n_empty_ref,
                n_points=n_points, seed=seed, cd_convention=pointcloud.CD_CONVENTION,
                sample_seconds=sample_seconds, matrix_seconds=m["matrix_seconds"])
+    if emd:
+        out.update({k: m[k] for k in ("mmd_emd", "cov_emd", "1nna_emd", "1nna_emd_gen", "1nna_emd_ref")})
+        out.update(emd_convention=pointcloud.EMD_CONVENTION, emd_eps=EMD_EPS, emd_max_gap=m["emd_max_gap"],
+                   emd_seconds=m["emd_seconds"])
     path = os.path.join(eval_dir, "metrics.json")
     with open(path, "w") as fh:
         json.dump(out, fh, indent=2)

@@ -1,9 +1,11 @@
-"""Point clouds of generated shapes and the Chamfer distance between them, on the sm_90a kernels
-(`mdb_mesh_sample_points`, `mdb_chamfer_matrix`). No reference counterpart: the reference's fitting code calls kaolin's
-`sample_points` / `chamfer_distance` (nvdiffrec/lib/geometry/dmtet.py:455-457) and ships no evaluation code.
+"""Point clouds of generated shapes and the Chamfer and Earth Mover's distances between them, on the sm_90a kernels
+(`mdb_mesh_sample_points`, `mdb_chamfer_matrix`, `mdb_emd_matrix`). No reference counterpart: the reference's fitting code
+calls kaolin's `sample_points` / `chamfer_distance` (nvdiffrec/lib/geometry/dmtet.py:455-457) and ships no evaluation code.
 
 Chamfer convention: CD(X, Y) = mean_x min_y |x - y|^2 + mean_y min_x |x - y|^2 (squared distances, sum of the two means),
 as kaolin's `chamfer_distance` and the PointFlow evaluation code compute it.
+EMD convention: EMD(X, Y) = min over bijections pi of (1/N) sum_i |x_i - y_pi(i)| (Euclidean distances), the quantity
+PointFlow's `emd_approx` approximates; here it is solved to within a stated eps and certified by a dual bound.
 """
 import numpy as np
 import torch
@@ -12,6 +14,7 @@ from .. import _native
 from . import dmtet
 
 CD_CONVENTION = "mean_x min_y |x-y|^2 + mean_y min_x |x-y|^2 (squared Euclidean, sum of the two means)"
+EMD_CONVENTION = "min over bijections pi of mean_x |x-pi(x)| (Euclidean, not squared; clouds of equal size)"
 
 
 def _offsets(off, n, name):
@@ -78,6 +81,58 @@ def chamfer_matrix(A, B=None):
     _native.check(L.mdb_chamfer_matrix(_native.ptr(A), A.shape[0], A.shape[1], _native.ptr(B), nB, M, _native.ptr(out),
                                        _native.current_stream()))
     return out
+
+
+# the auction's fp32 limit (csrc/emd.cu kFloor): eps must be at least this share of the pair's bounding-box diagonal
+EMD_EPS_FLOOR = 2.0 ** -18
+
+
+def emd_matrix(A, B=None, eps=1e-5):
+    """A fp32 [nA, N, 3], B fp32 [nB, N, 3] (CUDA) -> (EMD(A_i, B_j), certified gap), both float64 [nA, nB].
+
+    EMD is EMD_CONVENTION, solved by an auction to within eps of the optimum: every entry is the mean cost of a true
+    bijection, and gap = entry - a dual lower bound, so 0 <= entry - optimum <= gap <= eps (over the fp32 point distances).
+    B None: the self matrix of A (symmetric, diagonal exactly 0). Bitwise reproducible; entry (i, j) does not depend on
+    the other clouds. Clouds of different sizes, non-finite coordinates and an eps below what fp32 prices resolve at the
+    clouds' scale (EMD_EPS_FLOOR x the bounding-box diagonal of a pair) raise ValueError."""
+    L = _native.lib()
+    A = A.float().contiguous()
+    if A.dim() != 3 or A.shape[2] != 3 or not A.is_cuda:
+        raise ValueError("A must be a CUDA tensor [nA, N, 3]")
+    if B is not None:
+        B = B.float().contiguous()
+        if B.dim() != 3 or B.shape[2] != 3 or B.device != A.device:
+            raise ValueError("B must be a tensor [nB, N, 3] on the device of A")
+        if B.shape[1] != A.shape[1]:
+            raise ValueError(f"EMD needs clouds of equal size, got N = {A.shape[1]} and M = {B.shape[1]}")
+    if A.shape[1] < 1:
+        raise ValueError("clouds need at least one point")
+    eps = float(eps)
+    if not (eps > 0 and np.isfinite(eps)):
+        raise ValueError("eps must be positive and finite")
+    nB = A.shape[0] if B is None else B.shape[0]
+    out = torch.zeros(A.shape[0], nB, device=A.device, dtype=torch.float64)
+    gap = torch.zeros_like(out)
+    if A.shape[0] == 0 or nB == 0:
+        return out, gap
+    Bs = A if B is None else B
+    if not (bool(torch.isfinite(A).all()) and bool(torch.isfinite(Bs).all())):
+        raise ValueError("point coordinates must be finite")
+    # the largest pair diagonal: the auction cannot resolve an eps below the floor at that scale
+    lo_a, hi_a, lo_b, hi_b = A.amin(1), A.amax(1), Bs.amin(1), Bs.amax(1)
+    ext = torch.maximum(hi_a[:, None], hi_b[None]) - torch.minimum(lo_a[:, None], lo_b[None])
+    cmax = float(ext.square().sum(-1).sqrt().max())
+    if np.float32(eps) < np.float32(cmax) * np.float32(EMD_EPS_FLOOR):
+        raise ValueError(f"eps = {eps:.3g} is below what fp32 prices resolve at these clouds' scale: the floor is "
+                         f"{EMD_EPS_FLOOR:.3g} x the bounding-box diagonal {cmax:.3g} = {cmax * EMD_EPS_FLOOR:.3g}")
+    _native.check(L.mdb_emd_matrix(_native.ptr(A), A.shape[0], _native.ptr(B), nB, A.shape[1], np.float32(eps).item(),
+                                   _native.ptr(out), _native.ptr(gap), _native.current_stream()))
+    bad = torch.isnan(out)
+    if bool(bad.any()):
+        capped = int((bad & torch.isinf(gap)).sum())
+        raise _native.NativeError(f"emd_matrix: {int(bad.sum())} entries did not converge ({capped} hit the auction's round "
+                                  f"limit; the others have an eps below the fp32 floor of their pair)")
+    return out, gap
 
 
 _TETS = {}
