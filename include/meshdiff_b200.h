@@ -82,6 +82,13 @@ int mdb_unet_set_dropout(mdb_unet* net, float p, unsigned long long seed);
 int mdb_unet_backward(mdb_unet* net, const float* dout, float* grads, long long grads_numel, int batch, int accumulate,
                       void* stream);
 int mdb_unet_grad_offset(mdb_unet* net, const char* name, long long* offset);
+/* dx = dL/dx fp32 NCDHW [B][C][R][R][R] of the immediately preceding mdb_unet_forward (same contract as mdb_unet_backward;
+ * engines with 4 input channels). grads == NULL: input gradient only -- launches whose only outputs are parameter gradients
+ * are not enqueued. grads != NULL: the full mdb_unet_backward (same grads / accumulate semantics) plus dx. dx is bitwise the
+ * same either way. Vector-Jacobian products of the score network for the probability-flow likelihood (no reference
+ * counterpart: the reference differentiates with torch autograd, lib/diffusion/likelihood.py:26-37). */
+int mdb_unet_backward_input(mdb_unet* net, const float* dout, float* dx, float* grads, long long grads_numel, int batch,
+                            int accumulate, void* stream);
 /* Data-parallel overlap (replaces the gradient gather of nn.DataParallel, lib/diffusion/models/utils.py:95): the backward
  * plan is a fixed launch list; mdb_unet_grad_ready gives, per parameter, the number of launches after which its gradient
  * is final (0 = never written). mdb_unet_backward_marked is mdb_unet_backward that additionally records the caller's CUDA
@@ -296,6 +303,16 @@ int mdb_chamfer_matrix(const float* A, int nA, int N, const float* B, int nB, in
  * Bitwise reproducible and batch-invariant. B == NULL: self matrix of A (nB ignored), only i < j computed and mirrored,
  * diagonal exactly 0 with gap 0. About 35 N bytes of shared memory per pair: N up to about 6000 points. */
 int mdb_emd_matrix(const float* A, int nA, const float* B, int nB, int N, float eps, double* out, double* gap, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Probability-flow ODE likelihood (lib/diffusion/likelihood.py:26-113 with the continuous VP score -e / std(t)).
+ * One evaluation of the ODE right-hand side between the network's forward and its input-only backward:
+ *   drift = mask * (-0.5 beta) (x - e / std)                       (VPSDE.sde + reverse(probability_flow=True))
+ *   div[b] = -0.5 beta * ( sum_masked h^2  -  (1/std) sum_masked h * g )   g = J_e^T (h * mask), from mdb_unet_backward_input
+ * x, e, h, g, drift fp32 [B][C][V]; mask [V] shared by the batch, or NULL (all ones); h = Hutchinson noise.
+ * div: fp64 per sample, fixed-order reduction (bitwise reproducible, batch-invariant). */
+int mdb_pflow_drift_div(const float* x, const float* e, const float* h, const float* g, const float* mask, float beta, float std,
+                        float* drift, double* div, int batch, int channels, long long voxels, void* stream);
 
 #ifdef __cplusplus
 }

@@ -64,6 +64,7 @@ SIGNATURES = {
     "mdb_unet_set_dropout": (_i, [_vp, _f, _u64]),
     "mdb_unet_backward": (_i, [_vp, _vp, _vp, _ll, _i, _i, _vp]),
     "mdb_unet_grad_offset": (_i, [_vp, ctypes.c_char_p, ctypes.POINTER(_ll)]),
+    "mdb_unet_backward_input": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
     "mdb_unet_grad_ready": (_i, [_vp, ctypes.c_char_p, ctypes.POINTER(_i)]),
     "mdb_unet_backward_marked": (_i, [_vp, _vp, _vp, _ll, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_vp), _i, _vp]),
     "mdb_unet_debug_stats": (_i, [_vp, _vp, _ll, ctypes.POINTER(_ll)]),
@@ -99,6 +100,7 @@ SIGNATURES = {
     "mdb_mesh_sample_points": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _u64, _ll, _vp, _vp, _vp, _vp]),
     "mdb_chamfer_matrix": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp]),
     "mdb_emd_matrix": (_i, [_vp, _i, _vp, _i, _i, _f, _vp, _vp, _vp]),
+    "mdb_pflow_drift_div": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _i, _i, _ll, _vp]),
 }
 
 

@@ -148,6 +148,14 @@ int mdb_unet_backward_marked(mdb_unet* n, const float* dout, float* grads, long 
   MDB_API_END
 }
 
+int mdb_unet_backward_input(mdb_unet* n, const float* dout, float* dx, float* grads, long long grads_numel, int B, int accumulate,
+                            void* stream) {
+  MDB_API_BEGIN
+  if (grads && grads_numel != n->net->total_param_numel()) throw std::runtime_error("mdb: gradient buffer has the wrong size");
+  n->net->backward_input(dout, dx, grads, B, accumulate != 0, (cudaStream_t)stream);
+  MDB_API_END
+}
+
 int mdb_unet_grad_ready(mdb_unet* n, const char* name, int* step) {
   MDB_API_BEGIN
   *step = n->net->grad_ready_step(name);

@@ -252,8 +252,10 @@ void launch_gn_bwd_reduce(const GnBwdArgs& a, int B, cudaStream_t s) {
   MDB_LAUNCH_CHECK();
   gn_bwd_sums_kernel<<<(B * C + 255) / 256, 256, 0, s>>>(a.part, a.sums, gx, B * C);
   MDB_LAUNCH_CHECK();
-  gn_bwd_param_kernel<<<(C + 127) / 128, 128, 0, s>>>(a.sums, a.dgamma, a.dbeta, B, C, a.accumulate);
-  MDB_LAUNCH_CHECK();
+  if (a.dgamma) {  // null: input gradient only
+    gn_bwd_param_kernel<<<(C + 127) / 128, 128, 0, s>>>(a.sums, a.dgamma, a.dbeta, B, C, a.accumulate);
+    MDB_LAUNCH_CHECK();
+  }
 }
 
 constexpr int kApplyDepth = 4;
@@ -488,8 +490,10 @@ void launch_gnb_tile_reduce(const GnBwdArgs& a, const float* tile_part, int T, i
   const int C = a.C0 + a.C1;
   gnb_tile_reduce_kernel<<<dim3((C + 31) / 32, B), dim3(32, 8), 0, s>>>(tile_part, a.sums, T, bb, C);
   MDB_LAUNCH_CHECK();
-  gn_bwd_param_kernel<<<(C + 127) / 128, 128, 0, s>>>(a.sums, a.dgamma, a.dbeta, B, C, a.accumulate);
-  MDB_LAUNCH_CHECK();
+  if (a.dgamma) {  // null: input gradient only
+    gn_bwd_param_kernel<<<(C + 127) / 128, 128, 0, s>>>(a.sums, a.dgamma, a.dbeta, B, C, a.accumulate);
+    MDB_LAUNCH_CHECK();
+  }
 }
 
 // ------------------------------------------------------------------ column sums (bias / time-embedding gradients)

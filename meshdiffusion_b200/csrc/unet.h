@@ -101,6 +101,9 @@ class UNet {
   // the rest of the backward pass still runs (grad_ready_step tells it after which launch a parameter's gradient is final)
   void backward(const float* dout, float* grads, int B, bool accumulate, cudaStream_t s, const int* mark_steps = nullptr,
                 void* const* mark_events = nullptr, int n_marks = 0);
+  // backward() that also writes dx = dL/dx (fp32 NCDHW, like the forward's x). grads == nullptr: the input gradient only --
+  // launches whose only outputs are parameter gradients are skipped, and dx is bitwise the same as with grads
+  void backward_input(const float* dout, float* dx, float* grads, int B, bool accumulate, cudaStream_t s);
   int grad_ready_step(const std::string& name) const;
   long long grad_offset(const std::string& name) const;
   long long total_param_numel() const;
@@ -132,7 +135,9 @@ class UNet {
   size_t stats_doubles_ = 0, stats_cursor_ = 0;
   std::vector<std::unique_ptr<GemmOp>> gemms_;
   std::vector<std::unique_ptr<GemmOp>> commit_gemms_;
-  struct Step { std::string name; std::function<void(cudaStream_t, int)> fn; };
+  // kind (backward plan): which outputs a launch has, so a pass that does not want them can skip it
+  enum StepKind { kAlways = 0, kParamGradOnly = 1, kInputGradOnly = 2 };
+  struct Step { std::string name; std::function<void(cudaStream_t, int)> fn; int kind = kAlways; };
   std::vector<Step> steps_, commit_steps_;
   bool committed_ = false;
   double flops_ = 0;
@@ -174,10 +179,17 @@ class UNet {
   mutable std::vector<std::string> touched_;  // parameters whose gradient offset the running backward emitter asked for
   std::map<std::string, int> grad_ready_;     // parameter -> number of backward launches after which its gradient is final
   float* rt_grads_ = nullptr; const float* rt_dout_ = nullptr; bool rt_accum_ = false;
+  float* rt_dx_ = nullptr;
+  bool has_input_grad_ = false;  // the plan carries the stem's data gradient (4 input channels, as the head's shift-sum)
   int rt_drop_thresh_ = 0; float rt_drop_scale_ = 1.f; unsigned long long rt_seed_ = 0;
   float* d_dense_out_ = nullptr;  // [mb][dense_total] gradient of the time-embedding projections
   int bwd_count_ = 0;  // launches of the backward plan emitted so far (counted in the dry pass too)
-  void add_bwd(const std::string& name, std::function<void(cudaStream_t, int)> fn) { ++bwd_count_; if (!dry_) bwd_steps_.push_back({name, fn}); }
+  void add_bwd(const std::string& name, std::function<void(cudaStream_t, int)> fn, int kind = kAlways) {
+    ++bwd_count_;
+    if (!dry_) bwd_steps_.push_back({name, fn, kind});
+  }
+  void run_backward(const float* dout, float* grads, float* dx, int B, bool accumulate, cudaStream_t s, const int* mark_steps,
+                    void* const* mark_events, int n_marks);
   void free_act(const TensP& t);
   GradView new_grad(int C, int R);
   GradView grad_view(const GradView& g, int c0, int C);

@@ -102,22 +102,36 @@ void UNet::set_dropout(float p, unsigned long long seed) {
 
 void UNet::backward(const float* dout, float* grads, int B, bool accumulate, cudaStream_t s, const int* mark_steps,
                     void* const* mark_events, int n_marks) {
+  if (!grads) throw std::runtime_error("mdb: backward() needs a gradient buffer");
+  run_backward(dout, grads, nullptr, B, accumulate, s, mark_steps, mark_events, n_marks);
+}
+
+void UNet::backward_input(const float* dout, float* dx, float* grads, int B, bool accumulate, cudaStream_t s) {
+  if (!dx) throw std::runtime_error("mdb: backward_input() needs a dx buffer");
+  if (train_ && !has_input_grad_) throw std::runtime_error("mdb: the input gradient is built for 4 input channels");
+  run_backward(dout, grads, dx, B, accumulate, s, nullptr, nullptr, 0);
+}
+
+void UNet::run_backward(const float* dout, float* grads, float* dx, int B, bool accumulate, cudaStream_t s, const int* mark_steps,
+                        void* const* mark_events, int n_marks) {
   if (!train_) throw std::runtime_error("mdb: backward() needs an engine created with training = 1");
   if (!committed_) throw std::runtime_error("mdb: parameters changed, call commit() before backward()");
   if (B < 1 || B > cfg_.max_batch) throw std::runtime_error("mdb: batch out of range");
   for (int j = 1; j < n_marks; ++j)
     if (mark_steps[j] < mark_steps[j - 1]) throw std::runtime_error("mdb: backward marks must be in ascending step order");
-  rt_dout_ = dout; rt_grads_ = grads; rt_accum_ = accumulate;
+  rt_dout_ = dout; rt_grads_ = grads; rt_accum_ = accumulate; rt_dx_ = dx;
   int mi = 0;
   auto fire = [&](int done) {
     while (mi < n_marks && mark_steps[mi] <= done) MDB_CUDA_CHECK(cudaEventRecord((cudaEvent_t)mark_events[mi++], s));
   };
   fire(0);
   for (size_t i = 0; i < bwd_steps_.size(); ++i) {
-    bwd_steps_[i].fn(s, B);
+    const int kind = bwd_steps_[i].kind;
+    if (!((kind == kParamGradOnly && !grads) || (kind == kInputGradOnly && !dx))) bwd_steps_[i].fn(s, B);
     fire((int)i + 1);
   }
   fire(1 << 30);
+  rt_dx_ = nullptr;
 }
 
 std::vector<std::pair<std::string, float>> UNet::profile_backward(const float* dout, float* grads, int B, cudaStream_t s) {
@@ -128,7 +142,7 @@ std::vector<std::pair<std::string, float>> UNet::profile_backward(const float* d
   for (auto& e : ev) MDB_CUDA_CHECK(cudaEventCreate(&e));
   MDB_CUDA_CHECK(cudaEventRecord(ev[0], s));
   for (size_t i = 0; i < bwd_steps_.size(); ++i) {
-    bwd_steps_[i].fn(s, B);
+    if (bwd_steps_[i].kind != kInputGradOnly) bwd_steps_[i].fn(s, B);
     MDB_CUDA_CHECK(cudaEventRecord(ev[i + 1], s));
   }
   MDB_CUDA_CHECK(cudaStreamSynchronize(s));
@@ -161,7 +175,7 @@ void UNet::emit_colsum(const std::string& name, const GradView& t, int R, float*
       c.total2 = g2 >= 0 ? rt_grads_ + g2 : nullptr;
       c.accumulate = rt_accum_ ? 1 : 0;
       launch_colsum(c, B, s);
-    });
+    }, kParamGradOnly);
   }
   tmp_free(part);
 }
@@ -178,7 +192,7 @@ void UNet::emit_wgrad(const std::string& name, const Act& dy, const Act& x, int 
     WgradOp* raw = op.get();
     wgrads_.push_back(std::move(op));
     const bool fixed = dy.B == 1 && cfg_.max_batch != 1;  // batch-reduced operand (mask_layer)
-    add_bwd(name, [=](cudaStream_t s, int B) { raw->launch(s, fixed ? 1 : B, rt_accum_, rt_grads_ + goff); });
+    add_bwd(name, [=](cudaStream_t s, int B) { raw->launch(s, fixed ? 1 : B, rt_accum_, rt_grads_ + goff); }, kParamGradOnly);
   }
   tmp_free(sc);
 }
@@ -304,7 +318,9 @@ GradView UNet::emit_gn_backward(const std::string& pname, const std::vector<Tens
         c.drop_thresh = rt_drop_thresh_; c.drop_scale = rt_drop_scale_;
         c.seed = rt_seed_ + 0x632BE59BD9B4E019ull * (unsigned long long)(drop_layer + 1);
       }
-      c.dgamma = rt_grads_ + gw; c.dbeta = rt_grads_ + gb; c.accumulate = rt_accum_ ? 1 : 0;
+      // input gradient only: no gamma / beta gradient (the reduce launch then skips its parameter kernel)
+      c.dgamma = rt_grads_ ? rt_grads_ + gw : nullptr; c.dbeta = rt_grads_ ? rt_grads_ + gb : nullptr;
+      c.accumulate = rt_accum_ ? 1 : 0;
       return c;
     };
     if (fused) {
@@ -370,7 +386,7 @@ void UNet::tape_resblock(const std::vector<TensP>& ins, TensP a, TensP h, TensP 
       const long long gw = G(pre + "Dense_0.weight"), gb = G(pre + "Dense_0.bias");
       add_bwd(nm + ".dense.wgrad", [=](cudaStream_t s, int B) {
         launch_outer_sum(dd, dt, ta, tdim, rt_grads_ + gw, rt_grads_ + gb, B, out_ch, tdim, rt_accum_ ? 1 : 0, s);
-      });
+      }, kParamGradOnly);
     }
     emit_wgrad(nm + ".conv0.wgrad", act_of_grad(dh, R), act_of(a), 3, 1, G(pre + "Conv_0.weight"), oidhw_layout(Cin));
     free_act(a);
@@ -576,6 +592,29 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
     free_act(h0);
     GradView dh = h0->grad;
     if (!dh.valid() || dh.ld != nf) throw std::runtime_error("mdb: stem needs a dense upstream gradient");
+    // data gradient (only `all_modules.2` reads x): the head's two-phase convolution in the mirrored direction,
+    //   P[v][tap'*Cin + ci] = sum_co dh[v][co] W[co][ci][T-1-tap']     (one GEMM, N = T*Cin = 108 / 500, K = nf)
+    //   dx[ci][v] = sum_tap' P[v + off(tap')][tap'*Cin + ci]            (off(T-1-tap') = -off(tap'); the head's shift-sum)
+    if (Cin == 4) {
+      has_input_grad_ = true;
+      const int Np = ((T * Cin + 7) / 8) * 8;
+      const bool pf32 = prec_ != kBF16;  // as the head: split bf16 keeps the per-tap projections fp32
+      Tmp Pd = tmp_alloc((size_t)cfg_.max_batch * V0 * Np * (pf32 ? 4 : 2));
+      if (!dry_) {
+        const float* sw = P("all_modules.2.weight", {});
+        GemmOp* g = new_bwd_gemm("stem.dgrad.proj");
+        g->set_output(prec_, R0, R0, R0, cfg_.max_batch, T * Cin, Pd.ptr, Np, pf32);
+        WSrc wd{sw + (T - 1), (long long)T, (long long)Cin * T, 0, nf, Cin, -1};
+        g->add_pointwise_w({act_of_grad(dh, R0)}, &wd);
+        g->finalize(0, false);
+        add_bwd(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); }, kInputGradOnly);
+        const float* zero = (const float*)dmalloc(Cin * sizeof(float));
+        const void* pp = Pd.ptr;
+        add_bwd("stem.dgrad.shift_sum", [=](cudaStream_t s, int B) { launch_tap_shift_sum(pp, Np, pf32 ? 1 : 0, zero, rt_dx_, B, R0, k, Cin, s); },
+                kInputGradOnly);
+      }
+      tmp_free(Pd);
+    }
     // h0 = conv(x) + b + pos_layer.bias + mask_layer(mask): the three biases receive the same column sum
     emit_colsum("stem.dbias", dh, R0, nullptr, 0, G("all_modules.2.bias"), cfg_.use_pos_bias ? G("pos_layer.bias") : -1, G("mask_layer.bias"));
     // stem weight: dW[co][ci*T + tap] = sum_v dh[v][co] im2col(x)[v][ci*T + tap]  (im2col recomputed)
@@ -583,7 +622,7 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
     Tmp A0 = tmp_alloc((size_t)cfg_.max_batch * V0 * Kpad * es * P);
     if (!dry_) {
       void* a0 = A0.ptr;
-      add_bwd("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, mode, s); });
+      add_bwd("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, mode, s); }, kParamGradOnly);
     }
     {
       Act xa; xa.ptr = A0.ptr; xa.C = Kpad; xa.X = xa.Y = xa.Z = R0; xa.B = cfg_.max_batch;
@@ -595,7 +634,7 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
     Tmp hs = tmp_alloc((size_t)V0 * nf * es * P);
     if (!dry_) {
       const void* src = dh.ptr; void* dst = hs.ptr; const int x3 = prec_ == kBF16X3 ? 1 : 0;
-      add_bwd("stem.batch_sum", [=](cudaStream_t s, int B) { launch_batch_sum(src, dst, B, V0 * nf, s, nf, x3); });
+      add_bwd("stem.batch_sum", [=](cudaStream_t s, int B) { launch_batch_sum(src, dst, B, V0 * nf, s, nf, x3); }, kParamGradOnly);
     }
     {
       Act da; da.ptr = hs.ptr; da.C = nf; da.X = da.Y = da.Z = R0; da.B = 1;
@@ -616,7 +655,8 @@ void UNet::tape_head(TensP h, TensP a, const std::string& gn_name, const std::st
     float* hw = P(conv_name + ".weight", {});
     if (!dry_) {
       const long long gb = G(conv_name + ".bias");
-      add_bwd("head.dbias", [=](cudaStream_t s, int B) { launch_rowsum_nc(rt_dout_, rt_grads_ + gb, B, Cin, V0, rt_accum_ ? 1 : 0, s); });
+      add_bwd("head.dbias", [=](cudaStream_t s, int B) { launch_rowsum_nc(rt_dout_, rt_grads_ + gb, B, Cin, V0, rt_accum_ ? 1 : 0, s); },
+              kParamGradOnly);
     }
     // im2col of dL/dout ([voxel][co*T + tap'], reading dout at v + off(tap')) serves both gradients:
     //   dW[co][c][T-1-tap'] = sum_v a[v][c] Ad[v][co*T + tap'],   da[v][c] = sum_k Ad[v][k] W[co][c][T-1-tap']
@@ -664,7 +704,7 @@ void UNet::tape_temb() {
       launch_temb_bwd(rt_labels_, tw0, tb0, tw1, tb1, dact, dt2, h1, dt1, emb, B, nf, s);
       launch_outer_sum(dt2, tdim, h1, tdim, rt_grads_ + g_w1, rt_grads_ + g_b1, B, tdim, tdim, rt_accum_ ? 1 : 0, s);
       launch_outer_sum(dt1, tdim, emb, nf, rt_grads_ + g_w0, rt_grads_ + g_b0, B, tdim, nf, rt_accum_ ? 1 : 0, s);
-    });
+    }, kParamGradOnly);
   });
 }
 

@@ -99,11 +99,12 @@ def make_grad_buckets(entries, total_numel, bucket_bytes):
 class _ScoreNetFn(torch.autograd.Function):
     """Autograd node of the whole score network: forward and backward both run inside the native engine, so the stock
     `loss.backward()` of the reference's step_fn (losses.py:104-139) works unchanged. Parameter gradients are written
-    by the engine straight into the module's flat fp32 gradient buffer (`p.grad` are views of it)."""
+    by the engine straight into the module's flat fp32 gradient buffer (`p.grad` are views of it). The gradient of x is
+    formed when autograd asks for it; with no parameter asking for one, the engine's input-only backward runs."""
 
     @staticmethod
     def forward(ctx, net, x, labels, *params):
-        out = net._train_forward(x, labels)
+        out = net._train_forward(x, labels, net._diff_precision(), net.dropout if net.training else 0.0)
         ctx.net = net
         ctx.save_for_backward(x, labels)
         return out
@@ -111,8 +112,8 @@ class _ScoreNetFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         x, labels = ctx.saved_tensors
-        ctx.net._train_backward(x, labels, dout)
-        return (None, None, None) + (None,) * len(ctx.net._trainable)
+        dx = ctx.net._train_backward(x, labels, dout, want_x=ctx.needs_input_grad[1], want_params=any(ctx.needs_input_grad[3:]))
+        return (None, dx, None) + (None,) * len(ctx.net._trainable)
 
 
 class _Scope(nn.Module):
@@ -138,6 +139,9 @@ class ScoreNet(nn.Module):
         self.scale_by_sigma = bool(config.model.scale_by_sigma)
         self.dropout = float(config.model.get("dropout", 0.0)) if hasattr(config.model, "get") else 0.0
         self._train_handle, self._train_batch, self._train_synced = None, 0, None
+        # training-plan engine in the inference operand mode, for input gradients through model.eval() when that mode
+        # differs from the training one (built on first use)
+        self._xgrad_handle, self._xgrad_batch, self._xgrad_synced = None, 0, None
         self._flat_grad, self._drop_calls, self._pending = None, 0, None
         # data-parallel training: when True (the trainer sets it for the last micro-batch of an optimiser step) the backward
         # pass all-reduces finished gradient buckets on a side stream while the remaining launches run
@@ -221,6 +225,9 @@ class ScoreNet(nn.Module):
         if getattr(self, "_train_handle", None) is not None:
             _native.lib().mdb_unet_destroy(self._train_handle)
             self._train_handle = None
+        if getattr(self, "_xgrad_handle", None) is not None:
+            _native.lib().mdb_unet_destroy(self._xgrad_handle)
+            self._xgrad_handle = None
 
     # ---- training engine (bf16 or split-bf16 operands, fp32 master parameters and gradients) ---------------------
     def _ensure_train_engine(self, batch, device):
@@ -237,6 +244,12 @@ class ScoreNet(nn.Module):
         with torch.cuda.device(device):
             _native.check(L.mdb_unet_create(ctypes.byref(cfg), ctypes.byref(h)))
         self._train_handle, self._train_batch, self._train_synced = h, batch, None
+        self._ensure_flat_grad(h, device)
+        self._buckets = None
+
+    def _ensure_flat_grad(self, h, device):
+        """The flat fp32 gradient buffer (parameter offsets are the same in every engine of this architecture)."""
+        L = _native.lib()
         numel = ctypes.c_longlong()
         _native.check(L.mdb_unet_train_info(h, None, None, ctypes.byref(numel)))
         if self._flat_grad is None or self._flat_grad.numel() != numel.value or self._flat_grad.device != device:
@@ -247,7 +260,38 @@ class ScoreNet(nn.Module):
                 _native.check(L.mdb_unet_grad_offset(h, n.encode(), ctypes.byref(off)))
                 p = self._param(n)
                 self._grad_views[n] = self._flat_grad[off.value:off.value + p.numel()].view(p.shape)
-        self._buckets = None
+
+    def _diff_precision(self):
+        """Operand mode of the differentiable path: the training one in model.train(), else the inference one -- which
+        the training plan must support (it refuses tf32)."""
+        if self.training:
+            return self.train_precision
+        if self.precision not in TRAIN_PRECISIONS:
+            raise ValueError(f"input gradients through model.eval() run the training plan, which takes config.model.compute_dtype "
+                             f"'bf16' or 'bf16x3', not '{self.precision}'")
+        return self.precision
+
+    def _diff_engine(self, precision, batch, device):
+        """Training-plan engine in `precision` with the current parameters: the training engine when the precisions agree,
+        else a second engine built on first use."""
+        if precision == self.train_precision:
+            self._ensure_train_engine(batch, device)
+            self._train_synced = self._push_parameters(self._train_handle, self._train_synced)
+            return self._train_handle
+        L = _native.lib()
+        if self._xgrad_handle is None or batch > self._xgrad_batch:
+            if device.type != "cuda":
+                raise _native.NativeError("the score network runs only on a CUDA (sm_90a) device; there is no CPU path")
+            if self._xgrad_handle is not None:
+                L.mdb_unet_destroy(self._xgrad_handle)
+                self._xgrad_handle = None
+            cfg = _config_c(self.arch, batch, precision, training=True)
+            h = ctypes.c_void_p()
+            with torch.cuda.device(device):
+                _native.check(L.mdb_unet_create(ctypes.byref(cfg), ctypes.byref(h)))
+            self._xgrad_handle, self._xgrad_batch, self._xgrad_synced = h, batch, None
+        self._xgrad_synced = self._push_parameters(self._xgrad_handle, self._xgrad_synced)
+        return self._xgrad_handle
 
     def _grad_buckets(self):
         """[(ready_launches, lo, hi)] covering the flat gradient buffer from its END (the head's gradients are final first,
@@ -328,56 +372,70 @@ class ScoreNet(nn.Module):
             if src.is_cuda:
                 src.record_stream(torch.cuda.current_stream())
 
-    def _train_forward(self, x, labels):
+    def _train_forward(self, x, labels, precision, p):
         L = _native.lib()
         B = x.shape[0]
         with torch.cuda.device(x.device):
-            self._ensure_train_engine(B, x.device)
-            self._train_synced = self._push_parameters(self._train_handle, self._train_synced)
-            p = self.dropout if self.training else 0.0
+            h = self._diff_engine(precision, B, x.device)
             self._drop_calls += 1
             seed = (torch.initial_seed() * 1000003 + self._drop_calls) & 0xFFFFFFFFFFFFFFFF
-            _native.check(L.mdb_unet_set_dropout(self._train_handle, p, seed))
+            _native.check(L.mdb_unet_set_dropout(h, p, seed))
             out = torch.empty_like(x)
-            _native.check(L.mdb_unet_forward(self._train_handle, _native.ptr(x), _native.ptr(labels), _native.ptr(out), B,
-                                             _native.current_stream()))
-        self._pending = (x.data_ptr(), B)
+            _native.check(L.mdb_unet_forward(h, _native.ptr(x), _native.ptr(labels), _native.ptr(out), B, _native.current_stream()))
+        self._pending = (h.value, x.data_ptr(), B)
         return out
 
-    def _train_backward(self, x, labels, dout):
+    def _train_backward(self, x, labels, dout, want_x=False, want_params=True):
         """Engine backward of the LAST forward (its activations live in the engine's arena); gradients go into the flat
-        buffer: overwritten when every p.grad is None (after zero_grad), accumulated when they are the buffer's views."""
+        buffer: overwritten when every p.grad is None (after zero_grad), accumulated when they are the buffer's views.
+        Returns dL/dx when `want_x` (else None); `want_params=False` runs the input-only plan and touches no p.grad."""
         L = _native.lib()
         B = x.shape[0]
-        if self._pending != (x.data_ptr(), B):
+        if self._pending is None or self._pending[1:] != (x.data_ptr(), B):
             raise _native.NativeError("backward() must follow the forward() it differentiates: the engine keeps the "
                                       "activations of one forward pass at a time")
+        h = ctypes.c_void_p(self._pending[0])
+        dx = torch.empty_like(x) if want_x else None
+        if not want_params:
+            with torch.cuda.device(x.device):
+                _native.check(L.mdb_unet_backward_input(h, _native.ptr(dout.float().contiguous()), _native.ptr(dx), None, 0, B, 0,
+                                                        _native.current_stream()))
+            self._pending = None
+            return dx
+        self._ensure_flat_grad(h, x.device)
+
+        def backward(grads, accumulate):
+            if dx is None:
+                _native.check(L.mdb_unet_backward(h, _native.ptr(dout), _native.ptr(grads), grads.numel(), B, accumulate,
+                                                  _native.current_stream()))
+            else:
+                _native.check(L.mdb_unet_backward_input(h, _native.ptr(dout), _native.ptr(dx), _native.ptr(grads), grads.numel(), B,
+                                                        accumulate, _native.current_stream()))
         params = [self._param(n) for n in self._trainable]
         none = [p.grad is None for p in params]
         ours = [p.grad is not None and p.grad.data_ptr() == self._grad_views[n].data_ptr() for p, n in zip(params, self._trainable)]
         dout = dout.float().contiguous()
         import torch.distributed as dist
         overlap = (self.reduce_in_backward and self.grad_overlap and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
-                   and dist.get_backend() == "nccl")
+                   and dist.get_backend() == "nccl" and dx is None and h.value == getattr(self._train_handle, "value", None))
         with torch.cuda.device(x.device):
             if all(none) or all(ours):
                 if overlap:
                     self._backward_with_overlapped_allreduce(dout, B, accumulate=not all(none))
                 else:
-                    _native.check(L.mdb_unet_backward(self._train_handle, _native.ptr(dout), _native.ptr(self._flat_grad),
-                                                      self._flat_grad.numel(), B, 0 if all(none) else 1, _native.current_stream()))
+                    backward(self._flat_grad, 0 if all(none) else 1)
                 if all(none):
                     for p, n in zip(params, self._trainable):
                         p.grad = self._grad_views[n]
             else:  # gradients owned by someone else: compute into a scratch buffer and add
                 tmp = torch.zeros_like(self._flat_grad)
-                _native.check(L.mdb_unet_backward(self._train_handle, _native.ptr(dout), _native.ptr(tmp), tmp.numel(), B, 0,
-                                                  _native.current_stream()))
+                backward(tmp, 0)
                 for p, n in zip(params, self._trainable):
                     v = self._grad_views[n]
                     g = tmp[v.storage_offset():v.storage_offset() + v.numel()].view(p.shape)
                     p.grad = g.clone() if p.grad is None else p.grad + g
         self._pending = None
+        return dx
 
     def allreduce_grads(self):
         """Data-parallel training: the mean of the flat gradient buffer over the ranks (NCCL), replacing the reference's
@@ -448,7 +506,28 @@ class ScoreNet(nn.Module):
         _native.check(L.mdb_unet_commit(self._handle, stream))
         self._synced = fp
 
+    def score_vjp(self, x, labels, v):
+        """(out, dx) = (model(x, labels), J^T v) with J = d out / d x, for `not scale_by_sigma` networks: one forward of
+        the training-plan engine in the inference operand mode (dropout 0) and its input-only backward. No autograd
+        graph and no parameter gradient; the output matches the inference engine within the mode's tolerance."""
+        if self.scale_by_sigma:
+            raise ValueError("score_vjp differentiates the raw network output (scale_by_sigma=False)")
+        if not x.is_cuda:
+            raise _native.NativeError("the score network runs only on a CUDA (sm_90a) device; there is no CPU path")
+        precision = self._diff_precision()
+        x = x.float().contiguous()
+        labels = labels.to(device=x.device, dtype=torch.float32).contiguous()
+        out = self._train_forward(x, labels, precision, 0.0)
+        return out, self._train_backward(x, labels, v, want_x=True, want_params=False)
+
     def forward(self, x, labels):
+        # input gradients through model.eval(): autograd enabled and x requiring grad runs the training-plan engine in the
+        # inference operand mode with dropout 0. Its output equals the inference engine's only within the mode's tolerance
+        # (the training plan materialises the nearest upsample; the inference plan folds it into eight parity
+        # convolutions with summed weights, which rounds differently).
+        input_grad = not self.training and torch.is_grad_enabled() and x.requires_grad
+        if input_grad:
+            self._diff_precision()  # refuses tf32 before anything runs
         if not x.is_cuda:
             raise _native.NativeError("the score network runs only on a CUDA (sm_90a) device; there is no CPU path")
         L = _native.lib()
@@ -456,8 +535,9 @@ class ScoreNet(nn.Module):
         labels = labels.to(device=x.device, dtype=torch.float32).contiguous()
         B = x.shape[0]
         # training path: model.train() + autograd enabled (what step_fn(train=True) sets up, losses.py:104-139 with
-        # get_model_fn(train=True)); everything else -- model.eval() or no_grad -- is the inference engine
-        if self.training and torch.is_grad_enabled() and any(self._param(n).requires_grad for n in self._trainable):
+        # get_model_fn(train=True)); the input-gradient path above; everything else -- model.eval() or no_grad -- is the
+        # inference engine
+        if input_grad or (self.training and torch.is_grad_enabled() and any(self._param(n).requires_grad for n in self._trainable)):
             out = _ScoreNetFn.apply(self, x, labels, *[self._param(n) for n in self._trainable])
             if self.scale_by_sigma:
                 out = out / self.sigmas.to(out.device)[labels.long(), None, None, None, None].float()

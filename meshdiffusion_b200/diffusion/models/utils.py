@@ -65,10 +65,13 @@ def get_model_fn(model, train=False):
 
 
 def get_score_fn(sde, model, train=False, continuous=False, std_scale=True):
-    """VP-SDE score from the noise-prediction network: labels = t (N-1); score = -eps / sqrt(1 - alpha_bar)."""
+    """VP-SDE score from the noise-prediction network: labels = t (N-1); score = -eps / std.
+
+    continuous=False: std = sqrt(1 - alpha_bar)[labels.long()], the discrete table the sampler and the loss use.
+    continuous=True: std = sde.marginal_prob(0, t)[1], smooth in t -- the form the probability-flow likelihood asks for
+    (the reference's likelihood.py:61, score_sde's VP likelihood): the table lookup is piecewise constant, so the ODE's
+    right-hand side would jump N - 1 times on [eps, 1] and an adaptive solver would reject a step at every jump."""
     from .. import sde_lib
-    if continuous:
-        raise AssertionError("continuous-time score models are not part of this path")
     if not isinstance(sde, sde_lib.VPSDE):
         raise NotImplementedError(f"SDE class {sde.__class__.__name__} not yet supported.")
     model_fn = get_model_fn(model, train=train)
@@ -78,7 +81,10 @@ def get_score_fn(sde, model, train=False, continuous=False, std_scale=True):
         eps = model_fn(x, labels)
         if not std_scale:
             return eps
-        std = sde.sqrt_1m_alphas_cumprod.to(labels.device)[labels.long()]
+        if continuous:
+            std = sde.marginal_prob(torch.zeros_like(x), t)[1]
+        else:
+            std = sde.sqrt_1m_alphas_cumprod.to(labels.device)[labels.long()]
         return -eps / std[:, None, None, None, None]
 
     return score_fn
