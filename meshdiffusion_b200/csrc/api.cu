@@ -302,10 +302,11 @@ int mdb_conv3d(const void* x, int B, int cin, int z, int y_, int x_, const float
 int mdb_groupnorm_act(const void* x, const long long* stats, const float* gamma, const float* beta, void* y, int B,
                       long long V, int C, int silu, int precision, void* stream) {
   MDB_API_BEGIN
+  if (!stats) throw std::runtime_error("mdb: GroupNorm needs the per-channel statistics of x (stats)");
   cudaStream_t s = (cudaStream_t)stream;
   NormActArgs na{};
-  na.x0 = x; na.C0 = C; na.ld0 = C; na.x1 = nullptr; na.C1 = 0; na.ld1 = 0; na.scale = nullptr; na.shift = nullptr;
-  na.y = y; na.voxels = V; na.silu = silu; na.tf32 = (int)precision_from_int(precision);
+  na.x0 = x; na.C0 = C; na.ld0 = C; na.x1 = nullptr; na.C1 = 0; na.ld1 = 0;
+  na.y = y; na.voxels = V; na.silu = silu; na.prec = precision_from_int(precision);
   na.stats0 = stats; na.stats1 = nullptr; na.gamma = gamma; na.beta = beta; na.groups = 32; na.eps = 1e-6f;
   launch_norm_act(na, B, s);
   MDB_CUDA_CHECK(cudaStreamSynchronize(s));
@@ -361,6 +362,7 @@ int mdb_groupnorm_act_backward_prec(const void* x, const long long* stats, const
                                     const void* add, void* dx, float* dgamma, float* dbeta, int B, long long V, int C, int silu,
                                     float dropout_p, unsigned long long seed, int precision, void* stream) {
   MDB_API_BEGIN
+  if (!stats) throw std::runtime_error("mdb: GroupNorm backward needs the forward statistics of x (stats)");
   cudaStream_t s = (cudaStream_t)stream;
   const Precision pr = precision_from_int(precision);
   if (pr == kTF32) throw std::runtime_error("mdb: GroupNorm backward takes bf16 (0) or bf16x3 (2) operands");
@@ -370,10 +372,11 @@ int mdb_groupnorm_act_backward_prec(const void* x, const long long* stats, const
   GnBwdArgs a{};
   a.x0 = x; a.C0 = C; a.ld0 = C; a.stats0 = stats; a.gamma = gamma; a.beta = beta; a.da = da;
   a.voxels = V; a.silu = silu; a.groups = 32; a.eps = 1e-6f;
-  a.drop_thresh = (int)lround((double)dropout_p * 65536.0); a.drop_scale = dropout_p > 0.f ? 1.f / (1.f - dropout_p) : 1.f; a.seed = seed;
+  const DropoutParams d = dropout_params(dropout_p);
+  a.drop_thresh = d.thresh; a.drop_scale = d.scale; a.seed = seed;
   a.part = part; a.sums = sums; a.dgamma = dgamma; a.dbeta = dbeta; a.accumulate = 0;
   a.dx = dx; a.add0 = add; a.add0_ld = C;
-  a.x3 = pr == kBF16X3 ? 1 : 0;
+  a.prec = pr;
   launch_gn_bwd_reduce(a, B, s);
   launch_gn_bwd_apply(a, B, s);
   MDB_CUDA_CHECK(cudaStreamSynchronize(s));

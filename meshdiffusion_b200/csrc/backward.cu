@@ -1,64 +1,12 @@
 // Bandwidth-bound kernels of the training backward pass (bf16 or split-bf16 activations, fp32 parameter gradients).
-// MODE template parameter: 0 = bf16, 2 = split bf16 (X3: every 16-byte vector of hi parts has a lo vector one logical row
-// further on; decoded as hi + lo, computed in fp32, stored as (hi, lo) again).
+// Template parameter PR: kBF16 or kBF16X3 (every 16-byte vector of hi parts has a lo vector one logical row further on;
+// decoded as hi + lo, computed in fp32, stored as (hi, lo) again: act_format.cuh).
 #include "backward.cuh"
 #include "gn_stats.cuh"
-#include <stdexcept>
-#include <string>
 
 namespace mdb {
 
-#define MDB_LAUNCH_CHECK()                                                                              \
-  do {                                                                                                  \
-    cudaError_t _e = cudaGetLastError();                                                                \
-    if (_e != cudaSuccess) throw std::runtime_error(std::string("mdb launch: ") + cudaGetErrorString(_e)); \
-  } while (0)
-
 constexpr int VEC = 8;  // bf16 elements per 16-byte vector
-
-__device__ __forceinline__ void unpack8(const uint4& raw, float* x) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&raw);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) { const float2 f = __bfloat1622float2(h[j]); x[2 * j] = f.x; x[2 * j + 1] = f.y; }
-}
-__device__ __forceinline__ uint4 pack8(const float* x) {
-  uint4 t;
-  __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&t);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) h[j] = __floats2bfloat162_rn(x[2 * j], x[2 * j + 1]);
-  return t;
-}
-__device__ __forceinline__ float sigmoid_fast(float x) {
-  float t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
-  return fmaf(0.5f, t, 0.5f);
-}
-__device__ __forceinline__ float dsilu(float y) {
-  const float s = sigmoid_fast(y);
-  return s * fmaf(y, 1.f - s, 1.f);
-}
-// SiLU derivative for split-bf16 gradients: sigmoid as ex2.approx + rcp.approx (~2^-22 each, the form of the forward
-// norm/act kernel) -- tanh.approx's 2^-11 error alone would cap the gradient accuracy near 5e-4
-__device__ __forceinline__ float dsilu_x3(float y) {
-  float e, s;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(y * -1.4426950408889634f));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(s) : "f"(1.f + e));
-  return s * fmaf(y, 1.f - s, 1.f);
-}
-// lo vector of a split-bf16 store: what the bf16 rounding of the hi vector `hi` (= pack8(x)) lost
-__device__ __forceinline__ uint4 pack8_lo(const uint4& hi, const float* x) {
-  float h[VEC], d[VEC];
-  unpack8(hi, h);
-#pragma unroll
-  for (int j = 0; j < VEC; ++j) d[j] = x[j] - h[j];
-  return pack8(d);
-}
-__device__ __forceinline__ void add8(const uint4& raw, float* x) {
-  float l[VEC];
-  unpack8(raw, l);
-#pragma unroll
-  for (int j = 0; j < VEC; ++j) x[j] += l[j];
-}
 
 // grid.x for the staged, grid-stride kernels: the whole grid is ONE full wave of `target` = 132 x (resident blocks per
 // SM) blocks -- a launch a few blocks over one wave would spend a second, nearly empty wave on them.
@@ -72,9 +20,7 @@ static inline int blocks_x(long long voxels, int k, int B, int target) {
 
 // mean / rstd of the GroupNorm group of each of the thread's VEC channels, from the forward statistics
 __device__ __forceinline__ void gn_stats_of(const GnBwdArgs& a, int b, int c, float* mean, float* rstd) {
-  const int C = a.C0 + a.C1;
-  const int cpg = C / a.groups;
-  const double n = (double)a.voxels * cpg;
+  const int cpg = (a.C0 + a.C1) / a.groups;
   int cur_g = -1;
   float m = 0.f, r = 0.f;
 #pragma unroll
@@ -82,44 +28,17 @@ __device__ __forceinline__ void gn_stats_of(const GnBwdArgs& a, int b, int c, fl
     const int g = (c + j) / cpg;
     if (g != cur_g) {
       cur_g = g;
-      StatAcc acc;
-      for (int i = 0; i < cpg; ++i) {
-        const int cc = g * cpg + i;
-        acc.add((cc < a.C0) ? a.stats0 + ((long long)b * a.C0 + cc) * kStatWords : a.stats1 + ((long long)b * a.C1 + (cc - a.C0)) * kStatWords);
-      }
-      const double mm = acc.sum() / n;
-      double var = acc.sumsq() / n - mm * mm;
-      if (var < 0) var = 0;
-      m = (float)mm;
-      r = (float)(1.0 / sqrt(var + (double)a.eps));
+      gn_group_stats(a.stats0, a.C0, a.stats1, a.C1, b, g, cpg, a.voxels, a.eps, m, r);
     }
     mean[j] = m; rstd[j] = r;
   }
 }
 
-// dy[j] = da[j] * act'(y[j]) * dropout, xh[j] = normalised input
-__device__ __forceinline__ void gn_dy(const GnBwdArgs& a, const float* x, const float* da, const float* mean, const float* rstd,
-                                      const float* g, const float* be, long long e0, float* xh, float* dy) {
-  unsigned long long h0 = 0, h1 = 0;
-  if (a.drop_thresh > 0) { h0 = drop_hash64(a.seed, (unsigned long long)(e0 >> 2)); h1 = drop_hash64(a.seed, (unsigned long long)(e0 >> 2) + 1); }
-#pragma unroll
-  for (int j = 0; j < VEC; ++j) {
-    xh[j] = (x[j] - mean[j]) * rstd[j];
-    float d = da[j];
-    if (a.drop_thresh > 0) {
-      const unsigned r16 = (unsigned)(((j < 4 ? h0 : h1) >> (16 * (j & 3))) & 0xFFFFu);
-      d = r16 >= (unsigned)a.drop_thresh ? d * a.drop_scale : 0.f;
-    }
-    if (a.silu) d *= dsilu(fmaf(g[j], xh[j], be[j]));
-    dy[j] = d;
-  }
-}
-
 // Pass 1. Per element: h = 0.5*y straight from x (one FMA with folded constants), silu'(y) = t + 0.5*h*q with
 // t = (1+tanh h)/2, q = 1 - tanh^2 h; S2 is accumulated as sum(dy*x) and rebased to sum(dy*xhat) once per thread.
-template <int MODE>
+template <Precision PR>
 __global__ void __launch_bounds__(256, 2) gn_bwd_reduce_kernel(GnBwdArgs a, int cv, int k) {
-  constexpr bool X3 = MODE == 2;
+  constexpr bool X3 = PR == kBF16X3;
   constexpr int P = X3 ? 2 : 1;
   constexpr int UNROLL = 4;
   __shared__ float red[256 * VEC * 2];
@@ -165,38 +84,21 @@ __global__ void __launch_bounds__(256, 2) gn_bwd_reduce_kernel(GnBwdArgs a, int 
       const long long v = v0 + u * step;
       if (v >= a.voxels) continue;
       float x[VEC], dy[VEC];
-      unpack8(rx[u], x); unpack8(rd[u], dy);
-      if constexpr (X3) { add8(rxl[u], x); add8(rdl[u], dy); }
-      if (a.drop_thresh > 0) {
-        const unsigned long long e4 = (unsigned long long)((((long long)b * a.voxels + v) * C + c) >> 2);
-        const unsigned long long h0 = drop_hash64(a.seed, e4), h1 = drop_hash64(a.seed, e4 + 1);
-#pragma unroll
-        for (int j = 0; j < VEC; ++j) {
-          const unsigned r16 = (unsigned)(((j < 4 ? h0 : h1) >> (16 * (j & 3))) & 0xFFFFu);
-          dy[j] = r16 >= (unsigned)a.drop_thresh ? dy[j] * a.drop_scale : 0.f;
-        }
-      }
+      decode_vec<PR>(rx[u], rxl[X3 ? u : 0], x);
+      decode_vec<PR>(rd[u], rdl[X3 ? u : 0], dy);
+      if (a.drop_thresh > 0)
+        apply_dropout<2>(dy, a.seed, (unsigned long long)((((long long)b * a.voxels + v) * C + c) >> 2), a.drop_thresh, a.drop_scale);
       if (a.silu) {
 #pragma unroll
         for (int j = 0; j < VEC; ++j) {
           const float h = fmaf(x[j], hsc[j], hsh[j]);
-          if constexpr (X3) {
-            dy[j] *= dsilu_x3(2.f * h);
-          } else {
-            float th;
-            asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(h));
-            const float q = fmaf(-th, th, 1.f);
-            const float t = fmaf(0.5f, th, 0.5f);
-            dy[j] *= fmaf(0.5f, h * q, t);
-          }
+          dy[j] *= X3 ? dsilu_ex2(2.f * h) : dsilu_tanh_half(h);
         }
       }
 #pragma unroll
       for (int j = 0; j < VEC; ++j) { s1[j] += dy[j]; s2[j] = fmaf(dy[j], x[j], s2[j]); }
       // dy replaces da in place: pass 2 then needs neither the activation derivative nor the dropout hash again
-      const uint4 hv = pack8(dy);
-      *((uint4*)(dsrc + v * d_stride)) = hv;
-      if constexpr (X3) *((uint4*)(dsrc + v * d_stride + d_lo)) = pack8_lo(hv, dy);
+      store_vec<PR>(dsrc + v * d_stride, d_lo, dy);
     }
   }
   {
@@ -247,8 +149,8 @@ void launch_gn_bwd_reduce(const GnBwdArgs& a, int B, cudaStream_t s) {
   gn_launch_shape(a, cv, k);
   const int C = a.C0 + a.C1;
   const int gx = blocks_x(a.voxels, k, B, 2 * 132);
-  if (a.x3) gn_bwd_reduce_kernel<2><<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
-  else gn_bwd_reduce_kernel<0><<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
+  if (a.prec == kBF16X3) gn_bwd_reduce_kernel<kBF16X3><<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
+  else gn_bwd_reduce_kernel<kBF16><<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
   MDB_LAUNCH_CHECK();
   gn_bwd_sums_kernel<<<(B * C + 255) / 256, 256, 0, s>>>(a.part, a.sums, gx, B * C);
   MDB_LAUNCH_CHECK();
@@ -268,9 +170,9 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // NADD = number of addend streams (0, 1, 2): absent streams cost no instructions (GroupNorm_1 layers have none)
-template <int NADD, int MODE>
+template <int NADD, Precision PR>
 __global__ void __launch_bounds__(256, 3) gn_bwd_apply_kernel(GnBwdArgs a, int cv, int k) {
-  constexpr bool X3 = MODE == 2;
+  constexpr bool X3 = PR == kBF16X3;
   constexpr int P = X3 ? 2 : 1;
   constexpr int DEPTH = X3 ? kApplyDepth / 2 : kApplyDepth;  // the same 64 KB ring
   constexpr int NS = 4 * P;                                   // slots per stage: 4 streams (X3: hi slots 0-3, lo 4-7)
@@ -352,31 +254,26 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_apply_kernel(GnBwdArgs a, int c
     if (nst >= DEPTH) nst -= DEPTH;
     issue(v + (long long)(DEPTH - 1) * step, nst);
     cp_async_wait<DEPTH - 1>();
-    const uint4 cx = *slot(stage, 0), cd = *slot(stage, 1);
     float x[VEC], dy[VEC], o[VEC];
-    unpack8(cx, x); unpack8(cd, dy);
-    if constexpr (X3) { add8(*slot(stage, 4), x); add8(*slot(stage, 5), dy); }
+    decode_vec<PR>(*slot(stage, 0), *slot(stage, X3 ? 4 : 0), x);
+    decode_vec<PR>(*slot(stage, 1), *slot(stage, X3 ? 5 : 1), dy);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) o[j] = fmaf(-x[j], k1[j], fmaf(c1[j], dy[j], -k0[j]));
     if (NADD >= 1) {
       float e[VEC];
-      unpack8(*slot(stage, 2), e);
-      if constexpr (X3) add8(*slot(stage, 6), e);
+      decode_vec<PR>(*slot(stage, 2), *slot(stage, X3 ? 6 : 2), e);
 #pragma unroll
       for (int j = 0; j < VEC; ++j) o[j] += e[j];
     }
     if (NADD >= 2) {
       float e[VEC];
-      unpack8(*slot(stage, 3), e);
-      if constexpr (X3) add8(*slot(stage, 7), e);
+      decode_vec<PR>(*slot(stage, 3), *slot(stage, X3 ? 7 : 3), e);
 #pragma unroll
       for (int j = 0; j < VEC; ++j) o[j] += e[j];
     }
 #pragma unroll
     for (int j = 0; j < VEC; ++j) cs[j] += o[j];
-    const uint4 hv = pack8(o);
-    *((uint4*)(dst + v * d_stride)) = hv;
-    if constexpr (X3) *((uint4*)(dst + v * d_stride + d_lo)) = pack8_lo(hv, o);
+    store_vec<PR>(dst + v * d_stride, d_lo, o);
     if (++stage == DEPTH) stage = 0;
   }
   cp_async_wait<0>();
@@ -412,25 +309,25 @@ void launch_gn_bwd_apply(const GnBwdArgs& a, int B, cudaStream_t s) {
   cudaGetDevice(&dev);
   bool& configured = configured_dev[dev < 64 ? dev : 63];
   if (!configured || dev >= 63) {
-    cudaFuncSetAttribute(gn_bwd_apply_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
-    cudaFuncSetAttribute(gn_bwd_apply_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
-    cudaFuncSetAttribute(gn_bwd_apply_kernel<2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
-    cudaFuncSetAttribute(gn_bwd_apply_kernel<0, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
-    cudaFuncSetAttribute(gn_bwd_apply_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
-    cudaFuncSetAttribute(gn_bwd_apply_kernel<2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
+    cudaFuncSetAttribute(gn_bwd_apply_kernel<0, kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
+    cudaFuncSetAttribute(gn_bwd_apply_kernel<1, kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
+    cudaFuncSetAttribute(gn_bwd_apply_kernel<2, kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
+    cudaFuncSetAttribute(gn_bwd_apply_kernel<0, kBF16X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
+    cudaFuncSetAttribute(gn_bwd_apply_kernel<1, kBF16X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
+    cudaFuncSetAttribute(gn_bwd_apply_kernel<2, kBF16X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApplySmem);
     configured = true;
   }
   GnBwdArgs q = a;
   if (!q.add0 && q.add1) { q.add0 = q.add1; q.add0_ld = q.add1_ld; q.add1 = nullptr; }  // streams are filled front to back
   const dim3 grid((unsigned)gx, B);
-  if (q.x3) {
-    if (q.add1) gn_bwd_apply_kernel<2, 2><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
-    else if (q.add0) gn_bwd_apply_kernel<1, 2><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
-    else gn_bwd_apply_kernel<0, 2><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
+  if (q.prec == kBF16X3) {
+    if (q.add1) gn_bwd_apply_kernel<2, kBF16X3><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
+    else if (q.add0) gn_bwd_apply_kernel<1, kBF16X3><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
+    else gn_bwd_apply_kernel<0, kBF16X3><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
   } else {
-    if (q.add1) gn_bwd_apply_kernel<2, 0><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
-    else if (q.add0) gn_bwd_apply_kernel<1, 0><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
-    else gn_bwd_apply_kernel<0, 0><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
+    if (q.add1) gn_bwd_apply_kernel<2, kBF16><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
+    else if (q.add0) gn_bwd_apply_kernel<1, kBF16><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
+    else gn_bwd_apply_kernel<0, kBF16><<<grid, cv * k, kApplySmem, s>>>(q, cv, k);
   }
   MDB_LAUNCH_CHECK();
   if (a.cs_part) {
@@ -445,17 +342,9 @@ __global__ void gn_consts_kernel(GnBwdArgs a, float4* __restrict__ out, int B) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * C) return;
   const int b = i / C, c = i % C;
-  const int cpg = C / a.groups, g = c / cpg;
-  StatAcc acc;
-  for (int j = 0; j < cpg; ++j) {
-    const int cc = g * cpg + j;
-    acc.add((cc < a.C0) ? a.stats0 + ((long long)b * a.C0 + cc) * kStatWords : a.stats1 + ((long long)b * a.C1 + (cc - a.C0)) * kStatWords);
-  }
-  const double n = (double)a.voxels * cpg;
-  const double mm = acc.sum() / n;
-  double var = acc.sumsq() / n - mm * mm;
-  if (var < 0) var = 0;
-  const float mean = (float)mm, rstd = (float)(1.0 / sqrt(var + (double)a.eps));
+  const int cpg = C / a.groups;
+  float mean, rstd;
+  gn_group_stats(a.stats0, a.C0, a.stats1, a.C1, b, c / cpg, cpg, a.voxels, a.eps, mean, rstd);
   const float sc = rstd * a.gamma[c];
   out[i] = make_float4(0.5f * sc, 0.5f * fmaf(-mean, sc, a.beta[c]), rstd, -mean * rstd);
 }
@@ -497,9 +386,9 @@ void launch_gnb_tile_reduce(const GnBwdArgs& a, const float* tile_part, int T, i
 }
 
 // ------------------------------------------------------------------ column sums (bias / time-embedding gradients)
-template <int MODE>
+template <Precision PR>
 __global__ void __launch_bounds__(256) colsum_kernel(ColsumArgs a, int cv, int k) {
-  constexpr bool X3 = MODE == 2;
+  constexpr bool X3 = PR == kBF16X3;
   constexpr int P = X3 ? 2 : 1;
   constexpr int UNROLL = 4;
   __shared__ float red[256 * VEC];
@@ -526,8 +415,7 @@ __global__ void __launch_bounds__(256) colsum_kernel(ColsumArgs a, int cv, int k
 #pragma unroll
     for (int u = 0; u < UNROLL; ++u) {
       float x[VEC];
-      unpack8(r[u], x);
-      if constexpr (X3) add8(rl[u], x);
+      decode_vec<PR>(r[u], rl[X3 ? u : 0], x);
 #pragma unroll
       for (int j = 0; j < VEC; ++j) s1[j] += x[j];
     }
@@ -584,20 +472,14 @@ void launch_colsum(const ColsumArgs& a, int B, cudaStream_t s) {
   if (cv < 1 || cv > 256 || a.C % VEC != 0) throw std::runtime_error("mdb: unsupported channel count in colsum");
   const int k = 256 / cv;
   const int gx = blocks_x(a.voxels, k, B, 4 * 132);
-  if (a.x3) colsum_kernel<2><<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
-  else colsum_kernel<0><<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
+  if (a.prec == kBF16X3) colsum_kernel<kBF16X3><<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
+  else colsum_kernel<kBF16><<<dim3(gx, B), cv * k, 0, s>>>(a, cv, k);
   MDB_LAUNCH_CHECK();
   colsum_final_kernel<<<(a.C + 31) / 32, dim3(32, 8), 0, s>>>(a, gx, B);
   MDB_LAUNCH_CHECK();
 }
 
 // ------------------------------------------------------------------ resampling data movement
-static inline int grid_for(long long work_items, int threads) {
-  long long b = (work_items + threads - 1) / threads;
-  const long long cap = 132LL * 8;
-  if (b > cap) b = cap;
-  return b < 1 ? 1 : (int)b;
-}
 
 __global__ void zero_stuff2x_kernel(const uint4* __restrict__ dy, uint4* __restrict__ z, int B, int R, int cv) {
   const int R2 = 2 * R;
@@ -620,9 +502,9 @@ void launch_zero_stuff2x(const void* dy, void* z, int B, int R, int C, cudaStrea
   MDB_LAUNCH_CHECK();
 }
 
-template <int MODE>
+template <Precision PR>
 __global__ void downsum2x_kernel(const uint4* __restrict__ dup, uint4* __restrict__ dx, int B, int R, int cv) {
-  constexpr bool X3 = MODE == 2;
+  constexpr bool X3 = PR == kBF16X3;
   constexpr int P = X3 ? 2 : 1;  // row = P * cv vectors (X3: cv hi vectors, then cv lo vectors)
   const int R2 = 2 * R;
   const long long total = (long long)B * R * R * R * cv;
@@ -640,33 +522,25 @@ __global__ void downsum2x_kernel(const uint4* __restrict__ dup, uint4* __restric
         for (int dxx = 0; dxx < 2; ++dxx) {
           float t[VEC];
           const uint4* sp = dup + ((((long long)r * R2 + 2 * zo + dz) * R2 + 2 * yo + dyy) * R2 + 2 * xo + dxx) * P * cv + c;
-          unpack8(__ldg(sp), t);
-          if constexpr (X3) add8(__ldg(sp + cv), t);
+          load_vec<PR>(sp, cv * 16LL, t);
 #pragma unroll
           for (int j = 0; j < VEC; ++j) acc[j] += t[j];
         }
-    if constexpr (X3) {
-      uint4* dp = dx + (i / cv) * 2 * cv + c;
-      const uint4 hv = pack8(acc);
-      dp[0] = hv;
-      dp[cv] = pack8_lo(hv, acc);
-    } else {
-      dx[i] = pack8(acc);
-    }
+    store_vec<PR>(X3 ? dx + (i / cv) * 2 * cv + c : dx + i, cv * 16LL, acc);
   }
 }
-void launch_downsum2x(const void* dup, void* dx, int B, int R, int C, cudaStream_t s, int x3) {
+void launch_downsum2x(const void* dup, void* dx, int B, int R, int C, Precision prec, cudaStream_t s) {
   const int cv = C / VEC;
   const long long total = (long long)B * R * R * R * cv;
-  if (x3) downsum2x_kernel<2><<<grid_for(total, 256), 256, 0, s>>>((const uint4*)dup, (uint4*)dx, B, R, cv);
-  else downsum2x_kernel<0><<<grid_for(total, 256), 256, 0, s>>>((const uint4*)dup, (uint4*)dx, B, R, cv);
+  if (prec == kBF16X3) downsum2x_kernel<kBF16X3><<<grid_for(total, 256), 256, 0, s>>>((const uint4*)dup, (uint4*)dx, B, R, cv);
+  else downsum2x_kernel<kBF16><<<grid_for(total, 256), 256, 0, s>>>((const uint4*)dup, (uint4*)dx, B, R, cv);
   MDB_LAUNCH_CHECK();
 }
 
 // n = hi vectors per sample; X3: vector i of the hi parts sits at (i / cv) * 2cv + i % cv, its lo vector cv further on
-template <int MODE>
+template <Precision PR>
 __global__ void batch_sum_kernel(const uint4* __restrict__ t, uint4* __restrict__ out, int B, long long n, int cv) {
-  constexpr bool X3 = MODE == 2;
+  constexpr bool X3 = PR == kBF16X3;
   constexpr int P = X3 ? 2 : 1;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const long long o = X3 ? (i / cv) * 2 * cv + i % cv : i;
@@ -676,23 +550,20 @@ __global__ void batch_sum_kernel(const uint4* __restrict__ t, uint4* __restrict_
     for (int b = 0; b < B; ++b) {
       float x[VEC];
       const uint4* sp = t + (long long)b * n * P + o;
-      unpack8(__ldg(sp), x);
-      if constexpr (X3) add8(__ldg(sp + cv), x);
+      load_vec<PR>(sp, cv * 16LL, x);
 #pragma unroll
       for (int j = 0; j < VEC; ++j) acc[j] += x[j];
     }
-    const uint4 hv = pack8(acc);
-    out[o] = hv;
-    if constexpr (X3) out[o + cv] = pack8_lo(hv, acc);
+    store_vec<PR>(out + o, cv * 16LL, acc);
   }
 }
-void launch_batch_sum(const void* t, void* out, int B, long long VC, cudaStream_t s, int C, int x3) {
+void launch_batch_sum(const void* t, void* out, int B, long long VC, int C, Precision prec, cudaStream_t s) {
   const long long n = VC / VEC;
-  if (x3) {
+  if (prec == kBF16X3) {
     if (C % VEC != 0 || C <= 0) throw std::runtime_error("mdb: split-bf16 batch_sum needs the channel count");
-    batch_sum_kernel<2><<<grid_for(n, 256), 256, 0, s>>>((const uint4*)t, (uint4*)out, B, n, C / VEC);
+    batch_sum_kernel<kBF16X3><<<grid_for(n, 256), 256, 0, s>>>((const uint4*)t, (uint4*)out, B, n, C / VEC);
   } else {
-    batch_sum_kernel<0><<<grid_for(n, 256), 256, 0, s>>>((const uint4*)t, (uint4*)out, B, n, 0);
+    batch_sum_kernel<kBF16><<<grid_for(n, 256), 256, 0, s>>>((const uint4*)t, (uint4*)out, B, n, 0);
   }
   MDB_LAUNCH_CHECK();
 }
@@ -720,9 +591,9 @@ void launch_rowsum_nc(const float* t, float* out, int B, int C, long long V, int
 }
 
 // ------------------------------------------------------------------ attention softmax backward (layers.py:604)
-template <int MODE>
+template <Precision PR>
 __global__ void __launch_bounds__(256) softmax_bwd_rows_kernel(const float* __restrict__ P, float* __restrict__ dP, long long rows, int L) {
-  constexpr bool X3 = MODE == 2;
+  constexpr bool X3 = PR == kBF16X3;
   __shared__ float red[8];
   for (long long row = blockIdx.x; row < rows; row += gridDim.x) {
     const __nv_bfloat16* p = reinterpret_cast<const __nv_bfloat16*>(P + row * L);
@@ -745,20 +616,15 @@ __global__ void __launch_bounds__(256) softmax_bwd_rows_kernel(const float* __re
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       const int i = threadIdx.x + j * 256;
-      if (i < L) {
-        const float ds = pv[j] * (dv[j] - dot);
-        const __nv_bfloat16 hb = __float2bfloat16(ds);
-        reinterpret_cast<__nv_bfloat16*>(d)[i] = hb;
-        if (X3) reinterpret_cast<__nv_bfloat16*>(d)[L + i] = __float2bfloat16(ds - __bfloat162float(hb));
-      }
+      if (i < L) store_split<PR>(reinterpret_cast<__nv_bfloat16*>(d) + i, L, pv[j] * (dv[j] - dot));
     }
   }
 }
-void launch_softmax_bwd_rows(const float* P, float* dP, long long rows, int L, cudaStream_t s, int x3) {
+void launch_softmax_bwd_rows(const float* P, float* dP, long long rows, int L, Precision prec, cudaStream_t s) {
   if (L > 16 * 256) throw std::runtime_error("mdb: softmax row too long");
   const int grid = (int)(rows < 132LL * 16 ? rows : 132LL * 16);
-  if (x3) softmax_bwd_rows_kernel<2><<<grid, 256, 0, s>>>(P, dP, rows, L);
-  else softmax_bwd_rows_kernel<0><<<grid, 256, 0, s>>>(P, dP, rows, L);
+  if (prec == kBF16X3) softmax_bwd_rows_kernel<kBF16X3><<<grid, 256, 0, s>>>(P, dP, rows, L);
+  else softmax_bwd_rows_kernel<kBF16><<<grid, 256, 0, s>>>(P, dP, rows, L);
   MDB_LAUNCH_CHECK();
 }
 
@@ -798,8 +664,6 @@ void launch_dense_bwd_input(const float* dy, long long dy_ld, const float* W, fl
   MDB_LAUNCH_CHECK();
 }
 
-__device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + __expf(-x)); }
-
 // One block per sample. Recomputes emb -> t1 -> h1 -> t2 (elementwise.cu temb_kernel), then
 // dt2 = dact * silu'(t2), dh1 = W1^T dt2, dt1 = dh1 * silu'(t1).
 __global__ void temb_bwd_kernel(const float* __restrict__ labels, const float* __restrict__ w0, const float* __restrict__ b0,
@@ -827,7 +691,7 @@ __global__ void temb_bwd_kernel(const float* __restrict__ labels, const float* _
     float acc = b0[n];
     for (int k = 0; k < nf; ++k) acc += w0[(long long)n * nf + k] * emb[k];
     t1[n] = acc;
-    const float sg = sigmoid_f(acc);
+    const float sg = sigmoid_expf(acc);
     h1[n] = acc * sg;
     h1o[(long long)b * H + n] = h1[n];
   }
@@ -835,7 +699,7 @@ __global__ void temb_bwd_kernel(const float* __restrict__ labels, const float* _
   for (int n = threadIdx.x; n < H; n += blockDim.x) {
     float acc = b1[n];
     for (int k = 0; k < H; ++k) acc += w1[(long long)n * H + k] * h1[k];
-    const float sg = sigmoid_f(acc);
+    const float sg = sigmoid_expf(acc);
     const float d = dact[(long long)b * H + n] * sg * (1.f + acc * (1.f - sg));
     d2[n] = d;
     dt2[(long long)b * H + n] = d;
@@ -844,7 +708,7 @@ __global__ void temb_bwd_kernel(const float* __restrict__ labels, const float* _
   for (int k = threadIdx.x; k < H; k += blockDim.x) {
     float acc = 0.f;
     for (int n = 0; n < H; ++n) acc = fmaf(d2[n], __ldg(w1 + (long long)n * H + k), acc);
-    const float sg = sigmoid_f(t1[k]);
+    const float sg = sigmoid_expf(t1[k]);
     dt1[(long long)b * H + k] = acc * sg * (1.f + t1[k] * (1.f - sg));
   }
 }

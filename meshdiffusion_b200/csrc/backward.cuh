@@ -3,13 +3,11 @@
 // column sums, the data movement of Down/Upsample backward, attention softmax backward and the time-embedding MLP.
 // Every reduction is staged (per-thread -> per-block partial -> fixed-order final sum): gradients are bitwise
 // reproducible run to run.
-// Activation-dtype tensors are bf16, or with `x3` set split bf16 (gemm_host.h, Precision::kBF16X3): a row of logical
+// Activation-dtype tensors are bf16 or split bf16 (Precision kBF16 / kBF16X3, act_format.cuh): a row of logical
 // pitch ld holds the hi parts of its channels at [0, ld) and their lo parts at [ld, 2 ld). Pointers and pitches passed
 // here stay logical; the kernels decode hi + lo, compute in fp32 and store (hi, lo) again.
 #pragma once
-#include <cuda_runtime.h>
-#include <cuda_bf16.h>
-#include <stdint.h>
+#include "act_format.cuh"
 
 namespace mdb {
 
@@ -30,7 +28,7 @@ struct GnBwdArgs {
   const float* gamma; const float* beta;
   const void* da;          // [B][V][C] dense, activation dtype; OVERWRITTEN with dy by pass 1 (pass 2 reads dy from it)
   long long voxels; int silu; int groups; float eps;
-  // dropout that followed the activation in the forward pass (keep iff hash16(seed, element) >= drop_thresh)
+  // dropout that followed the activation in the forward pass (act_format.cuh: apply_dropout)
   int drop_thresh; float drop_scale; unsigned long long seed;
   // pass 1 output / pass 2 input
   float* part;             // [gx][B][C][2] block partials (scratch)
@@ -42,7 +40,7 @@ struct GnBwdArgs {
   const void* add1; long long add1_ld;
   // optional by-product of pass 2: cs_per[b][c] = sum_v dx[b][v][c] (cs_part: [rows][C] block partials)
   float* cs_part; float* cs_per;
-  int x3;                  // x0 / x1 / da / dx / add0 / add1 are split bf16
+  Precision prec;          // of x0 / x1 / da / dx / add0 / add1: kBF16 or kBF16X3
 };
 void launch_gn_bwd_reduce(const GnBwdArgs& a, int B, cudaStream_t s);  // part -> sums -> dgamma/dbeta
 void launch_gn_bwd_apply(const GnBwdArgs& a, int B, cudaStream_t s);
@@ -62,7 +60,7 @@ struct ColsumArgs {
   float* per; long long per_ld;
   float* total0; float* total1; float* total2; int accumulate;
   const float* from_per; long long from_ld;  // per-sample sums already computed by the producing kernel ([B][from_ld])
-  int x3;                     // t is split bf16
+  Precision prec;             // of t: kBF16 or kBF16X3
 };
 void launch_colsum(const ColsumArgs& a, int B, cudaStream_t s);
 
@@ -70,16 +68,16 @@ void launch_colsum(const ColsumArgs& a, int B, cudaStream_t s);
 // Moves whole rows, so a split-bf16 tensor is passed as 2C channels.
 void launch_zero_stuff2x(const void* dy, void* z, int B, int R, int C, cudaStream_t s);
 // Upsample backward: dx[b][i][c] = sum over the 2x2x2 block of d_up (R = extents of dx).
-void launch_downsum2x(const void* dup, void* dx, int B, int R, int C, cudaStream_t s, int x3 = 0);
-// out[v][c] = sum_b t[b][v][c]  (bf16; x3: split bf16 rows of C channels)
-void launch_batch_sum(const void* t, void* out, int B, long long VC, cudaStream_t s, int C = 0, int x3 = 0);
+void launch_downsum2x(const void* dup, void* dx, int B, int R, int C, Precision prec, cudaStream_t s);
+// out[v][c] = sum_b t[b][v][c]  (VC = voxels x C; split bf16: rows of C channels)
+void launch_batch_sum(const void* t, void* out, int B, long long VC, int C, Precision prec, cudaStream_t s);
 // out[c] (+)= sum_{b,v} t[b][c][v]  (fp32 NCDHW, e.g. the head bias gradient)
 void launch_rowsum_nc(const float* t, float* out, int B, int C, long long V, int accumulate, cudaStream_t s);
 
 // Attention softmax backward, in place: row r holds dP (fp32, L values); P holds the probabilities written by the
-// forward softmax (bf16 at the start of rows of L fp32 slots; x3: L hi parts followed by L lo parts, filling the slots).
+// forward softmax (bf16 at the start of rows of L fp32 slots; split bf16: L hi parts followed by L lo parts, filling the slots).
 // Writes dS = P*(dP - sum(P*dP)) in the same convention over each dP row.
-void launch_softmax_bwd_rows(const float* P, float* dP, long long rows, int L, cudaStream_t s, int x3 = 0);
+void launch_softmax_bwd_rows(const float* P, float* dP, long long rows, int L, Precision prec, cudaStream_t s);
 
 // dW[n][k] (+)= sum_b dy[b][n] x[b][k];  db[n] (+)= sum_b dy[b][n]      (fp32, small)
 void launch_outer_sum(const float* dy, long long dy_ld, const float* x, long long x_ld, float* dW, float* db, int B, int N, int K,
@@ -90,13 +88,5 @@ void launch_dense_bwd_input(const float* dy, long long dy_ld, const float* W, fl
 // dt2, h1 [B][4nf] and dt1 [B][4nf], emb [B][nf] for the outer-product weight gradients.
 void launch_temb_bwd(const float* labels, const float* w0, const float* b0, const float* w1, const float* b1, const float* dact,
                      float* dt2, float* h1, float* dt1, float* emb, int B, int nf, cudaStream_t s);
-
-// 16-bit dropout hash shared by the forward GroupNorm-apply kernel and its backward
-__device__ __forceinline__ unsigned long long drop_hash64(unsigned long long seed, unsigned long long idx) {
-  unsigned long long z = idx + seed * 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
 
 }  // namespace mdb

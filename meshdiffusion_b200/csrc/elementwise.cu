@@ -1,5 +1,4 @@
 #include "elementwise.cuh"
-#include "backward.cuh"
 #include "gn_stats.cuh"
 #include <curand_kernel.h>
 #include <stdexcept>
@@ -7,100 +6,25 @@
 
 namespace mdb {
 
-#define MDB_LAUNCH_CHECK()                                                                              \
-  do {                                                                                                  \
-    cudaError_t _e = cudaGetLastError();                                                                \
-    if (_e != cudaSuccess) throw std::runtime_error(std::string("mdb launch: ") + cudaGetErrorString(_e)); \
-  } while (0)
-
-static inline int grid_for(long long work_items, int threads) {
-  long long b = (work_items + threads - 1) / threads;
-  const long long cap = 132LL * 8;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (int)b;
-}
-
-__device__ __forceinline__ float round_tf32_rna(float x) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-  return __uint_as_float(u);
-}
-// x * sigmoid(x) = x / (1 + 2^(-x log2 e)) in five instructions: ex2.approx + rcp.approx (each ~1 ulp; the IEEE division and
-// __frcp_rn expand to a MUFU plus Newton steps -- ncu showed the bf16x3 GroupNorm pass issue-bound at 32 instructions per
-// element with them, profiles/r02_ncu_norm_act_x3.txt)
-__device__ __forceinline__ float silu_f(float x) {
-  float e, r;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * -1.4426950408889634f));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.f + e));
-  return x * r;
-}
-// x*sigmoid(x) = 0.5x(1 + tanh(x/2)) with the single-MUFU tanh.approx (rel. error 2^-11: below bf16 resolution);
-// halves the MUFU pressure of the bf16 GroupNorm+SiLU pass, which otherwise co-limits with HBM bandwidth.
-__device__ __forceinline__ float silu_fast(float x) {
-  float t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
-  const float h = 0.5f * x;
-  return fmaf(h, t, h);
-}
-
-// ------------------------------------------------------------------ GroupNorm finalize
-// nn.GroupNorm(32, C, eps=1e-6) statistics (layers.py:589,652,660; ddpm_res64.py:120): biased variance over
-// (C/32) channels x voxels. Channel sums arrive from the producing GEMM's epilogue as split fixed-point integer pairs (gn_stats.cuh)
-// (integer atomics commute, so the statistics -- and with them the whole forward pass -- are bitwise reproducible).
-__global__ void gn_finalize_kernel(GnFinalizeArgs a) {
-  const int b = blockIdx.x;
-  const int C = a.C0 + a.C1;
-  const int cpg = C / a.groups;
-  for (int g = threadIdx.x; g < a.groups; g += blockDim.x) {
-    StatAcc acc;
-    for (int i = 0; i < cpg; ++i) {
-      const int c = g * cpg + i;
-      acc.add((c < a.C0) ? a.stats0 + ((long long)b * a.C0 + c) * kStatWords
-                         : a.stats1 + ((long long)b * a.C1 + (c - a.C0)) * kStatWords);
-    }
-    const double s = acc.sum(), ss = acc.sumsq();
-    const double n = a.count_per_channel * cpg;
-    const double mean = s / n;
-    double var = ss / n - mean * mean;
-    if (var < 0) var = 0;
-    const float rstd = (float)(1.0 / sqrt(var + (double)a.eps));
-    for (int i = 0; i < cpg; ++i) {
-      const int c = g * cpg + i;
-      const float sc = a.gamma[c] * rstd;
-      a.scale[(long long)b * C + c] = sc;
-      a.shift[(long long)b * C + c] = a.beta[c] - (float)mean * sc;
-    }
-  }
-}
-void launch_gn_finalize(const GnFinalizeArgs& a, int B, cudaStream_t s) {
-  gn_finalize_kernel<<<B, 32, 0, s>>>(a);
-  MDB_LAUNCH_CHECK();
-}
-
 // ------------------------------------------------------------------ GroupNorm apply (+SiLU), concat-aware
 // blockIdx.y = sample. Every thread owns ONE 16-byte channel vector for the whole kernel (block = k voxels x C/VEC
 // vectors): its scale/shift live in registers, its source pointer is selected once, and the loop body is
 // load -> fma -> silu -> store with 4 voxels in flight. No div/mod or table lookups in the loop: the kernel is
 // HBM-bound instead of issue-bound.
-// MODE: 0 = bf16, 1 = tf32 (fp32 storage), 2 = split bf16 (X3: a channel vector is a 16-byte hi part and a 16-byte lo
-// part one logical row apart, on the input as on the output)
-template <int MODE>
-__global__ void __launch_bounds__(256, MODE == 1 ? 4 : 3) norm_act_kernel(NormActArgs a, int cv, int k) {
-  constexpr bool TF32 = MODE == 1;
-  constexpr bool X3 = MODE == 2;
-  constexpr int VEC = TF32 ? 4 : 8;  // 16 bytes
+// X3: a channel vector is a 16-byte hi part and a 16-byte lo part one logical row apart, on the input as on the output.
+// GroupNorm finalize is fused into the prologue: each thread derives mean / rstd of the group(s) of ITS channels from the
+// per-channel sums the producing GEMM left behind (cpg channels x 2 values, L2-resident) -- 80 fewer launches.
+template <Precision P>
+__global__ void __launch_bounds__(256, P == kTF32 ? 4 : 3) norm_act_kernel(NormActArgs a, int cv, int k) {
+  constexpr int VEC = kVecElems<P>;  // 16 bytes
   constexpr int UNROLL = 4;
   const int C = a.C0 + a.C1;
   const int b = blockIdx.y;
   const int cvi = threadIdx.x % cv, vl = threadIdx.x / cv;
   const int c = cvi * VEC;
   float sc[VEC], sh[VEC];
-  if (a.stats0) {
-    // GroupNorm finalize fused into the prologue: each thread derives mean / rstd of the group(s) of ITS channels from
-    // the per-channel sums the producing GEMM left behind (cpg channels x 2 values, L2-resident) -- 80 fewer launches
+  {
     const int cpg = C / a.groups;
-    const double n = (double)a.voxels * cpg;
     int cur_g = -1;
     float mean = 0.f, rstd = 0.f;
 #pragma unroll
@@ -108,30 +32,14 @@ __global__ void __launch_bounds__(256, MODE == 1 ? 4 : 3) norm_act_kernel(NormAc
       const int ch = c + j, g = ch / cpg;
       if (g != cur_g) {
         cur_g = g;
-        StatAcc acc;
-        for (int i = 0; i < cpg; ++i) {
-          const int cc = g * cpg + i;
-          acc.add((cc < a.C0) ? a.stats0 + ((long long)b * a.C0 + cc) * kStatWords
-                              : a.stats1 + ((long long)b * a.C1 + (cc - a.C0)) * kStatWords);
-        }
-        const double m = acc.sum() / n;
-        double var = acc.sumsq() / n - m * m;
-        if (var < 0) var = 0;
-        mean = (float)m;
-        rstd = (float)(1.0 / sqrt(var + (double)a.eps));
+        gn_group_stats(a.stats0, a.C0, a.stats1, a.C1, b, g, cpg, a.voxels, a.eps, mean, rstd);
       }
       sc[j] = a.gamma[ch] * rstd;
       sh[j] = a.beta[ch] - mean * sc[j];
     }
-  } else {
-#pragma unroll
-    for (int j = 0; j < VEC; ++j) {
-      sc[j] = a.scale[(long long)b * C + c + j];
-      sh[j] = a.shift[(long long)b * C + c + j];
-    }
   }
-  const int es = TF32 ? 4 : 2;
-  constexpr int PARTS = X3 ? 2 : 1;
+  const int es = esize(P);
+  constexpr int PARTS = P == kBF16X3 ? 2 : 1;
   const bool first = c < a.C0;
   const char* src = first ? (const char*)a.x0 + ((long long)b * a.voxels * a.ld0 * PARTS + c) * es
                           : (const char*)a.x1 + ((long long)b * a.voxels * a.ld1 * PARTS + (c - a.C0)) * es;
@@ -142,13 +50,13 @@ __global__ void __launch_bounds__(256, MODE == 1 ? 4 : 3) norm_act_kernel(NormAc
   const long long dst_lo = (long long)C * es;
   const long long step = (long long)gridDim.x * k;
   for (long long v0 = (long long)blockIdx.x * k + vl; v0 < a.voxels; v0 += step * UNROLL) {
-    uint4 raw[UNROLL], rawl[X3 ? UNROLL : 1];
+    uint4 raw[UNROLL], rawl[UNROLL];
 #pragma unroll
     for (int u = 0; u < UNROLL; ++u) {
       const long long v = v0 + u * step;
       if (v < a.voxels) {
         raw[u] = __ldg((const uint4*)(src + v * src_stride));
-        if constexpr (X3) rawl[u] = __ldg((const uint4*)(src + v * src_stride + src_lo));
+        if constexpr (P == kBF16X3) rawl[u] = __ldg((const uint4*)(src + v * src_stride + src_lo));
       }
     }
 #pragma unroll
@@ -156,62 +64,22 @@ __global__ void __launch_bounds__(256, MODE == 1 ? 4 : 3) norm_act_kernel(NormAc
       const long long v = v0 + u * step;
       if (v >= a.voxels) continue;
       float x[VEC];
-      if (TF32) {
-        const float* f = (const float*)&raw[u];
-#pragma unroll
-        for (int j = 0; j < VEC; ++j) x[j] = f[j];
-      } else {
-        const __nv_bfloat162* h = (const __nv_bfloat162*)&raw[u];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { float2 f = __bfloat1622float2(h[j]); x[2 * j] = f.x; x[2 * j + 1] = f.y; }
-        if constexpr (X3) {
-          const __nv_bfloat162* l = (const __nv_bfloat162*)&rawl[u];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) { float2 f = __bfloat1622float2(l[j]); x[2 * j] += f.x; x[2 * j + 1] += f.y; }
-        }
-      }
+      decode_vec<P>(raw[u], rawl[u], x);
 #pragma unroll
       for (int j = 0; j < VEC; ++j) {
         float y = fmaf(x[j], sc[j], sh[j]);
-        if (a.silu) y = MODE == 0 ? silu_fast(y) : silu_f(y);
+        if (a.silu) y = P == kBF16 ? silu_tanh(y) : silu_ex2(y);
         x[j] = y;
       }
-      // dropout (training engines; bf16 and split bf16): same hash and element index as the GroupNorm backward kernels and
-      // the GNB epilogue, so all three agree on the mask
-      if (MODE != 1 && a.drop_thresh > 0) {
-        const unsigned long long e4 = (unsigned long long)((((long long)b * a.voxels + v) * C + c) >> 2);
-        const unsigned long long h0 = drop_hash64(a.seed, e4), h1 = drop_hash64(a.seed, e4 + 1);
-#pragma unroll
-        for (int j = 0; j < VEC; ++j) {
-          const unsigned r16 = (unsigned)(((j < 4 ? h0 : h1) >> (16 * (j & 3))) & 0xFFFFu);
-          x[j] = r16 >= (unsigned)a.drop_thresh ? x[j] * a.drop_scale : 0.f;
-        }
-      }
-      if (TF32) {
-        *((float4*)(dst + v * dst_stride)) =
-            make_float4(round_tf32_rna(x[0]), round_tf32_rna(x[1]), round_tf32_rna(x[2]), round_tf32_rna(x[3]));
-      } else {
-        uint4 t;
-        __nv_bfloat162* h = (__nv_bfloat162*)&t;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) h[j] = __floats2bfloat162_rn(x[2 * j], x[2 * j + 1]);
-        *((uint4*)(dst + v * dst_stride)) = t;
-        if constexpr (X3) {
-          uint4 tl;
-          __nv_bfloat162* l = (__nv_bfloat162*)&tl;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float2 f = __bfloat1622float2(h[j]);
-            l[j] = __floats2bfloat162_rn(x[2 * j] - f.x, x[2 * j + 1] - f.y);
-          }
-          *((uint4*)(dst + v * dst_stride + dst_lo)) = tl;
-        }
-      }
+      if (P != kTF32 && a.drop_thresh > 0)  // training engines (bf16 and split bf16)
+        apply_dropout<VEC / 4>(x, a.seed, (unsigned long long)((((long long)b * a.voxels + v) * C + c) >> 2), a.drop_thresh,
+                               a.drop_scale);
+      store_vec<P>(dst + v * dst_stride, dst_lo, x);
     }
   }
 }
 void launch_norm_act(const NormActArgs& a, int B, cudaStream_t s) {
-  const int vec = a.tf32 == 1 ? 4 : 8;
+  const int vec = a.prec == kTF32 ? 4 : 8;
   const int C = a.C0 + a.C1;
   const int cv = C / vec;
   if (cv > 256 || cv < 1 || a.C0 % vec != 0) throw std::runtime_error("mdb: unsupported channel count in norm_act");
@@ -222,9 +90,9 @@ void launch_norm_act(const NormActArgs& a, int B, cudaStream_t s) {
   if (gx > cap) gx = cap;
   if (gx < 1) gx = 1;
   dim3 grid((unsigned)gx, (unsigned)B);
-  if (a.tf32 == 1) norm_act_kernel<1><<<grid, threads, 0, s>>>(a, cv, k);
-  else if (a.tf32 == 2) norm_act_kernel<2><<<grid, threads, 0, s>>>(a, cv, k);
-  else norm_act_kernel<0><<<grid, threads, 0, s>>>(a, cv, k);
+  if (a.prec == kTF32) norm_act_kernel<kTF32><<<grid, threads, 0, s>>>(a, cv, k);
+  else if (a.prec == kBF16X3) norm_act_kernel<kBF16X3><<<grid, threads, 0, s>>>(a, cv, k);
+  else norm_act_kernel<kBF16><<<grid, threads, 0, s>>>(a, cv, k);
   MDB_LAUNCH_CHECK();
 }
 
@@ -241,8 +109,8 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict
     y[i] = __ldg(x + src);
   }
 }
-void launch_upsample2x(const void* x, void* y, int B, int Z, int Y, int X, int C, int tf32, cudaStream_t s) {
-  const int cv = C / (tf32 ? 4 : 8);
+void launch_upsample2x(const void* x, void* y, int B, int Z, int Y, int X, int C, int elem_bytes, cudaStream_t s) {
+  const int cv = C * elem_bytes / 16;
   const long long total = (long long)B * 8 * Z * Y * X * cv;
   upsample2x_kernel<<<grid_for(total, 256), 256, 0, s>>>((const uint4*)x, (uint4*)y, B, Z, Y, X, cv);
   MDB_LAUNCH_CHECK();
@@ -253,11 +121,9 @@ void launch_upsample2x(const void* x, void* y, int B, int Z, int Y, int X, int C
 // (a warp per row, no per-element div/mod), then every thread emits 16-byte vectors of the [voxel][Kpad] operand
 // matrix (column = cin*k^3 + tap) through a per-column slab-offset table.
 constexpr int kIm2colYB = 4;
-template <int MODE>  // 0 bf16, 1 tf32, 2 split bf16 (row = [Kpad hi | Kpad lo])
+template <Precision P>  // split bf16: row = [Kpad hi | Kpad lo]
 __global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ x, void* __restrict__ a, int Cin, int R, int k, int Kpad) {
-  constexpr bool TF32 = MODE == 1;
-  constexpr bool X3 = MODE == 2;
-  constexpr int VEC = TF32 ? 4 : 8;
+  constexpr int VEC = kVecElems<P>;
   constexpr int YB = kIm2colYB;
   extern __shared__ float slab[];  // [Cin][k][k+YB-1][R + 2*pad]
   const int pad = k / 2, W = R + 2 * pad, T = k * k * k, KH = k + YB - 1;
@@ -299,55 +165,33 @@ __global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ x
         const int off = coloff[col0 + j];
         v[j] = off >= 0 ? slab[off + ybase + xo] : 0.f;
       }
-      if (TF32) {
-        *((float4*)((float*)a + (row0 + xo) * Kpad + col0)) =
-            make_float4(round_tf32_rna(v[0]), round_tf32_rna(v[1]), round_tf32_rna(v[2]), round_tf32_rna(v[3]));
-      } else {
-        uint4 t;
-        __nv_bfloat162* h = (__nv_bfloat162*)&t;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) h[j] = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-        if constexpr (X3) {
-          uint4 tl;
-          __nv_bfloat162* l = (__nv_bfloat162*)&tl;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float2 f = __bfloat1622float2(h[j]);
-            l[j] = __floats2bfloat162_rn(v[2 * j] - f.x, v[2 * j + 1] - f.y);
-          }
-          *((uint4*)((__nv_bfloat16*)a + (row0 + xo) * 2 * Kpad + col0)) = t;
-          *((uint4*)((__nv_bfloat16*)a + (row0 + xo) * 2 * Kpad + Kpad + col0)) = tl;
-        } else {
-          *((uint4*)((__nv_bfloat16*)a + (row0 + xo) * Kpad + col0)) = t;
-        }
-      }
+      store_vec<P>((char*)a + ((row0 + xo) * parts(P) * Kpad + col0) * esize(P), (long long)Kpad * esize(P), v);
     }
   }
 }
-void launch_im2col(const float* x, void* a, int B, int Cin, int R, int k, int Kpad, int tf32, cudaStream_t s) {
+void launch_im2col(const float* x, void* a, int B, int Cin, int R, int k, int Kpad, Precision prec, cudaStream_t s) {
   if (R % kIm2colYB != 0) throw std::runtime_error("mdb: im2col needs a grid size divisible by 4");
   const size_t smem = (size_t)Cin * k * (k + kIm2colYB - 1) * (R + 2 * (k / 2)) * sizeof(float) + (size_t)Kpad * sizeof(int);
   static bool configured[64] = {};  // per device
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev >= 64 || !configured[dev]) {
-    cudaFuncSetAttribute(im2col_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    cudaFuncSetAttribute(im2col_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    cudaFuncSetAttribute(im2col_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+    cudaFuncSetAttribute(im2col_kernel<kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+    cudaFuncSetAttribute(im2col_kernel<kTF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+    cudaFuncSetAttribute(im2col_kernel<kBF16X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
     if (dev < 64) configured[dev] = true;
   }
   if (smem > 100 * 1024) throw std::runtime_error("mdb: im2col slab too large");
   const unsigned grid = (unsigned)(B * R * (R / kIm2colYB));
-  if (tf32 == 1) im2col_kernel<1><<<grid, 256, smem, s>>>(x, a, Cin, R, k, Kpad);
-  else if (tf32 == 2) im2col_kernel<2><<<grid, 256, smem, s>>>(x, a, Cin, R, k, Kpad);
-  else im2col_kernel<0><<<grid, 256, smem, s>>>(x, a, Cin, R, k, Kpad);
+  if (prec == kTF32) im2col_kernel<kTF32><<<grid, 256, smem, s>>>(x, a, Cin, R, k, Kpad);
+  else if (prec == kBF16X3) im2col_kernel<kBF16X3><<<grid, 256, smem, s>>>(x, a, Cin, R, k, Kpad);
+  else im2col_kernel<kBF16><<<grid, 256, smem, s>>>(x, a, Cin, R, k, Kpad);
   MDB_LAUNCH_CHECK();
 }
 
 // ------------------------------------------------------------------ row softmax (layers.py:604)
-template <int MODE>  // 0 bf16, 1 tf32, 2 split bf16: hi parts in the first L bf16 of the row, lo parts in the next L
+template <Precision P>  // split bf16: hi parts in the first L bf16 of the row, lo parts in the next L
 __global__ void softmax_rows_kernel(float* __restrict__ s, long long rows, int L) {
-  constexpr bool TF32 = MODE == 1;
   __shared__ float red[32];
   for (long long row = blockIdx.x; row < rows; row += gridDim.x) {
     float* p = s + row * L;
@@ -379,23 +223,18 @@ __global__ void softmax_rows_kernel(float* __restrict__ s, long long rows, int L
     for (int j = 0; j < 16; ++j) {
       const int i = threadIdx.x + j * 256;
       if (i < L) {
-        if (TF32) p[i] = round_tf32_rna(vals[j] * inv);
-        else {
-          const float pv = vals[j] * inv;
-          const __nv_bfloat16 hb = __float2bfloat16(pv);
-          ((__nv_bfloat16*)p)[i] = hb;
-          if (MODE == 2) ((__nv_bfloat16*)p)[L + i] = __float2bfloat16(pv - __bfloat162float(hb));
-        }
+        if constexpr (P == kTF32) p[i] = to_tf32_rna(vals[j] * inv);
+        else store_split<P>((__nv_bfloat16*)p + i, L, vals[j] * inv);
       }
     }
   }
 }
-void launch_softmax_rows(float* s, long long rows, int L, int tf32, cudaStream_t st) {
+void launch_softmax_rows(float* s, long long rows, int L, Precision prec, cudaStream_t st) {
   if (L > 16 * 256) throw std::runtime_error("mdb: softmax row too long");
   const int grid = (int)(rows < 132LL * 16 ? rows : 132LL * 16);
-  if (tf32 == 1) softmax_rows_kernel<1><<<grid, 256, 0, st>>>(s, rows, L);
-  else if (tf32 == 2) softmax_rows_kernel<2><<<grid, 256, 0, st>>>(s, rows, L);
-  else softmax_rows_kernel<0><<<grid, 256, 0, st>>>(s, rows, L);
+  if (prec == kTF32) softmax_rows_kernel<kTF32><<<grid, 256, 0, st>>>(s, rows, L);
+  else if (prec == kBF16X3) softmax_rows_kernel<kBF16X3><<<grid, 256, 0, st>>>(s, rows, L);
+  else softmax_rows_kernel<kBF16><<<grid, 256, 0, st>>>(s, rows, L);
   MDB_LAUNCH_CHECK();
 }
 
@@ -441,17 +280,17 @@ __global__ void __launch_bounds__(256) transpose_vc_bf16x2_kernel(const __nv_bfl
   }
 }
 
-void launch_transpose_vc(const void* in, long long ld, int c0, void* out, int B, int V, int C, int tf32, cudaStream_t s,
+void launch_transpose_vc(const void* in, long long ld, int c0, void* out, int B, int V, int C, int elem_bytes, cudaStream_t s,
                          long long ld_out) {
   const long long ldo = ld_out ? ld_out : V;
-  if (!tf32 && V % 64 == 0 && C % 64 == 0 && ld % 2 == 0 && c0 % 2 == 0 && ldo % 2 == 0) {
+  if (elem_bytes == 2 && V % 64 == 0 && C % 64 == 0 && ld % 2 == 0 && c0 % 2 == 0 && ldo % 2 == 0) {
     dim3 grid(V / 64, C / 64, B), block(32, 8);
     transpose_vc_bf16x2_kernel<<<grid, block, 0, s>>>((const __nv_bfloat16*)in, ld, c0, (__nv_bfloat16*)out, V, C, ldo);
     MDB_LAUNCH_CHECK();
     return;
   }
   dim3 grid((V + 31) / 32, (C + 31) / 32, B), block(32, 8);
-  if (tf32) transpose_vc_kernel<float><<<grid, block, 0, s>>>((const float*)in, ld, c0, (float*)out, V, C, ldo);
+  if (elem_bytes == 4) transpose_vc_kernel<float><<<grid, block, 0, s>>>((const float*)in, ld, c0, (float*)out, V, C, ldo);
   else transpose_vc_kernel<__nv_bfloat16><<<grid, block, 0, s>>>((const __nv_bfloat16*)in, ld, c0, (__nv_bfloat16*)out, V, C, ldo);
   MDB_LAUNCH_CHECK();
 }
@@ -480,13 +319,13 @@ __global__ void temb_kernel(const float* __restrict__ labels, const float* __res
   for (int n = threadIdx.x; n < H; n += blockDim.x) {
     float acc = b0[n];
     for (int k = 0; k < nf; ++k) acc += w0[(long long)n * nf + k] * emb[k];
-    h1[n] = silu_f(acc);
+    h1[n] = silu_ex2(acc);
   }
   __syncthreads();
   for (int n = threadIdx.x; n < H; n += blockDim.x) {
     float acc = b1[n];
     for (int k = 0; k < H; ++k) acc += w1[(long long)n * H + k] * h1[k];
-    out[(long long)b * H + n] = silu_f(acc);
+    out[(long long)b * H + n] = silu_ex2(acc);
   }
 }
 void launch_temb(const float* labels, const float* w0, const float* b0, const float* w1, const float* b1, float* out,
@@ -560,9 +399,9 @@ void launch_tap_shift_sum(const void* P, long long ldp, int p_fp32, const float*
 // blockIdx.y = sample, blockIdx.x = chunk of voxels; thread = output channel (coalesced rows). Each thread owns a
 // channel for its chunk, so its statistics are accumulated in a fixed order (deterministic) and published with one
 // integer atomic per (block, channel).
-template <int MODE>  // 0 bf16, 1 tf32, 2 split bf16 (out / res rows are [N hi | N lo])
+template <Precision P>  // split bf16: out / res rows are [N hi | N lo]
 __global__ void __launch_bounds__(256) split_reduce_kernel(SplitReduceArgs a, int vchunk) {
-  constexpr bool TF32 = MODE == 1;
+  constexpr bool TF32 = P == kTF32;
   const int b = blockIdx.y;
   const long long v0 = (long long)blockIdx.x * vchunk;
   const long long v1 = v0 + vchunk < a.voxels ? v0 + vchunk : a.voxels;
@@ -576,7 +415,7 @@ __global__ void __launch_bounds__(256) split_reduce_kernel(SplitReduceArgs a, in
       for (int sp = 0; sp < a.splits; ++sp) acc += a.partial[sp * a.split_stride + idx];
       if (a.res) {
         const long long ridx = (long long)b * a.res_batch_stride + v * a.N + n;
-        if (MODE == 2) {
+        if constexpr (P == kBF16X3) {
           const __nv_bfloat16* rp = (const __nv_bfloat16*)a.res + 2 * ((long long)b * a.res_batch_stride + v * a.N) + n;
           acc += __bfloat162float(rp[0]) + __bfloat162float(rp[a.N]);
         } else {
@@ -584,14 +423,8 @@ __global__ void __launch_bounds__(256) split_reduce_kernel(SplitReduceArgs a, in
         }
       }
       s1 += acc; s2 += acc * acc;
-      if (TF32) ((float*)a.out)[idx] = round_tf32_rna(acc);
-      else if (MODE == 2) {
-        __nv_bfloat16* op = (__nv_bfloat16*)a.out + 2 * (idx - n) + n;
-        const __nv_bfloat16 hb = __float2bfloat16(acc);
-        op[0] = hb;
-        op[a.N] = __float2bfloat16(acc - __bfloat162float(hb));
-      }
-      else ((__nv_bfloat16*)a.out)[idx] = __float2bfloat16(acc);
+      if constexpr (TF32) ((float*)a.out)[idx] = to_tf32_rna(acc);
+      else store_split<P>((__nv_bfloat16*)a.out + parts(P) * (idx - n) + n, a.N, acc);
     }
     if (a.stats) {
       long long* dst = a.stats + ((long long)b * a.N + n) * kStatWords;
@@ -604,9 +437,9 @@ void launch_split_reduce(const SplitReduceArgs& a, int B, cudaStream_t s) {
   const int vchunk = 8;
   dim3 grid((unsigned)((a.voxels + vchunk - 1) / vchunk), (unsigned)B);
   const int threads = a.N < 256 ? ((a.N + 31) / 32) * 32 : 256;
-  if (a.tf32 == 1) split_reduce_kernel<1><<<grid, threads, 0, s>>>(a, vchunk);
-  else if (a.tf32 == 2) split_reduce_kernel<2><<<grid, threads, 0, s>>>(a, vchunk);
-  else split_reduce_kernel<0><<<grid, threads, 0, s>>>(a, vchunk);
+  if (a.prec == kTF32) split_reduce_kernel<kTF32><<<grid, threads, 0, s>>>(a, vchunk);
+  else if (a.prec == kBF16X3) split_reduce_kernel<kBF16X3><<<grid, threads, 0, s>>>(a, vchunk);
+  else split_reduce_kernel<kBF16><<<grid, threads, 0, s>>>(a, vchunk);
   MDB_LAUNCH_CHECK();
 }
 
@@ -694,16 +527,6 @@ void launch_sampler_update(const SamplerUpdateArgs& a, int B, cudaStream_t s) {
   const float one_m = 1.f - a.beta;
   const float sq1m = sqrtf(one_m), sqb = sqrtf(a.beta);
   sampler_update_kernel<<<grid_for(a.V * a.C * B, 256), 256, 0, s>>>(a, B, sq1m, sqb, a.stdv);
-  MDB_LAUNCH_CHECK();
-}
-
-__global__ void mask_mul_kernel(float* x, const float* mask, long long V, long long total) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
-    x[i] *= __ldg(mask + (i % V));
-}
-void launch_mask_mul(float* x, const float* mask, long long V, int C, int B, cudaStream_t s) {
-  const long long total = V * C * B;
-  mask_mul_kernel<<<grid_for(total, 256), 256, 0, s>>>(x, mask, V, total);
   MDB_LAUNCH_CHECK();
 }
 

@@ -2,48 +2,37 @@
 // stem im2col, attention softmax / V transpose, time-embedding MLP, ancestral-sampling update.
 // All of these are HBM-roofline kernels: 16-byte vector accesses, grid-stride loops sized to the SM count.
 #pragma once
-#include <cuda_runtime.h>
-#include <cuda_bf16.h>
-#include <stdint.h>
+#include "act_format.cuh"
 
 namespace mdb {
 
-struct GnFinalizeArgs {
-  const long long* stats0; int C0;   // [B][C0][kStatWords] split fixed-point (sum, sumsq) records (gn_stats.cuh)
-  const long long* stats1; int C1;   // optional second (concatenated) source
-  const float* gamma; const float* beta;
-  float* scale; float* shift;     // [B][C0+C1]
-  int groups; float eps; double count_per_channel;  // voxels per channel
-};
-void launch_gn_finalize(const GnFinalizeArgs& a, int B, cudaStream_t s);
-
-// y[b][v][c] = act(x[b][v][c] * scale[b][c] + shift[b][c]) over the channel concatenation of up to 2 sources.
+// y[b][v][c] = act(GroupNorm(x)[b][v][c]) over the channel concatenation of up to 2 sources, in operand mode `prec`.
 struct NormActArgs {
   const void* x0; int C0; long long ld0;
   const void* x1; int C1; long long ld1;
-  const float* scale; const float* shift;  // [B][C0+C1] (only when stats0 == nullptr: precomputed by gn_finalize)
   void* y;                                 // [B][V][C0+C1] dense
-  long long voxels; int silu; int tf32;  // tf32: storage mode 0 = bf16, 1 = fp32 (tf32 operands), 2 = split bf16 (hi | lo rows)
-  // fused GroupNorm finalize: per-channel (sum, sumsq) records of the two sources (gn_stats.cuh), affine parameters
+  long long voxels; int silu; Precision prec;
+  // per-channel (sum, sumsq) records of the two sources (gn_stats.cuh), affine parameters
   const long long* stats0; const long long* stats1;
   const float* gamma; const float* beta;
   int groups; float eps;
-  // training: nn.Dropout after the activation (layers.py:661,682): keep iff hash16(seed, element) >= drop_thresh
+  // training: nn.Dropout after the activation (act_format.cuh: apply_dropout)
   int drop_thresh; float drop_scale; unsigned long long seed;
 };
 void launch_norm_act(const NormActArgs& a, int B, cudaStream_t s);
 
-void launch_upsample2x(const void* x, void* y, int B, int Z, int Y, int X, int C, int tf32, cudaStream_t s);
+// moves whole rows: elem_bytes = 2 (bf16; a split-bf16 row is passed as 2C channels) or 4 (fp32)
+void launch_upsample2x(const void* x, void* y, int B, int Z, int Y, int X, int C, int elem_bytes, cudaStream_t s);
 
 // x fp32 NCDHW [B][Cin][R^3] -> A[b][voxel][Kpad], column = cin*k^3 + tap (tap = (kd*k+kh)*k+kw), zero padded.
-void launch_im2col(const float* x, void* a, int B, int Cin, int R, int ksize, int Kpad, int tf32, cudaStream_t s);
+void launch_im2col(const float* x, void* a, int B, int Cin, int R, int ksize, int Kpad, Precision prec, cudaStream_t s);
 
 // in-place row softmax: rows of L fp32 logits (row stride L floats); writes probabilities in the activation dtype
 // at the start of each row (bf16 rows keep the fp32 row pitch).
-void launch_softmax_rows(float* s, long long rows, int L, int tf32, cudaStream_t st);
+void launch_softmax_rows(float* s, long long rows, int L, Precision prec, cudaStream_t st);
 
-// out[b][c][v] = in[b][v][c0 + c]
-void launch_transpose_vc(const void* in, long long ld_in, int c0, void* out, int B, int V, int C, int tf32,
+// out[b][c][v] = in[b][v][c0 + c], elements of elem_bytes = 2 or 4 bytes
+void launch_transpose_vc(const void* in, long long ld_in, int c0, void* out, int B, int V, int C, int elem_bytes,
                          cudaStream_t s, long long ld_out = 0);
 
 // temb path (ddpm_res64.py:132-136 + layers.py:542-556,680): act(temb)[B][4nf]
@@ -63,7 +52,7 @@ struct SplitReduceArgs {
   const float* partial; long long split_stride; int splits;
   const float* bias; const float* rowbias; long long rowbias_ld;
   const void* res; long long res_batch_stride;  // same [V][N] layout as out (activation dtype)
-  void* out; long long* stats; long long voxels; int N; int tf32;
+  void* out; long long* stats; long long voxels; int N; Precision prec;
 };
 void launch_split_reduce(const SplitReduceArgs& a, int B, cudaStream_t s);
 
@@ -94,7 +83,5 @@ struct SamplerUpdateArgs {
   const float* cond_noise;       // z' [B][V] or null (then Philox(seed, element, offset + 2))
 };
 void launch_sampler_update(const SamplerUpdateArgs& a, int B, cudaStream_t s);
-
-void launch_mask_mul(float* x, const float* mask, long long V, int C, int B, cudaStream_t s);
 
 }  // namespace mdb

@@ -354,18 +354,12 @@ void GemmOp::set_b_activation(void* ptr, int K, int N, int batch, long long rs, 
 struct PackWSrc { const float* ptr; long long sn, sc, st; int cvalid; int ndiv; long long sn_hi; int cdiv; long long sc_hi; };
 struct PackArgs { PackWSrc w[4]; };
 
-__device__ __forceinline__ float round_tf32(float x) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-  return __uint_as_float(u);
-}
-
-// MODE: 0 = bf16, 1 = tf32 (rna), 2 = split bf16 (entry.wpart selects hi = bf16(w) or lo = bf16(w - hi)).
+// split bf16: entry.wpart selects hi = bf16(w) or lo = bf16(w - hi).
 // One thread = 8 consecutive K elements (one 16- / 32-byte store) of EVERY k-step of one load entry for one output row: the
 // entry / source / offset arithmetic is done once per 8 * nk outputs. (The first version, one thread per packed element with
 // two 64-bit divisions and a table walk each, made the per-optimiser-step re-pack of the training engine instruction-bound:
 // 6-8 ms for 2.9 GB of traffic.)
-template <int MODE>
+template <Precision P>
 __global__ void __launch_bounds__(256) pack_weights_kernel(const LoadEntry* __restrict__ loads, const int* __restrict__ load_ks0,
                                                          int n_loads, const __grid_constant__ PackArgs args, int N, int ksteps,
                                                          int KB, void* __restrict__ out) {
@@ -395,17 +389,17 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const LoadEntry* __re
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = (valid >> i) & 1u ? __ldg(w.ptr + coff[i] + toff) : 0.f;
       const long long o = obase + (long long)j * KB;
-      if (MODE == 1) {
+      if (P == kTF32) {
         float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + o);
-        op[0] = make_float4(round_tf32(v[0]), round_tf32(v[1]), round_tf32(v[2]), round_tf32(v[3]));
-        op[1] = make_float4(round_tf32(v[4]), round_tf32(v[5]), round_tf32(v[6]), round_tf32(v[7]));
+        op[0] = make_float4(to_tf32_rna(v[0]), to_tf32_rna(v[1]), to_tf32_rna(v[2]), to_tf32_rna(v[3]));
+        op[1] = make_float4(to_tf32_rna(v[4]), to_tf32_rna(v[5]), to_tf32_rna(v[6]), to_tf32_rna(v[7]));
       } else {
         uint4 pk;
         __nv_bfloat16* h = reinterpret_cast<__nv_bfloat16*>(&pk);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const __nv_bfloat16 hi = __float2bfloat16(v[i]);
-          h[i] = (MODE == 2 && e.wpart) ? __float2bfloat16(v[i] - __bfloat162float(hi)) : hi;
+          h[i] = (P == kBF16X3 && e.wpart) ? bf16_lo(v[i], hi) : hi;
         }
         *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(out) + o) = pk;
       }
@@ -431,11 +425,11 @@ void GemmOp::repack(cudaStream_t stream) {
   int blocks = (int)((total + 255) / 256);
   if (blocks > kPlanSMs * 16) blocks = kPlanSMs * 16;
   if (prec == kTF32)
-    pack_weights_kernel<1><<<blocks, 256, 0, stream>>>(d_loads, d_ks0, n_loads, args, p.N, ksteps, KB, d_wpacked);
+    pack_weights_kernel<kTF32><<<blocks, 256, 0, stream>>>(d_loads, d_ks0, n_loads, args, p.N, ksteps, KB, d_wpacked);
   else if (prec == kBF16X3)
-    pack_weights_kernel<2><<<blocks, 256, 0, stream>>>(d_loads, d_ks0, n_loads, args, p.N, ksteps, KB, d_wpacked);
+    pack_weights_kernel<kBF16X3><<<blocks, 256, 0, stream>>>(d_loads, d_ks0, n_loads, args, p.N, ksteps, KB, d_wpacked);
   else
-    pack_weights_kernel<0><<<blocks, 256, 0, stream>>>(d_loads, d_ks0, n_loads, args, p.N, ksteps, KB, d_wpacked);
+    pack_weights_kernel<kBF16><<<blocks, 256, 0, stream>>>(d_loads, d_ks0, n_loads, args, p.N, ksteps, KB, d_wpacked);
   MDB_CUDA_CHECK(cudaGetLastError());
 }
 
@@ -559,7 +553,7 @@ void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
     a.partial = p.partial; a.split_stride = p.split_stride; a.splits = p.splits;
     a.bias = p.bias; a.rowbias = p.rowbias; a.rowbias_ld = p.rowbias_ld;
     a.res = p.res; a.res_batch_stride = p.rsb;
-    a.out = p.out; a.stats = p.stats; a.voxels = (long long)p.X * p.Y * p.Z; a.N = p.N; a.tf32 = tf ? 1 : (x3 ? 2 : 0);
+    a.out = p.out; a.stats = p.stats; a.voxels = (long long)p.X * p.Y * p.Z; a.N = p.N; a.prec = prec;
     if (x3) a.res_batch_stride = p.rsb / 2;  // the reduction kernel takes logical strides
     launch_split_reduce(a, p.Bn, stream);
   }

@@ -6,6 +6,7 @@
 #include <string>
 #include <vector>
 #include <stdexcept>
+#include "act_format.cuh"
 #include "gemm_tc.cuh"
 
 namespace mdb {
@@ -18,19 +19,8 @@ namespace mdb {
                                std::to_string(__LINE__) + " (" #expr ")");                           \
   } while (0)
 
-// kBF16X3 ("split bf16"): every fp32 value v is carried as a bf16 pair hi = bf16(v), lo = bf16(v - hi) and every product
-// is evaluated as hi*hi + hi*lo + lo*hi into the same fp32 accumulator (three bf16 MMAs per k-step; the
-// dropped lo*lo term is 2^-16 relative) -- fp32-class results (the mode that meets the 1e-3 parity contract) at
-// one third of the bf16 tensor rate. An X3 tensor with a logical row pitch of `ld` channels occupies 2*ld bf16 per
-// voxel: hi parts at [0, ld), lo parts at [ld, 2*ld). All pitches handed to GemmOp / Act stay LOGICAL.
-enum Precision { kBF16 = 0, kTF32 = 1, kBF16X3 = 2 };
-inline int esize(Precision p) { return p == kTF32 ? 4 : 2; }
+// K elements per k-step of operand mode p (Precision and the row format: act_format.cuh)
 inline int kb_elems(Precision p) { return kRowBytes / esize(p); }
-inline int parts(Precision p) { return p == kBF16X3 ? 2 : 1; }
-inline Precision precision_from_int(int v) {
-  if (v < 0 || v > 2) throw std::runtime_error("mdb: precision must be 0 (bf16), 1 (tf32) or 2 (bf16x3)");
-  return static_cast<Precision>(v);
-}
 
 // A dense NDHWC activation tensor (channels innermost).
 struct Act {

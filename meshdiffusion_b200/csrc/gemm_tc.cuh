@@ -19,6 +19,7 @@
 // Warp roles (384 threads): warpgroup 0 = TMA producer (warp 0), warpgroups 1-2 = MMA + epilogue.
 #pragma once
 #include "ptx.cuh"
+#include "act_format.cuh"
 #include "gn_stats.cuh"
 
 namespace mdb {
@@ -125,14 +126,6 @@ struct GemmCfg {
   static constexpr int kFixedBytes = 1024 + kAccFloats * 4 + kStatsFloats * 4 + 2 * kMaxStages * 8;
 };
 constexpr int kRegsProducer = 40, kRegsConsumer = 232;  // 128 x 40 + 256 x 232 <= 65 536
-
-// dropout hash shared with the GroupNorm kernels (backward.cuh::drop_hash64)
-__device__ __forceinline__ unsigned long long gn_drop_hash64(unsigned long long seed, unsigned long long idx) {
-  unsigned long long z = idx + seed * 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
 
 // K-major 128B-swizzled operand at `saddr` (SBO = 1024 B)
 __device__ __forceinline__ uint64_t kdesc(uint32_t saddr) { return make_wgmma_desc(saddr, 16, 1024); }
@@ -428,12 +421,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
         if constexpr (GNB) {
           if (valid) {
             const float4* cc = p.gnb_c + static_cast<long long>(bg) * p.N + nb;
+            // dropout mask of act_format.cuh (apply_dropout, interleaved with the loop below: the helper's separate pass
+            // changes this instantiation's register allocation)
             unsigned long long hsh[8];
             if (p.gnb_drop_thresh > 0) {
-              // same element index as the forward GroupNorm-apply kernel: ((b*V + voxel)*C + channel)
               const unsigned long long e4 = (unsigned long long)((((static_cast<long long>(bg) * p.Z + zg) * p.Y + yg) * p.X + xg) * p.N + nb) >> 2;
 #pragma unroll
-              for (int i = 0; i < 8; ++i) hsh[i] = gn_drop_hash64(p.gnb_seed, e4 + i);
+              for (int i = 0; i < 8; ++i) hsh[i] = drop_hash64(p.gnb_seed, e4 + i);
             }
 #pragma unroll
             for (int i = 0; i < 32; ++i) {
@@ -448,17 +442,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
               }
               if (p.gnb_silu) {
                 const float h = fmaf(xv, kc.x, kc.y);
-                if constexpr (X3) {
-                  // silu'(y) = s(1 + y(1 - s)), s = sigmoid(y) = 1 / (1 + 2^(-y log2 e)), y = 2h
-                  float e, sg;
-                  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(h * -2.8853900817779268f));
-                  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(sg) : "f"(1.f + e));
-                  d *= sg * fmaf(2.f * h, 1.f - sg, 1.f);
-                } else {
-                  float th;
-                  asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(h));
-                  d *= fmaf(0.5f, h * fmaf(-th, th, 1.f), fmaf(0.5f, th, 0.5f));
-                }
+                d *= X3 ? dsilu_ex2_half(h) : dsilu_tanh_half(h);
               }
               v[i] = d;
               q2[i] = d * fmaf(xv, kc.z, kc.w);

@@ -32,4 +32,21 @@ struct StatAcc {
   __device__ __forceinline__ double sumsq() const { return (double)q_lo * (1.0 / 16777216.0) + (double)q_hi * 65536.0; }
 };
 
+// nn.GroupNorm(32, C, eps=1e-6) statistics (layers.py:589,652,660; ddpm_res64.py:120): mean and rstd (biased variance) of
+// group g (cpg channels) of sample b over the channel concatenation of stats0 (C0 channels) and stats1 (C1 channels)
+__device__ __forceinline__ void gn_group_stats(const long long* stats0, int C0, const long long* stats1, int C1, int b, int g,
+                                               int cpg, long long voxels, float eps, float& mean, float& rstd) {
+  StatAcc acc;
+  for (int i = 0; i < cpg; ++i) {
+    const int cc = g * cpg + i;
+    acc.add((cc < C0) ? stats0 + ((long long)b * C0 + cc) * kStatWords : stats1 + ((long long)b * C1 + (cc - C0)) * kStatWords);
+  }
+  const double n = (double)voxels * cpg;
+  const double m = acc.sum() / n;
+  double var = acc.sumsq() / n - m * m;
+  if (var < 0) var = 0;
+  mean = (float)m;
+  rstd = (float)(1.0 / sqrt(var + (double)eps));
+}
+
 }  // namespace mdb

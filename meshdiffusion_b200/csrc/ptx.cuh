@@ -149,12 +149,6 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-__device__ __forceinline__ float to_tf32_rna(float x) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-  return __uint_as_float(u);
-}
-
 // Register re-partitioning between warpgroups (all 4 warps of an aligned 128-thread group execute it together): ptxas allocates
 // the code that follows with the new per-thread limit. dec releases registers to the pool, inc blocks until they are there.
 template <int N>

@@ -151,14 +151,13 @@ TensP UNet::gn(const std::string& pname, const std::vector<TensP>& ins, bool sil
   NormActArgs na{};
   na.x0 = ins[0]->ptr; na.C0 = ins[0]->C; na.ld0 = ins[0]->C;
   na.x1 = ins.size() > 1 ? ins[1]->ptr : nullptr; na.C1 = ins.size() > 1 ? ins[1]->C : 0; na.ld1 = na.C1;
-  na.scale = nullptr; na.shift = nullptr; na.y = y->ptr; na.voxels = (long long)R * R * R; na.silu = silu ? 1 : 0;
-  na.tf32 = (int)prec_;
+  na.y = y->ptr; na.voxels = (long long)R * R * R; na.silu = silu ? 1 : 0; na.prec = prec_;
   na.stats0 = ins[0]->stats; na.stats1 = ins.size() > 1 ? ins[1]->stats : nullptr;
   na.gamma = gamma; na.beta = beta; na.groups = 32; na.eps = 1e-6f;
   if (train_ && drop_layer >= 0) {
     add_step("norm_act:" + pname, [na, this, drop_layer](cudaStream_t s, int B) {
       NormActArgs a = na;
-      a.drop_thresh = rt_drop_thresh_; a.drop_scale = rt_drop_scale_; a.seed = rt_seed_ + 0x632BE59BD9B4E019ull * (unsigned long long)(drop_layer + 1);
+      a.drop_thresh = rt_drop_thresh_; a.drop_scale = rt_drop_scale_; a.seed = dropout_layer_seed(rt_seed_, drop_layer);
       launch_norm_act(a, B, s);
     });
   } else {
@@ -265,15 +264,15 @@ TensP UNet::attn(const TensP& x, int midx) {
   // v^T [B][C][V] so that P.V has a K-major B operand
   TensP vT = new_act(C, R, false);
   if (!dry_) {
-    const void* src = qkv->ptr; void* dst = vT->ptr; const int tf = prec_ == kTF32;
+    const void* src = qkv->ptr; void* dst = vT->ptr; const int es = esize(prec_);
     if (prec_ == kBF16X3) {
       // qkv rows are [3C hi | 3C lo]; v^T rows become [V hi | V lo]
       add_step("attn" + std::to_string(midx) + ".vT", [=](cudaStream_t s, int B) {
-        launch_transpose_vc(src, 6 * C, 2 * C, dst, B, V, C, 0, s, 2 * V);
-        launch_transpose_vc(src, 6 * C, 5 * C, (__nv_bfloat16*)dst + V, B, V, C, 0, s, 2 * V);
+        launch_transpose_vc(src, 6 * C, 2 * C, dst, B, V, C, es, s, 2 * V);
+        launch_transpose_vc(src, 6 * C, 5 * C, (__nv_bfloat16*)dst + V, B, V, C, es, s, 2 * V);
       });
     } else
-    add_step("attn" + std::to_string(midx) + ".vT", [=](cudaStream_t s, int B) { launch_transpose_vc(src, 3 * C, 2 * C, dst, B, V, C, tf, s); });
+    add_step("attn" + std::to_string(midx) + ".vT", [=](cudaStream_t s, int B) { launch_transpose_vc(src, 3 * C, 2 * C, dst, B, V, C, es, s); });
   }
   // logits S[b][q][k] in fp32
   auto S = std::make_shared<Tens>();
@@ -290,8 +289,8 @@ TensP UNet::attn(const TensP& x, int midx) {
     g->set_alpha(1.0f / std::sqrt((float)C));
     g->finalize(0, false);
     add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-    float* sp = (float*)S->ptr; const int tf = (int)prec_;
-    add_step("attn" + std::to_string(midx) + ".softmax", [=](cudaStream_t s, int B) { launch_softmax_rows(sp, (long long)B * V, V, tf, s); });
+    float* sp = (float*)S->ptr; const Precision pr = prec_;
+    add_step("attn" + std::to_string(midx) + ".softmax", [=](cudaStream_t s, int B) { launch_softmax_rows(sp, (long long)B * V, V, pr, s); });
     GemmOp* g2 = new_gemm("attn" + std::to_string(midx) + ".pv");
     g2->set_output_strided(prec_, V, 1, 1, mb, C, O->ptr, C, 0, 0, (long long)V * C, false);
     Act pa; pa.ptr = S->ptr; pa.C = V; pa.ld = (prec_ == kBF16) ? 2 * V : V; pa.X = V; pa.Y = 1; pa.Z = 1; pa.B = mb;
@@ -372,9 +371,9 @@ TensP UNet::upsample(const TensP& x, int midx) {
   }
   TensP up = new_act(C, R, false);
   if (!dry_) {
-    const void* src = x->ptr; void* dst = up->ptr; const int r = x->R; const int tf = prec_ == kTF32;
+    const void* src = x->ptr; void* dst = up->ptr; const int r = x->R; const int es = esize(prec_);
     const int Cp = C * parts(prec_);  // X3: a row is 2C bf16 (hi | lo), copied as it is
-    add_step("up" + std::to_string(midx) + ".nearest", [=](cudaStream_t s, int B) { launch_upsample2x(src, dst, B, r, r, r, Cp, tf, s); });
+    add_step("up" + std::to_string(midx) + ".nearest", [=](cudaStream_t s, int B) { launch_upsample2x(src, dst, B, r, r, r, Cp, es, s); });
   }
   TensP out = new_act(C, R, true);
   Scratch sp = split_begin(R, C, C, 27);
@@ -446,10 +445,10 @@ void UNet::build() {
     float* field = (float*)dmalloc(V0 * nf * 4);
     Am = dmalloc(V0 * Kpad_m * esize(prec_) * parts(prec_));
     float* fbias = (float*)dmalloc(nf * 4);
-    const int tf = (int)prec_;
+    const Precision pr = prec_;
     const bool use_pos = cfg_.use_pos_bias != 0;
     commit_steps_.push_back({"field.bias", [=](cudaStream_t s, int) { launch_add_vec(mbias, use_pos ? posb : nullptr, fbias, nf, s); }});
-    commit_steps_.push_back({"field.im2col", [=](cudaStream_t s, int) { launch_im2col(mask, Am, 1, 1, R0, k, Kpad_m, tf, s); }});
+    commit_steps_.push_back({"field.im2col", [=](cudaStream_t s, int) { launch_im2col(mask, Am, 1, 1, R0, k, Kpad_m, pr, s); }});
     GemmOp* gf = new_gemm("stem.field", true);
     gf->set_output(prec_, R0, R0, R0, 1, nf, field, nf, true);
     Act am; am.ptr = Am; am.C = Kpad_m; am.X = am.Y = am.Z = R0; am.B = 1;
@@ -460,7 +459,7 @@ void UNet::build() {
     commit_steps_.push_back({"field.gemm", [gf](cudaStream_t s, int) { gf->repack(s); gf->launch(s, 1); }});
 
     void* a0 = A0->ptr;
-    add_step("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, tf, s); });
+    add_step("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, pr, s); });
     GemmOp* g = new_gemm("stem.gemm");
     g->set_output(prec_, R0, R0, R0, mb, nf, h0->ptr, nf, false);
     Act a; a.ptr = a0; a.C = Kpad; a.X = a.Y = a.Z = R0; a.B = mb;

@@ -95,8 +95,9 @@ GemmOp* UNet::new_bwd_gemm(const std::string& name) {
 
 void UNet::set_dropout(float p, unsigned long long seed) {
   if (p < 0.f || p >= 1.f) throw std::runtime_error("mdb: dropout probability out of range");
-  rt_drop_thresh_ = (int)std::lround((double)p * 65536.0);
-  rt_drop_scale_ = p > 0.f ? 1.f / (1.f - p) : 1.f;
+  const DropoutParams d = dropout_params(p);
+  rt_drop_thresh_ = d.thresh;
+  rt_drop_scale_ = d.scale;
   rt_seed_ = seed;
 }
 
@@ -167,7 +168,7 @@ void UNet::emit_colsum(const std::string& name, const GradView& t, int R, float*
     a.t = t.ptr; a.ld = t.ld; a.C = t.C; a.voxels = (long long)R * R * R;
     a.part = (float*)part.ptr; a.per = per; a.per_ld = per_ld;
     a.from_per = t.colsum; a.from_ld = t.cs_ld;
-    a.x3 = prec_ == kBF16X3 ? 1 : 0;
+    a.prec = prec_;
     add_bwd(name, [=](cudaStream_t s, int B) {
       ColsumArgs c = a;
       c.total0 = g0 >= 0 ? rt_grads_ + g0 : nullptr;
@@ -250,7 +251,7 @@ GradView UNet::emit_conv_dgrad(const std::string& name, const GradView& dy, int 
     add_bwd(name, [g, this, dl](cudaStream_t s, int B) {
       if (dl >= 0) {
         g->rt_drop_thresh = rt_drop_thresh_; g->rt_drop_scale = rt_drop_scale_;
-        g->rt_seed = rt_seed_ + 0x632BE59BD9B4E019ull * (unsigned long long)(dl + 1);
+        g->rt_seed = dropout_layer_seed(rt_seed_, dl);
       }
       g->launch(s, B);
     });
@@ -310,13 +311,13 @@ GradView UNet::emit_gn_backward(const std::string& pname, const std::vector<Tens
     a.add0 = add0 ? add0->ptr : nullptr; a.add0_ld = add0 ? add0->ld : 0;
     a.add1 = add1 ? add1->ptr : nullptr; a.add1_ld = add1 ? add1->ld : 0;
     a.cs_part = (float*)cs_part.ptr; a.cs_per = dx.colsum;
-    a.x3 = prec_ == kBF16X3 ? 1 : 0;
+    a.prec = prec_;
     const long long gw = G(pname + ".weight"), gb = G(pname + ".bias");
     auto with_rt = [this, a, gw, gb, drop_layer]() {
       GnBwdArgs c = a;
       if (drop_layer >= 0) {
         c.drop_thresh = rt_drop_thresh_; c.drop_scale = rt_drop_scale_;
-        c.seed = rt_seed_ + 0x632BE59BD9B4E019ull * (unsigned long long)(drop_layer + 1);
+        c.seed = dropout_layer_seed(rt_seed_, drop_layer);
       }
       // input gradient only: no gamma / beta gradient (the reduce launch then skips its parameter kernel)
       c.dgamma = rt_grads_ ? rt_grads_ + gw : nullptr; c.dbeta = rt_grads_ ? rt_grads_ + gb : nullptr;
@@ -435,7 +436,8 @@ void UNet::tape_attn(TensP x, TensP hn, TensP qkv, TensP S, TensP O, TensP out, 
       return a;
     };
     const float alpha = 1.0f / std::sqrt((float)C);
-    const int es = esize(prec_), P = parts(prec_), x3 = prec_ == kBF16X3 ? 1 : 0;
+    const int es = esize(prec_), P = parts(prec_);
+    const Precision pr = prec_;
     GradView dqkv = new_grad(3 * C, R);
     // dP[q][k] = dOo[q][:] . v[k][:]   (fp32, softmax backward then runs in place)
     Tmp dS = tmp_alloc((size_t)mb * V * V * 4);
@@ -455,8 +457,8 @@ void UNet::tape_attn(TensP x, TensP hn, TensP qkv, TensP S, TensP O, TensP out, 
       const void* sp = S->ptr; char* pt = (char*)PT.ptr; const void* dop = dOo.ptr; char* dot = (char*)dOT.ptr;
       add_bwd(nm + ".PT", [=](cudaStream_t s, int B) {
         for (int part = 0; part < P; ++part) {
-          launch_transpose_vc(sp, 2 * V, part * V, pt + (size_t)part * V * es, B, V, V, 0, s, (long long)P * V);
-          launch_transpose_vc(dop, (long long)P * C, part * C, dot + (size_t)part * V * es, B, V, C, 0, s, (long long)P * V);
+          launch_transpose_vc(sp, 2 * V, part * V, pt + (size_t)part * V * es, B, V, V, es, s, (long long)P * V);
+          launch_transpose_vc(dop, (long long)P * C, part * C, dot + (size_t)part * V * es, B, V, C, es, s, (long long)P * V);
         }
       });
       GemmOp* g = new_bwd_gemm(nm + ".dv");
@@ -466,7 +468,7 @@ void UNet::tape_attn(TensP x, TensP hn, TensP qkv, TensP S, TensP O, TensP out, 
       g->finalize(0, false);
       add_bwd(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
       float* dsp = (float*)dS.ptr; const float* pp = (const float*)S->ptr;
-      add_bwd(nm + ".softmax_bwd", [=](cudaStream_t s, int B) { launch_softmax_bwd_rows(pp, dsp, (long long)B * V, V, s, x3); });
+      add_bwd(nm + ".softmax_bwd", [=](cudaStream_t s, int B) { launch_softmax_bwd_rows(pp, dsp, (long long)B * V, V, pr, s); });
     }
     tmp_free(PT);
     tmp_free(dOT);
@@ -480,15 +482,15 @@ void UNet::tape_attn(TensP x, TensP hn, TensP qkv, TensP S, TensP O, TensP out, 
       const void* qp = qkv->ptr; char* ktp = (char*)kT.ptr; char* qtp = (char*)qT.ptr; const void* dsp = dS.ptr; char* dstp = (char*)dST.ptr;
       add_bwd(nm + ".kT", [=](cudaStream_t s, int B) {
         for (int part = 0; part < P; ++part) {  // qkv rows: [3C hi | 3C lo]; dS rows: V hi then V lo bf16
-          launch_transpose_vc(qp, 3LL * C * P, C + part * 3 * C, ktp + (size_t)part * V * es, B, V, C, 0, s, (long long)P * V);
-          launch_transpose_vc(qp, 3LL * C * P, part * 3 * C, qtp + (size_t)part * V * es, B, V, C, 0, s, (long long)P * V);
-          launch_transpose_vc(dsp, 2 * V, part * V, dstp + (size_t)part * V * es, B, V, V, 0, s, (long long)P * V);
+          launch_transpose_vc(qp, 3LL * C * P, C + part * 3 * C, ktp + (size_t)part * V * es, B, V, C, es, s, (long long)P * V);
+          launch_transpose_vc(qp, 3LL * C * P, part * 3 * C, qtp + (size_t)part * V * es, B, V, C, es, s, (long long)P * V);
+          launch_transpose_vc(dsp, 2 * V, part * V, dstp + (size_t)part * V * es, B, V, V, es, s, (long long)P * V);
         }
       });
       GemmOp* g = new_bwd_gemm(nm + ".dq");
       g->set_output_strided(prec_, V, 1, 1, mb, C, dqkv.ptr, 3 * C, 0, 0, (long long)V * 3 * C, false);
       // dS as the A operand: bf16 at the start of rows of V fp32 slots (logical pitch 2V), or X3 (hi | lo) rows filling them
-      g->add_pointwise({mat(dS.ptr, V, x3 ? V : 2 * V)}, nullptr, true);
+      g->add_pointwise({mat(dS.ptr, V, pr == kBF16X3 ? V : 2 * V)}, nullptr, true);
       g->set_b_activation(kT.ptr, V, C, mb, V, (long long)C * V);
       g->set_alpha(alpha);
       g->finalize(0, false);
@@ -575,8 +577,8 @@ void UNet::tape_upsample(TensP x, TensP up, TensP out, int midx) {
     unref(out->grad);
     GradView dx = new_grad(C, x->R);
     if (!dry_) {
-      const void* src = dup.ptr; void* dst = dx.ptr; const int r = x->R; const int x3 = prec_ == kBF16X3 ? 1 : 0;
-      add_bwd(nm + ".downsum", [=](cudaStream_t s, int B) { launch_downsum2x(src, dst, B, r, C, s, x3); });
+      const void* src = dup.ptr; void* dst = dx.ptr; const int r = x->R; const Precision pr = prec_;
+      add_bwd(nm + ".downsum", [=](cudaStream_t s, int B) { launch_downsum2x(src, dst, B, r, C, pr, s); });
     }
     unref(dup);
     if (x->grad.valid()) throw std::runtime_error("mdb: upsample input already has a gradient");
@@ -618,11 +620,12 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
     // h0 = conv(x) + b + pos_layer.bias + mask_layer(mask): the three biases receive the same column sum
     emit_colsum("stem.dbias", dh, R0, nullptr, 0, G("all_modules.2.bias"), cfg_.use_pos_bias ? G("pos_layer.bias") : -1, G("mask_layer.bias"));
     // stem weight: dW[co][ci*T + tap] = sum_v dh[v][co] im2col(x)[v][ci*T + tap]  (im2col recomputed)
-    const int es = esize(prec_), P = parts(prec_), mode = (int)prec_;
+    const int es = esize(prec_), P = parts(prec_);
+    const Precision pr = prec_;
     Tmp A0 = tmp_alloc((size_t)cfg_.max_batch * V0 * Kpad * es * P);
     if (!dry_) {
       void* a0 = A0.ptr;
-      add_bwd("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, mode, s); }, kParamGradOnly);
+      add_bwd("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, pr, s); }, kParamGradOnly);
     }
     {
       Act xa; xa.ptr = A0.ptr; xa.C = Kpad; xa.X = xa.Y = xa.Z = R0; xa.B = cfg_.max_batch;
@@ -633,8 +636,8 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
     // mask_layer weight: the mask is shared by the batch -> reduce dh over the batch first
     Tmp hs = tmp_alloc((size_t)V0 * nf * es * P);
     if (!dry_) {
-      const void* src = dh.ptr; void* dst = hs.ptr; const int x3 = prec_ == kBF16X3 ? 1 : 0;
-      add_bwd("stem.batch_sum", [=](cudaStream_t s, int B) { launch_batch_sum(src, dst, B, V0 * nf, s, nf, x3); }, kParamGradOnly);
+      const void* src = dh.ptr; void* dst = hs.ptr;
+      add_bwd("stem.batch_sum", [=](cudaStream_t s, int B) { launch_batch_sum(src, dst, B, V0 * nf, nf, pr, s); }, kParamGradOnly);
     }
     {
       Act da; da.ptr = hs.ptr; da.C = nf; da.X = da.Y = da.Z = R0; da.B = 1;
@@ -661,11 +664,11 @@ void UNet::tape_head(TensP h, TensP a, const std::string& gn_name, const std::st
     // im2col of dL/dout ([voxel][co*T + tap'], reading dout at v + off(tap')) serves both gradients:
     //   dW[co][c][T-1-tap'] = sum_v a[v][c] Ad[v][co*T + tap'],   da[v][c] = sum_k Ad[v][k] W[co][c][T-1-tap']
     const int Kp = ((Cin * T + 63) / 64) * 64;
-    const int mode = (int)prec_;
+    const Precision pr = prec_;
     Tmp Ad = tmp_alloc((size_t)cfg_.max_batch * V0 * Kp * esize(prec_) * parts(prec_));
     if (!dry_) {
       void* ad = Ad.ptr;
-      add_bwd("head.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_dout_, ad, B, Cin, R0, k, Kp, mode, s); });
+      add_bwd("head.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_dout_, ad, B, Cin, R0, k, Kp, pr, s); });
     }
     Act ada; ada.ptr = Ad.ptr; ada.C = Kp; ada.X = ada.Y = ada.Z = R0; ada.B = cfg_.max_batch;
     {

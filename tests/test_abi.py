@@ -53,3 +53,19 @@ def test_dry_plan_errors_are_reported_not_thrown():
     h = ctypes.c_void_p()
     rc = L.mdb_unet_create_dry(ctypes.byref(cfg), ctypes.byref(h))
     assert rc != 0 and b"image_size" in L.mdb_last_error()
+
+
+def test_groupnorm_entry_points_refuse_null_stats():
+    """The GroupNorm kernels derive mean / rstd from `stats` and have no other source of them: a NULL `stats` is an error
+    reported before anything is launched (so this needs no GPU)."""
+    from meshdiffusion_b200 import _native
+    L = _native.lib()
+    B, V, C = 1, 8, 32
+    assert L.mdb_groupnorm_act(None, None, None, None, None, B, V, C, 1, 0, None) != 0
+    assert b"stats" in L.mdb_last_error()
+    assert L.mdb_groupnorm_act_backward(None, None, None, None, None, None, None, None, None, B, V, C, 1, 0.0, 0, None) != 0
+    assert b"stats" in L.mdb_last_error()
+    for precision in (0, 2):
+        assert L.mdb_groupnorm_act_backward_prec(None, None, None, None, None, None, None, None, None, B, V, C, 1, 0.0, 0,
+                                                 precision, None) != 0
+        assert b"stats" in L.mdb_last_error()

@@ -208,7 +208,7 @@ def test_unet_backward_x3_accumulates_and_is_deterministic():
 
 
 def test_x3_dropout_gradients_fused_vs_two_pass(monkeypatch):
-    """The dropout mask of the split-bf16 forward (norm/act MODE 2), the two-pass GroupNorm backward and the fused GEMM
+    """The dropout mask of the split-bf16 forward (norm/act kernel), the two-pass GroupNorm backward and the fused GEMM
     epilogue agree: fused and two-pass engines give the same gradients, which differ from the no-dropout ones."""
     R, B = 16, 2
 

@@ -97,10 +97,10 @@ def run(batch=16, iters=4, steps=3, warmup=1, config="res64", dropout=0.1, no_ov
     timed(net, "_push_parameters", "weight_sync")
     orig_fwd = net._train_forward
 
-    def fwd(x, labels):  # forward minus the parameter push it starts with
+    def fwd(x, labels, *rest):  # forward minus the parameter push it starts with
         e0, e1 = ev(), ev()
         e0.record()
-        out = orig_fwd(x, labels)
+        out = orig_fwd(x, labels, *rest)
         e1.record()
         marks.append(("fwd_incl_sync", e0, e1))
         return out
