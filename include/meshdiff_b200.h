@@ -66,6 +66,9 @@ int mdb_unet_commit(mdb_unet* net, void* stream);
 /* score_model(x, labels): x fp32 NCDHW [B][C][R][R][R], labels fp32 [B], out fp32 NCDHW (ddpm_res64.py:126-199). */
 int mdb_unet_forward(mdb_unet* net, const float* x, const float* labels, float* out, int batch, void* stream);
 int mdb_unet_info(mdb_unet* net, double* flops_per_sample, long long* arena_bytes, int* n_gemm_launches, int* n_steps);
+/* Forward GEMM launch i (0 <= i < n_gemm_launches) at the engine's max batch: its step name (valid while the engine
+ * lives), executed FLOPs and the bytes TMA writes into shared memory (A boxes + weight tiles, summed over output tiles). */
+int mdb_unet_gemm_ops(mdb_unet* net, int i, const char** name, double* flops, double* fill_bytes);
 /* One profiled forward: per-step device milliseconds. names_buf receives '\n'-separated step names. Synchronises. */
 int mdb_unet_profile(mdb_unet* net, const float* x, const float* labels, float* out, int batch, void* stream,
                      char* names_buf, int names_len, float* ms, int max_steps, int* n_steps);

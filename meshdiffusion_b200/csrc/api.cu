@@ -109,6 +109,16 @@ int mdb_unet_info(mdb_unet* n, double* flops, long long* arena, int* ngemm, int*
   MDB_API_END
 }
 
+int mdb_unet_gemm_ops(mdb_unet* n, int i, const char** name, double* flops, double* fill_bytes) {
+  MDB_API_BEGIN
+  if (i < 0 || i >= n->net->num_gemm_launches()) throw std::runtime_error("mdb: GEMM launch index out of range");
+  const GemmOp& g = n->net->gemm(i);
+  if (name) *name = g.name.c_str();
+  if (flops) *flops = g.flops;
+  if (fill_bytes) *fill_bytes = g.fill_bytes();
+  MDB_API_END
+}
+
 int mdb_unet_profile(mdb_unet* n, const float* x, const float* labels, float* out, int B, void* stream, char* names,
                      int names_len, float* ms, int max_steps, int* nsteps) {
   MDB_API_BEGIN

@@ -46,6 +46,38 @@ void encode_map(CUtensorMap* m, Precision prec, int rank, void* base, const uint
   }
 }
 
+void GemmOp::pick_slots(GemmParams& q) const {
+  // Operand rings of this op in the shared memory left next to the epilogue scratch: two slots of each at least (one
+  // filling while one is read). Then B slots are added until they cover the k-steps of every A slot in flight, and A slots
+  // (entries in flight) up to MDB_MAX_STAGES (default 4), whichever is behind and still fits.
+  const int fixed = block_n == 32 ? GemmCfg<32>::kFixedBytes : GemmCfg<128>::kFixedBytes;
+  const int budget = kMaxDynSmem - fixed;
+  q.a_slot_bytes = (a_slot_need + 1023) / 1024 * 1024;
+  q.b_slot_bytes = parts(prec) * block_n * kRowBytes;
+  int cap = 4;
+  if (const char* e = getenv("MDB_MAX_STAGES")) { const int c = atoi(e); if (c >= 2) cap = c; }
+  if (cap > kMaxSlots) cap = kMaxSlots;
+  int na = 2, nb = 2;
+  int used = na * q.a_slot_bytes + nb * q.b_slot_bytes;
+  if (used > budget) throw std::runtime_error("mdb: operand rings need at least two slots each");
+  for (;;) {
+    if (nb < na * nk_max && nb < kMaxSlots && used + q.b_slot_bytes <= budget) { ++nb; used += q.b_slot_bytes; }
+    else if (na < cap && used + q.a_slot_bytes <= budget) { ++na; used += q.a_slot_bytes; }
+    else break;
+  }
+  q.n_aslots = na;
+  q.n_bslots = nb;
+}
+
+double GemmOp::fill_bytes(int B) const {
+  // bytes TMA writes into shared memory for one launch: every entry's A box(es) and weight tiles, once per output tile
+  // (split-K only divides the entries between CTAs)
+  double per_tile = 0;
+  for (const auto& e : loads) per_tile += parts(prec) * ((double)e.rows * kRowBytes + (double)e.nk * block_n * kRowBytes);
+  const int tb = B > 0 ? (B + p.bb - 1) / p.bb : p.tb;
+  return per_tile * p.tx * p.ty * p.tz * tb * p.n_tiles_n;
+}
+
 int sm_count() {
   static int n = 0;
   if (!n) {
@@ -73,11 +105,12 @@ int plan_splits(int X, int Y, int Z, int B, int N, int cin_total, int taps, Prec
   const int tiles_m = ((X + g.bx - 1) / g.bx) * ((Y + g.by - 1) / g.by) * ((Z + g.bz - 1) / g.bz) * ((B + g.bb - 1) / g.bb);
   const int block_n = N <= 32 ? 32 : 128;
   const int tiles = tiles_m * ((N + block_n - 1) / block_n);
-  const int ksteps = ((cin_total + kb_elems(prec) - 1) / kb_elems(prec)) * taps * (prec == kBF16X3 ? 3 : 1);
-  if (tiles > 49 || ksteps < 48) return 1;
+  // work per tile in k-step products: a split-bf16 k-step is three of them (hi.hi, hi.lo, lo.hi)
+  const int kprod = ((cin_total + kb_elems(prec) - 1) / kb_elems(prec)) * taps * (prec == kBF16X3 ? 3 : 1);
+  if (tiles > 49 || kprod < 48) return 1;
   int S = kPlanSMs / tiles;
   if (S > 16) S = 16;
-  if (S > ksteps / 8) S = ksteps / 8;
+  if (S > kprod / 8) S = kprod / 8;
   return S < 2 ? 1 : S;
 }
 
@@ -163,21 +196,13 @@ int GemmOp::add_amap(const Act& a, int halo, int sub, int px, int py, int pz, in
 
 void GemmOp::add_load_x(int tm_hi, int tm_lo, int nk, int rows, int jrows, int dx, int dy, int dz, int c0, int wsrc,
                         int wc0, int tap0, int tapj) {
-  if (prec != kBF16X3) { add_load(tm_hi, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 0); return; }
-  // K-extension form. Small terms first: (A lo, W hi) and (A hi, W lo) are ~2^-9 of the leading product
-  add_load(tm_lo, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 0);
-  add_load(tm_hi, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 1);
-  add_load(tm_hi, nk, rows, jrows, dx, dy, dz, c0, wsrc, wc0, tap0, tapj, 0);
-}
-
-void GemmOp::add_load(int tmap, int nk, int rows, int jrows, int dx, int dy, int dz, int c0, int wsrc, int wc0,
-                      int tap0, int tapj, int wpart) {
   if ((int)loads.size() >= kMaxLoads) throw std::runtime_error("mdb: load table overflow");
   if (rows > kAStageRows) throw std::runtime_error("mdb: A box exceeds the stage size");
   LoadEntry e{};
-  e.tmap = (uint8_t)tmap; e.nk = (uint8_t)nk; e.rows = (uint8_t)rows; e.jrows = (uint8_t)jrows;
+  e.tmap = (uint8_t)tm_hi; e.tmap_lo = (uint8_t)(prec == kBF16X3 ? tm_lo : tm_hi);
+  e.nk = (uint8_t)nk; e.rows = (uint8_t)rows; e.jrows = (uint8_t)jrows;
   e.dx = (int8_t)dx; e.dy = (int8_t)dy; e.dz = (int8_t)dz; e.wsrc = (uint8_t)wsrc;
-  e.c0 = (uint16_t)c0; e.wc0 = (uint16_t)wc0; e.tap0 = (uint8_t)tap0; e.tapj = (uint8_t)tapj; e.wpart = (uint16_t)wpart;
+  e.c0 = (uint16_t)c0; e.wc0 = (uint16_t)wc0; e.tap0 = (uint8_t)tap0; e.tapj = (uint8_t)tapj;
   loads.push_back(e);
   ksteps += nk;
 }
@@ -354,7 +379,8 @@ void GemmOp::set_b_activation(void* ptr, int K, int N, int batch, long long rs, 
 struct PackWSrc { const float* ptr; long long sn, sc, st; int cvalid; int ndiv; long long sn_hi; int cdiv; long long sc_hi; };
 struct PackArgs { PackWSrc w[4]; };
 
-// split bf16: entry.wpart selects hi = bf16(w) or lo = bf16(w - hi).
+// split bf16: every k-step is packed as its hi = bf16(w) tile followed by its lo = bf16(w - hi) tile (K columns
+// [2 ks KB, 2 ks KB + KB) and [2 ks KB + KB, 2 (ks + 1) KB)).
 // One thread = 8 consecutive K elements (one 16- / 32-byte store) of EVERY k-step of one load entry for one output row: the
 // entry / source / offset arithmetic is done once per 8 * nk outputs. (The first version, one thread per packed element with
 // two 64-bit divisions and a table walk each, made the per-optimiser-step re-pack of the training engine instruction-bound:
@@ -382,26 +408,29 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const LoadEntry* __re
       if (c < w.cvalid) valid |= 1u << i;
       coff[i] = noff + (w.cdiv ? (long long)(c % w.cdiv) * w.sc + (long long)(c / w.cdiv) * w.sc_hi : (long long)c * w.sc);
     }
-    const long long obase = ((long long)n * ksteps + load_ks0[l]) * KB + v8 * 8;
+    constexpr int kParts = P == kBF16X3 ? 2 : 1;
+    const long long obase = ((long long)n * ksteps + load_ks0[l]) * kParts * KB + v8 * 8;
     for (int j = 0; j < e.nk; ++j) {
       const long long toff = (long long)(e.tap0 + j * e.tapj) * w.st;
       float v[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = (valid >> i) & 1u ? __ldg(w.ptr + coff[i] + toff) : 0.f;
-      const long long o = obase + (long long)j * KB;
+      const long long o = obase + (long long)j * kParts * KB;
       if (P == kTF32) {
         float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + o);
         op[0] = make_float4(to_tf32_rna(v[0]), to_tf32_rna(v[1]), to_tf32_rna(v[2]), to_tf32_rna(v[3]));
         op[1] = make_float4(to_tf32_rna(v[4]), to_tf32_rna(v[5]), to_tf32_rna(v[6]), to_tf32_rna(v[7]));
       } else {
-        uint4 pk;
+        uint4 pk, pl;
         __nv_bfloat16* h = reinterpret_cast<__nv_bfloat16*>(&pk);
+        __nv_bfloat16* lo = reinterpret_cast<__nv_bfloat16*>(&pl);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          const __nv_bfloat16 hi = __float2bfloat16(v[i]);
-          h[i] = (P == kBF16X3 && e.wpart) ? bf16_lo(v[i], hi) : hi;
+          h[i] = __float2bfloat16(v[i]);
+          if (P == kBF16X3) lo[i] = bf16_lo(v[i], h[i]);
         }
         *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(out) + o) = pk;
+        if (P == kBF16X3) *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(out) + o + KB) = pl;
       }
     }
   }
@@ -436,27 +465,25 @@ void GemmOp::repack(cudaStream_t stream) {
 void GemmOp::finalize(cudaStream_t stream, bool pack) {
   if (loads.empty()) throw std::runtime_error("mdb: GemmOp without loads");
   p.b_explicit_k = 0;
+  p.b_kstep = kb_elems(prec) * parts(prec);  // packed weights: a k-step's tiles sit side by side (X3: hi, lo)
+  p.b_lo_k = kb_elems(prec);
+  if (b_from_act) p.b_kstep = kb_elems(prec);
   if (b_from_act && prec == kBF16X3) {
-    // activation-B operand in the split layout: every entry names the K coordinate of its B tile itself
-    // ((A hi, B hi), (A hi, B lo), (A lo, B hi) cannot be a running column of one matrix)
-    for (auto& e : loads) {
-      const long long k0 = (long long)e.wc0 + (e.wpart ? b_lo_off : 0);
-      if (k0 > 65535) throw std::runtime_error("mdb: X3 activation-B K coordinate exceeds the table's 16 bits");
-      e.wc0 = (uint16_t)k0;
-    }
+    // activation-B operand in the split layout: every entry names the K coordinate of its B hi tile itself (wc0); the
+    // lo parts of the rows are the K coordinates b_lo_off further on
     p.b_explicit_k = 1;
+    p.b_lo_k = (int)b_lo_off;
   }
   MDB_CUDA_CHECK(cudaMalloc(&d_loads, loads.size() * sizeof(LoadEntry)));
   MDB_CUDA_CHECK(cudaMemcpyAsync(d_loads, loads.data(), loads.size() * sizeof(LoadEntry), cudaMemcpyHostToDevice, stream));
   p.loads = d_loads;
   p.n_loads = (int)loads.size();
   if (p.splits < 1) p.splits = 1;
-  // pipeline segments: runs of identical entries, one entry (its A box and the weight tiles of its k-steps) per stage.
-  // The stage size is the largest group of this op and the ring takes as many stages as fit next to the epilogue scratch.
+  // pipeline segments: runs of identical entries. An entry's A box (X3: both parts) takes an A slot, the weight tiles of
+  // each of its k-steps a B slot; the A slot size is the largest box of this op.
   {
-    const int btile = block_n * kRowBytes;
-    const int max_stage = kAStageBytes + 3 * 128 * kRowBytes;
-    stage_need = 0;
+    a_slot_need = 0;
+    nk_max = 0;
     p.n_segs = 0;
     p.total_groups = 0;
     size_t i = 0;
@@ -469,9 +496,10 @@ void GemmOp::finalize(cudaStream_t stream, bool pack) {
       sg.a_bytes = loads[i].rows * kRowBytes;
       sg.a_stride = (sg.a_bytes + 1023) / 1024 * 1024;
       sg.jbytes = loads[i].jrows * kRowBytes;
-      const int need = sg.a_stride + sg.nk * btile;
-      if (need > max_stage) throw std::runtime_error("mdb: pipeline group exceeds the stage size");
-      if (need > stage_need) stage_need = need;
+      const int need = parts(prec) * sg.a_stride;
+      if (sg.a_stride > kAStageBytes) throw std::runtime_error("mdb: A box exceeds the slot size");
+      if (need > a_slot_need) a_slot_need = need;
+      if (sg.nk > nk_max) nk_max = sg.nk;
       p.segs[p.n_segs++] = sg;
       p.total_groups += sg.n_groups;
       i = j;
@@ -479,7 +507,7 @@ void GemmOp::finalize(cudaStream_t stream, bool pack) {
   }
   if (p.splits > p.total_groups) { p.splits = p.total_groups; splits = p.splits; }
   if (!b_from_act) {
-    const long long ktot = 1LL * ksteps * kb_elems(prec);
+    const long long ktot = 1LL * ksteps * kb_elems(prec) * parts(prec);
     const long long bytes = ktot * p.N * esize(prec);
     MDB_CUDA_CHECK(cudaMalloc(&d_wpacked, bytes));
     owns_w = true;
@@ -494,7 +522,7 @@ template <int BN, bool TF32, bool GNB = false, bool X3 = false>
 static void launch_impl(const GemmParams& p, int grid, cudaStream_t stream) {
   static bool configured[64] = {};  // the attribute is per device
   auto kern = gemm_tc_kernel<BN, TF32, GNB, X3>;
-  const int smem = GemmCfg<BN>::kFixedBytes + p.n_stages * p.stage_bytes;
+  const int smem = GemmCfg<BN>::kFixedBytes + p.n_aslots * p.a_slot_bytes + p.n_bslots * p.b_slot_bytes;
   int dev = 0;
   MDB_CUDA_CHECK(cudaGetDevice(&dev));
   if (dev >= 64 || !configured[dev]) {
@@ -507,17 +535,7 @@ static void launch_impl(const GemmParams& p, int grid, cudaStream_t stream) {
 
 void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
   GemmParams p = this->p;
-  {
-    // operand ring of this op: stage = its largest pipeline group, as many stages as the 227 KB allow
-    const int fixed = block_n == 32 ? GemmCfg<32>::kFixedBytes : GemmCfg<128>::kFixedBytes;
-    p.stage_bytes = (stage_need + 1023) / 1024 * 1024;
-    int ns = (kMaxDynSmem - fixed) / p.stage_bytes;
-    int cap = 4;
-    if (const char* e = getenv("MDB_MAX_STAGES")) { const int c = atoi(e); if (c >= 2) cap = c; }
-    if (ns > cap) ns = cap;
-    p.n_stages = ns > kMaxStages ? kMaxStages : ns;
-    if (p.n_stages < 2) throw std::runtime_error("mdb: operand ring needs at least two stages");
-  }
+  pick_slots(p);
   if (B > 0) {
     if (B > this->p.Bn) throw std::runtime_error("mdb: batch exceeds the batch the op was built for");
     p.Bn = B;

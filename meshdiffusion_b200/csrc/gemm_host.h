@@ -57,11 +57,11 @@ class GemmOp {
   std::vector<LoadEntry> loads;
   std::vector<WSrc> wsrcs;
   int n_amaps = 0;
-  int ksteps = 0;
+  int ksteps = 0;  // k-steps of the load table (X3: each with a W_hi and a W_lo tile)
   // device-owned
   LoadEntry* d_loads = nullptr;
   int* d_ks0 = nullptr;      // (weight packer) first k-step of every load entry
-  void* d_wpacked = nullptr;  // [N][ksteps*KB] in activation dtype
+  void* d_wpacked = nullptr;  // [N][ksteps * parts * KB] in activation dtype
   bool owns_w = false;
   double flops = 0;  // algorithmic FLOPs of one launch (2*M*N*K over valid taps, counted densely)
   std::string name;
@@ -79,10 +79,8 @@ class GemmOp {
   // adds a 5-D A tensor map over `a` (optionally a stride-2 parity sub-grid) with a (KB, bx, by+halo, bz, bb) box.
   // part: 0 = the tensor itself / the hi parts of an X3 tensor, 1 = its lo parts
   int add_amap(const Act& a, int halo_rows_y, int sub_stride = 1, int px = 0, int py = 0, int pz = 0, int part = 0);
-  void add_load(int tmap, int nk, int rows, int jrows, int dx, int dy, int dz, int c0, int wsrc, int wc0, int tap0,
-                int tapj, int wpart = 0);
-  // one logical A load -> 1 table entry (bf16 / tf32) or the 3 entries of the split product (X3): (A hi, W hi),
-  // (A hi, W lo), (A lo, W hi); tm_lo is the tensor map of the lo parts
+  // one A load (one table entry): the box of tensor map tm_hi, multiplied with the weight tiles of nk k-steps. X3: tm_lo
+  // is the tensor map of the lo parts, loaded next to the hi parts; each k-step brings its W_hi and W_lo tiles
   void add_load_x(int tm_hi, int tm_lo, int nk, int rows, int jrows, int dx, int dy, int dz, int c0, int wsrc, int wc0,
                   int tap0, int tapj);
   int add_wsrc(const WSrc& w) { wsrcs.push_back(w); return (int)wsrcs.size() - 1; }
@@ -133,11 +131,15 @@ class GemmOp {
   void repack(cudaStream_t stream);
   // B <= the batch the op was built for; out_override replaces the output pointer (user buffers).
   void launch(cudaStream_t stream, int B = -1, void* out_override = nullptr) const;
+  // bytes TMA writes into shared memory in one launch at batch B (<= 0: the batch the op was built for)
+  double fill_bytes(int B = -1) const;
 
  private:
   Geometry geo{};
   bool b_from_act = false;
-  int stage_need = 0;  // bytes of the largest pipeline group (decides the stage size / count at launch)
+  int a_slot_need = 0;  // bytes of the largest A box (X3: both parts): the A slot size
+  int nk_max = 0;       // most k-steps of one entry
+  void pick_slots(GemmParams& q) const;
   long long b_lo_off = 0;  // X3 activation-B: K coordinate of the lo parts
   void encode_bmap(void* ptr, int K, int N, int batch, long long row_stride_bytes, long long batch_stride_bytes);
 };

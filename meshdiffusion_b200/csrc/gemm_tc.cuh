@@ -45,18 +45,20 @@ struct __align__(16) LoadEntry {
                   // K coordinate of this entry's first B tile (activation-B operands of the X3 mode)
   uint8_t tap0;   // (weight packer) tap index of k-step 0
   uint8_t tapj;   // (weight packer) tap increment per k-step
-  uint16_t wpart; // (weight packer, X3) 0 = hi part bf16(w), 1 = lo part bf16(w - hi)
+  uint8_t tmap_lo;  // X3: index of the A tensor map of the lo parts (same box, loaded next to the hi parts)
+  uint8_t pad;
 };
 static_assert(sizeof(LoadEntry) == 16, "LoadEntry must be 16 bytes");
 
-// A run of identical pipeline groups. One group = one shared-memory stage = one full/empty mbarrier pair:
-// one A box and the nk weight tiles it is multiplied with. All fields are
-// warp-uniform kernel parameters, so the MMA warp's control flow and descriptor arithmetic never touch memory.
+// A run of identical pipeline groups. One group = one load-table entry: one A box (X3: its hi and lo parts) in an A slot,
+// multiplied with the weight tiles of its nk k-steps, one B slot per k-step (X3: the W_hi and W_lo tiles of the k-step).
+// All fields are warp-uniform kernel parameters, so the MMA warp's control flow and descriptor arithmetic never touch
+// memory.
 struct GemmSeg {
   int n_groups;
   int nk;        // k-steps per entry
   int a_bytes;   // bytes of one A box (rows * 128) -- the TMA transaction size
-  int a_stride;  // distance between the group's A boxes in the stage (multiple of 1024)
+  int a_stride;  // X3: distance from the hi to the lo box in the A slot (multiple of 1024)
   int jbytes;    // A-descriptor advance between the k-steps of one entry (halo reuse)
 };
 constexpr int kMaxSegs = 8;
@@ -81,7 +83,11 @@ struct GemmParams {
   int batch_fastest;   // enumerate the batch axis first among M-tiles (residual shared by all samples stays in L2)
   int kb_elems;        // K elements per k-step (64 bf16 / 32 tf32)
   int b_explicit_k;    // B tile K coordinates come from LoadEntry::wc0 instead of the running k column
-  int n_stages, stage_bytes;  // shared-memory operand ring: as many stages as fit next to the epilogue scratch
+  int b_kstep;         // K coordinate advance of the B tiles per k-step (X3 packed weights: 2 * kb_elems, hi + lo)
+  int b_lo_k;          // X3: K distance from a k-step's W_hi tile to its W_lo tile
+  // shared-memory operand rings (as many slots as fit next to the epilogue scratch): A slots hold one entry's A box,
+  // B slots the weight tiles of one k-step
+  int n_aslots, a_slot_bytes, n_bslots, b_slot_bytes;
   // X3 (split bf16) epilogue: the lo parts of the output / residual rows sit this many elements behind the hi parts
   long long out_lo_off, res_lo_off;
   // epilogue
@@ -113,7 +119,7 @@ struct GemmParams {
   float* gnb_part;      // [tiles_m * bb][N][2]
 };
 
-constexpr int kMaxStages = 6;
+constexpr int kMaxSlots = 8;  // per ring
 constexpr int kMaxDynSmem = 232448;  // 227 KB: the opt-in limit of dynamic shared memory per block on sm_90
 template <int BLOCK_N>
 struct GemmCfg {
@@ -122,8 +128,9 @@ struct GemmCfg {
   // accumulator staging [128 rows][kAccPitch]: the 4-float pad keeps the row-per-lane float4 reads conflict-free
   static constexpr int kAccPitch = BLOCK_N + 4;
   static constexpr int kAccFloats = kBlockM * kAccPitch;
-  // everything but the operand ring: alignment slack, accumulator staging, epilogue scratch, mbarriers (kMaxStages)
-  static constexpr int kFixedBytes = 1024 + kAccFloats * 4 + kStatsFloats * 4 + 2 * kMaxStages * 8;
+  // everything but the operand rings: alignment slack, accumulator staging, epilogue scratch, mbarriers (full / empty of
+  // both rings)
+  static constexpr int kFixedBytes = 1024 + kAccFloats * 4 + kStatsFloats * 4 + 4 * kMaxSlots * 8;
 };
 constexpr int kRegsProducer = 40, kRegsConsumer = 232;  // 128 x 40 + 256 x 232 <= 65 536
 
@@ -132,23 +139,27 @@ __device__ __forceinline__ uint64_t kdesc(uint32_t saddr) { return make_wgmma_de
 
 // GNB: GroupNorm-backward epilogue (see GemmParams::gnb_c) -- a separate instantiation, so the inference kernels'
 // code is untouched.
-// X3: split-bf16 operands (see Precision::kBF16X3): the main loop is unchanged (the three partial products are extra
-// k-steps of the load table); the epilogue reads residuals and stores outputs as (hi, lo) bf16 pairs. GNB && X3 reads
+// X3: split-bf16 operands (see Precision::kBF16X3): an entry loads the hi and lo parts of its A box, a k-step the W_hi and
+// W_lo tiles. Per k16 step, A_hi . [W_hi; W_lo] is one m64n(2 BLOCK_N) wgmma into acc[0, BLOCK_N) (first half: the W_hi
+// columns, second half: W_lo), then A_lo . W_hi an m64nBLOCK_N one into acc[0, BLOCK_N / 2); after the last k-step the
+// second half is folded into the first. The epilogue reads residuals and stores outputs as (hi, lo) bf16 pairs. GNB && X3 reads
 // the GroupNorm input as hi + lo, stores dy as (hi, lo) and takes the SiLU derivative from ex2/rcp (tanh.approx's 2^-11
 // would cap the gradient accuracy near 5e-4).
 template <int BLOCK_N, bool TF32, bool GNB = false, bool X3 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   using Cfg = GemmCfg<BLOCK_N>;
-  const int NS = p.n_stages;
-  const uint32_t kStageBytesRt = (uint32_t)p.stage_bytes;
+  constexpr int kParts = X3 ? 2 : 1;  // operand parts per A box / per k-step of weights
+  const int NA = p.n_aslots, NB = p.n_bslots;
+  const uint32_t a_slot = (uint32_t)p.a_slot_bytes, b_slot = (uint32_t)p.b_slot_bytes;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* s_acc = reinterpret_cast<float*>(smem + NS * p.stage_bytes);
+  float* s_acc = reinterpret_cast<float*>(smem + NA * p.a_slot_bytes + NB * p.b_slot_bytes);
   float* s_stats = s_acc + Cfg::kAccFloats;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_stats + Cfg::kStatsFloats);
 
-  const uint32_t stage0 = smem_u32(smem);
-  const uint32_t full = smem_u32(bars), empty = full + 8 * kMaxStages;
+  const uint32_t a_ring = smem_u32(smem), b_ring = a_ring + NA * a_slot;
+  const uint32_t a_full = smem_u32(bars), a_empty = a_full + 8 * kMaxSlots;
+  const uint32_t b_full = a_empty + 8 * kMaxSlots, b_empty = b_full + 8 * kMaxSlots;
 
   // (broadcast from lane 0, so the compiler can treat the warpgroup branches as warp-uniform)
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
@@ -159,7 +170,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
   }
   if (warp == 1 && lane == 0) {
     // full: the producer's expect_tx arrival; empty: one arrival per consumer warpgroup
-    for (int i = 0; i < NS; ++i) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 2); }
+    for (int i = 0; i < NA; ++i) { mbar_init(a_full + 8 * i, 1); mbar_init(a_empty + 8 * i, 2); }
+    for (int i = 0; i < NB; ++i) { mbar_init(b_full + 8 * i, 1); mbar_init(b_empty + 8 * i, 2); }
     fence_barrier_init();
     fence_proxy_async();
   }
@@ -197,7 +209,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
     setmaxnreg_dec<kRegsProducer>();
     if (warp == 0) {
       // ------------------------------------------------------------------ TMA producer
-      uint32_t st = 0, ph = 0;
+      uint32_t as = 0, aph = 0, bs = 0, bph = 0;
       for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
         int x0, y0, z0, b0, n0;
         decode(tile, x0, y0, z0, b0, n0);
@@ -206,33 +218,39 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
         const int bcoord = p.b_batched ? b0 : 0;
         for (int sg = 0; sg < p.n_segs; ++sg) {
           const GemmSeg& seg = p.segs[sg];
-          const uint32_t group_bytes = seg.a_bytes + seg.nk * Cfg::kBTileBytes;
           for (int g = 0; g < seg.n_groups; ++g, ++gi) {
             if (gi < g_lo || gi >= g_hi) {  // another CTA's share of this tile's K range
-              kcol += seg.nk * p.kb_elems;
+              kcol += seg.nk * p.b_kstep;
               ++l;
               continue;
             }
-            // the table entry of this group is fetched before blocking on the stage
+            // the table entry of this group is fetched before blocking on the slot
             const uint4 raw = __ldg(reinterpret_cast<const uint4*>(p.loads + l));
-            mbar_wait(empty + 8 * st, ph ^ 1);
+            const LoadEntry& en = reinterpret_cast<const LoadEntry&>(raw);
+            mbar_wait(a_empty + 8 * as, aph ^ 1);
             if (elect_one()) {
-              const uint32_t sbase = stage0 + st * kStageBytesRt;
-              int kc = kcol;
-              const uint32_t bar = full + 8 * st;
-              mbar_expect_tx(bar, group_bytes);
-              const LoadEntry& en = reinterpret_cast<const LoadEntry&>(raw);
-              if (X3 && p.b_explicit_k) kc = en.wc0;
-              tma_load_5d(&p.amap[en.tmap], bar, sbase, en.c0, x0 + en.dx, y0 + en.dy, z0 + en.dz, b0);
-              for (int j = 0; j < seg.nk; ++j) {
-                tma_load_3d(&p.bmap, bar, sbase + seg.a_stride + j * Cfg::kBTileBytes, kc, n0, bcoord);
-                kc += p.kb_elems;
-              }
+              const uint32_t abase = a_ring + as * a_slot, bar = a_full + 8 * as;
+              mbar_expect_tx(bar, kParts * seg.a_bytes);
+              tma_load_5d(&p.amap[en.tmap], bar, abase, en.c0, x0 + en.dx, y0 + en.dy, z0 + en.dz, b0);
+              if constexpr (X3) tma_load_5d(&p.amap[en.tmap_lo], bar, abase + seg.a_stride, en.c0, x0 + en.dx, y0 + en.dy, z0 + en.dz, b0);
             }
             __syncwarp();
-            kcol += seg.nk * p.kb_elems;
+            if (++as == (uint32_t)NA) { as = 0; aph ^= 1; }
+            int kc = (X3 && p.b_explicit_k) ? (int)en.wc0 : kcol;
+            for (int j = 0; j < seg.nk; ++j) {
+              mbar_wait(b_empty + 8 * bs, bph ^ 1);
+              if (elect_one()) {
+                const uint32_t bbase = b_ring + bs * b_slot, bar = b_full + 8 * bs;
+                mbar_expect_tx(bar, kParts * Cfg::kBTileBytes);
+                tma_load_3d(&p.bmap, bar, bbase, kc, n0, bcoord);
+                if constexpr (X3) tma_load_3d(&p.bmap, bar, bbase + Cfg::kBTileBytes, kc + p.b_lo_k, n0, bcoord);
+              }
+              __syncwarp();
+              kc += p.b_kstep;
+              if (++bs == (uint32_t)NB) { bs = 0; bph ^= 1; }
+            }
+            kcol += seg.nk * p.b_kstep;
             ++l;
-            if (++st == (uint32_t)NS) { st = 0; ph ^= 1; }
           }
         }
       }
@@ -260,42 +278,67 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
       want_cols = (p.stats != nullptr || p.gnb_part != nullptr) ? 1 : 0;
       asm volatile("" : "+r"(want_cols));
     }
-    uint32_t st = 0, ph = 0;
+    uint32_t as = 0, aph = 0, bs = 0, bph = 0;
     for (int tile = first_tile; tile < total_tiles; tile += tile_step, ++it) {
       const int vit = it;
       // ---------------------------------------------------------------- main loop: wgmma over the k-step groups
-      float acc[BLOCK_N / 2];
+      constexpr int kAccRegs = X3 ? BLOCK_N : BLOCK_N / 2;  // X3: [W_hi columns | W_lo columns] until the fold
+      float acc[kAccRegs];
+      float (&acc_hi)[BLOCK_N / 2] = *reinterpret_cast<float (*)[BLOCK_N / 2]>(acc);
 #pragma unroll
-      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+      for (int i = 0; i < kAccRegs; ++i) acc[i] = 0.f;
       {
         int gi = 0, g_lo, g_hi;
         split_range(tile, g_lo, g_hi);
-        int prev = -1;  // stage whose wgmmas may still be reading it
+        // slots whose wgmmas may still be reading them: each is handed back once the next k-step's wait shows them retired
+        int prev_b = -1, prev_a = -1;
         const uint32_t a_row0 = (uint32_t)wg * 64 * kRowBytes;
         for (int sg = 0; sg < p.n_segs; ++sg) {
           // (by reference: the segment stays in parameter space, where the compiler can see its fields are uniform)
           const GemmSeg& sgm = p.segs[sg];
           for (int g = 0; g < sgm.n_groups; ++g, ++gi) {
             if (gi < g_lo || gi >= g_hi) continue;
-            mbar_wait(full + 8 * st, ph);
-            const uint32_t sbase = stage0 + st * kStageBytesRt;
+            mbar_wait(a_full + 8 * as, aph);
+            const uint32_t abase = a_ring + as * a_slot + a_row0;
             for (int j = 0; j < sgm.nk; ++j) {
-              const uint64_t ad = kdesc(sbase + j * sgm.jbytes + a_row0);
-              const uint64_t bd = kdesc(sbase + sgm.a_stride + j * Cfg::kBTileBytes);
+              mbar_wait(b_full + 8 * bs, bph);
+              const uint64_t ad = kdesc(abase + j * sgm.jbytes);
+              const uint64_t bd = kdesc(b_ring + bs * b_slot);
               wgmma_fence();  // directly in front of the straight-line wgmmas: no branch between the fence and them
+              if constexpr (X3) {
+                const uint64_t adl = kdesc(abase + sgm.a_stride + j * sgm.jbytes);
 #pragma unroll
-              for (int k = 0; k < kRowBytes / 32; ++k) wgmma_kmajor<BLOCK_N, TF32>(acc, ad + 2 * k, bd + 2 * k, 1u);
+                for (int k = 0; k < kRowBytes / 32; ++k) wgmma_kmajor<2 * BLOCK_N, false>(acc, ad + 2 * k, bd + 2 * k, 1u);
+                wgmma_fence();  // the next wgmmas have another shape: order their accumulator accesses after these
+#pragma unroll
+                for (int k = 0; k < kRowBytes / 32; ++k) wgmma_kmajor<BLOCK_N, false>(acc_hi, adl + 2 * k, bd + 2 * k, 1u);
+              } else {
+#pragma unroll
+                for (int k = 0; k < kRowBytes / 32; ++k) wgmma_kmajor<BLOCK_N, TF32>(acc, ad + 2 * k, bd + 2 * k, 1u);
+              }
+              wgmma_commit();
+              wgmma_wait<1>();  // the previous k-step's wgmmas have retired: hand its slots back to the producer
+              if (wt == 0) {
+                if (prev_b >= 0) mbar_arrive(b_empty + 8 * prev_b);
+                if (prev_a >= 0) mbar_arrive(a_empty + 8 * prev_a);
+              }
+              prev_b = (int)bs;
+              prev_a = j + 1 == sgm.nk ? (int)as : -1;
+              if (++bs == (uint32_t)NB) { bs = 0; bph ^= 1; }
             }
-            wgmma_commit();
-            wgmma_wait<1>();  // the previous group's wgmmas have retired: hand its stage back to the producer
-            if (prev >= 0 && wt == 0) mbar_arrive(empty + 8 * prev);
-            prev = (int)st;
-            if (++st == (uint32_t)NS) { st = 0; ph ^= 1; }
+            if (++as == (uint32_t)NA) { as = 0; aph ^= 1; }
           }
         }
         wgmma_wait<0>();
         fence_operands(acc);
-        if (prev >= 0 && wt == 0) mbar_arrive(empty + 8 * prev);
+        if (wt == 0) {
+          if (prev_b >= 0) mbar_arrive(b_empty + 8 * prev_b);
+          if (prev_a >= 0) mbar_arrive(a_empty + 8 * prev_a);
+        }
+        if constexpr (X3) {
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] += acc[BLOCK_N / 2 + i];
+        }
       }
       int x0, y0, z0, b0, n0;
       decode(tile, x0, y0, z0, b0, n0);

@@ -116,6 +116,7 @@ class UNet {
   double flops_per_sample() const { return flops_ / cfg_.max_batch; }
   size_t arena_bytes() const { return arena_bytes_; }
   int num_gemm_launches() const { return (int)gemms_.size(); }
+  const GemmOp& gemm(int i) const { return *gemms_.at(i); }
   int num_steps() const { return (int)steps_.size(); }
   const UNetConfig& cfg() const { return cfg_; }
   // per-GEMM timing breakdown of one forward (ms), for profiling

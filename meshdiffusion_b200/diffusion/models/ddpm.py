@@ -559,6 +559,16 @@ class ScoreNet(nn.Module):
         return dict(flops_per_sample=fl.value, arena_bytes=ar.value, gemm_launches=ng.value, steps=ns.value,
                     max_batch=self._engine_batch, precision=self.precision)
 
+    def gemm_ops(self):
+        """Per forward GEMM launch at the engine's batch: [(step name, executed FLOPs, bytes TMA fills into shared memory)]."""
+        L = _native.lib()
+        rows = []
+        for i in range(self.engine_info()["gemm_launches"]):
+            name, fl, fb = ctypes.c_char_p(), ctypes.c_double(), ctypes.c_double()
+            _native.check(L.mdb_unet_gemm_ops(self._handle, i, ctypes.byref(name), ctypes.byref(fl), ctypes.byref(fb)))
+            rows.append((name.value.decode(), fl.value, fb.value))
+        return rows
+
     def profile(self, x, labels):
         """One profiled forward: [(step name, device ms)]."""
         L = _native.lib()
