@@ -44,7 +44,9 @@ typedef struct mdb_unet_config {
 } mdb_unet_config;
 
 int mdb_unet_create(const mdb_unet_config* cfg, mdb_unet** out);
-/* Plan only (parameter table, arena size); no GPU needed. forward()/set_param() must not be called on it. */
+/* Plan only, no GPU needed: built by the same code as mdb_unet_create, so it answers the parameter table, arena size,
+ * step and GEMM counts, mdb_unet_gemm_ops, FLOPs, mdb_unet_train_info and mdb_unet_grad_ready. It cannot run:
+ * set/get_param, commit, forward, backward* and profile* return an error. */
 int mdb_unet_create_dry(const mdb_unet_config* cfg, mdb_unet** out);
 void mdb_unet_destroy(mdb_unet* net);
 

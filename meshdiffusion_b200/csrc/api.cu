@@ -303,7 +303,9 @@ int mdb_conv3d(const void* x, int B, int cin, int z, int y_, int x_, const float
   if (rowbias) g.set_rowbias(rowbias, cout);
   if (residual) g.set_residual(residual, cout, (long long)xo * yo * zo * cout, false);
   if (stats) g.set_stats(stats);
-  g.finalize(s, true);
+  g.finalize();
+  g.upload(s);
+  g.repack(s);
   g.launch(s);
   MDB_CUDA_CHECK(cudaStreamSynchronize(s));
   MDB_API_END
@@ -355,7 +357,9 @@ int mdb_conv3d_backward_prec(const void* dy, const void* x, const float* w, int 
     g.set_output(pr, x_, y_, z, B, cin, dx, cin, false);
     if (ksize == 1) { WSrc ws{w, 1, (long long)cin, 0, cout}; g.add_pointwise_w({ady}, &ws); }
     else g.add_conv_dgrad(ady, w, cin, ksize);
-    g.finalize(s, true);
+    g.finalize();
+    g.upload(s);
+    g.repack(s);
     g.launch(s);
     MDB_CUDA_CHECK(cudaStreamSynchronize(s));
   }

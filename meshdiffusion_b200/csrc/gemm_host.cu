@@ -118,7 +118,7 @@ void GemmOp::enable_splits(int S, float* scratch) {
   if (S <= 1) return;
   if (p.ocs != 1 || p.out_fp32 || p.bias_on_m || p.alpha != 1.f || p.res_fp32)
     throw std::runtime_error("mdb: split-K is only wired for plain NDHWC conv outputs");
-  if (p.osx != (long long)p.N * parts(prec) || (p.res && p.rsx != (long long)p.N * parts(prec)))
+  if (p.osx != (long long)p.N * parts(prec) || (p.rsx && p.rsx != (long long)p.N * parts(prec)))
     throw std::runtime_error("mdb: split-K needs dense [B][V][N] output / residual");
   splits = S;
   p.splits = S;
@@ -172,12 +172,13 @@ void GemmOp::set_output(Precision pr, int X, int Y, int Z, int B, int N, void* o
 }
 
 int GemmOp::add_amap(const Act& a, int halo, int sub, int px, int py, int pz, int part) {
-  if (n_amaps >= kMaxAMaps) throw std::runtime_error("mdb: too many A tensor maps");
+  if ((int)amaps_.size() >= kMaxAMaps) throw std::runtime_error("mdb: too many A tensor maps");
   if (halo > 0 && (geo.bz != 1 || geo.bb != 1)) throw std::runtime_error("mdb: halo needs a (bx,by,1,1) tile");
   const long long es = esize(prec);
   const long long prow = a.row() * parts(prec);  // physical row pitch in elements
-  uint64_t dims[5], strides[4];
-  uint32_t box[5];
+  MapDesc m;
+  m.rank = 5;
+  uint64_t* dims = m.dims; uint64_t* strides = m.strides; uint32_t* box = m.box;
   char* base = static_cast<char*>(a.ptr) + (long long)part * a.row() * es;
   if (sub == 1) {
     dims[0] = a.C; dims[1] = a.X; dims[2] = a.Y; dims[3] = a.Z; dims[4] = a.B;
@@ -190,8 +191,9 @@ int GemmOp::add_amap(const Act& a, int halo, int sub, int px, int py, int pz, in
     base += px * sx + py * sy + pz * sz;
   }
   box[0] = kb_elems(prec); box[1] = geo.bx; box[2] = geo.by + halo; box[3] = geo.bz; box[4] = geo.bb;
-  encode_map(&p.amap[n_amaps], prec, 5, base, dims, strides, box);
-  return n_amaps++;
+  m.base = base;
+  amaps_.push_back(m);
+  return (int)amaps_.size() - 1;
 }
 
 void GemmOp::add_load_x(int tm_hi, int tm_lo, int nk, int rows, int jrows, int dx, int dy, int dz, int c0, int wsrc,
@@ -299,7 +301,6 @@ void GemmOp::add_conv_up2(const Act& s, const float* w8, int px, int py, int pz)
 void GemmOp::add_pointwise(const std::vector<Act>& srcs, const float* w, bool w_in_out) {
   int ctot = 0;
   for (auto& s : srcs) ctot += s.C;
-  if (!w) { add_pointwise_w(srcs, nullptr); return; }
   WSrc ws = w_in_out ? WSrc{w, 1, (long long)p.N, 0, ctot} : WSrc{w, (long long)ctot, 1, 0, ctot};
   add_pointwise_w(srcs, &ws);
 }
@@ -336,12 +337,12 @@ void GemmOp::set_gn_backward(const void* x0, long long ld0, int c0, const void* 
                              float* part) {
   if (prec == kTF32 || p.out_fp32 || p.ocs != 1)
     throw std::runtime_error("mdb: the GroupNorm-backward epilogue is built for bf16 / split-bf16 NDHWC outputs");
-  if (p.N % 32 != 0 || (x1 && c0 % 32 != 0)) throw std::runtime_error("mdb: GroupNorm-backward epilogue needs 32-channel aligned sources");
+  if (p.N % 32 != 0 || (ld1 > 0 && c0 % 32 != 0)) throw std::runtime_error("mdb: GroupNorm-backward epilogue needs 32-channel aligned sources");
   if (splits > 1) throw std::runtime_error("mdb: GroupNorm-backward epilogue cannot be combined with split-K");
   gnb = true;
   p.res = x0; p.res_fp32 = 0; p.batch_fastest = 0;
   p.rsx = ld0; p.rsy = ld0 * p.X; p.rsz = ld0 * p.X * p.Y; p.rsb = ld0 * p.X * p.Y * p.Z;
-  p.res1 = x1; p.res_c0 = x1 ? c0 : p.N;
+  p.res1 = x1; p.res_c0 = ld1 > 0 ? c0 : p.N;
   p.r1sx = ld1; p.r1sy = ld1 * p.X; p.r1sz = ld1 * p.X * p.Y; p.r1sb = ld1 * p.X * p.Y * p.Z;
   p.res_lo_off = 0; p.res1_lo_off = 0;
   if (prec == kBF16X3) {  // (hi, lo) rows: physical pitches twice the logical ones, lo parts one logical row behind
@@ -354,11 +355,13 @@ void GemmOp::set_gn_backward(const void* x0, long long ld0, int c0, const void* 
   p.gnb_part = part;
 }
 
-void GemmOp::encode_bmap(void* ptr, int K, int N, int batch, long long rsb, long long bsb) {
-  uint64_t dims[3] = {(uint64_t)K, (uint64_t)N, (uint64_t)batch};
-  uint64_t strides[2] = {(uint64_t)rsb, (uint64_t)bsb};
-  uint32_t box[3] = {(uint32_t)kb_elems(prec), (uint32_t)block_n, 1};
-  encode_map(&p.bmap, prec, 3, ptr, dims, strides, box);
+MapDesc GemmOp::b_desc(void* ptr, long long K, int N, int batch, long long rsb, long long bsb) const {
+  MapDesc m;
+  m.base = ptr; m.rank = 3;
+  m.dims[0] = (uint64_t)K; m.dims[1] = (uint64_t)N; m.dims[2] = (uint64_t)batch;
+  m.strides[0] = (uint64_t)rsb; m.strides[1] = (uint64_t)bsb;
+  m.box[0] = (uint32_t)kb_elems(prec); m.box[1] = (uint32_t)block_n; m.box[2] = 1;
+  return m;
 }
 
 void GemmOp::set_b_activation(void* ptr, int K, int N, int batch, long long rs, long long bs) {
@@ -369,10 +372,10 @@ void GemmOp::set_b_activation(void* ptr, int K, int N, int batch, long long rs, 
     // rows are (hi, lo) pairs: the lo parts are addressed as K coordinates [rs, rs + K) of the same map
     if (K % kb_elems(prec) != 0) throw std::runtime_error("mdb: X3 activation-B operands need K to be a multiple of 64");
     b_lo_off = rs;
-    encode_bmap(ptr, (int)(rs + K), N, batch, 2 * rs * es, 2 * bs * es);
+    bmap_ = b_desc(ptr, (int)(rs + K), N, batch, 2 * rs * es, 2 * bs * es);
     return;
   }
-  encode_bmap(ptr, K, N, batch, rs * es, bs * es);
+  bmap_ = b_desc(ptr, K, N, batch, rs * es, bs * es);
 }
 
 // ------------------------------------------------------------------ weight packing (device gather)
@@ -462,7 +465,7 @@ void GemmOp::repack(cudaStream_t stream) {
   MDB_CUDA_CHECK(cudaGetLastError());
 }
 
-void GemmOp::finalize(cudaStream_t stream, bool pack) {
+void GemmOp::finalize() {
   if (loads.empty()) throw std::runtime_error("mdb: GemmOp without loads");
   p.b_explicit_k = 0;
   p.b_kstep = kb_elems(prec) * parts(prec);  // packed weights: a k-step's tiles sit side by side (X3: hi, lo)
@@ -474,9 +477,7 @@ void GemmOp::finalize(cudaStream_t stream, bool pack) {
     p.b_explicit_k = 1;
     p.b_lo_k = (int)b_lo_off;
   }
-  MDB_CUDA_CHECK(cudaMalloc(&d_loads, loads.size() * sizeof(LoadEntry)));
-  MDB_CUDA_CHECK(cudaMemcpyAsync(d_loads, loads.data(), loads.size() * sizeof(LoadEntry), cudaMemcpyHostToDevice, stream));
-  p.loads = d_loads;
+  if (!b_from_act) p.b_batched = 0;
   p.n_loads = (int)loads.size();
   if (p.splits < 1) p.splits = 1;
   // pipeline segments: runs of identical entries. An entry's A box (X3: both parts) takes an A slot, the weight tiles of
@@ -506,15 +507,24 @@ void GemmOp::finalize(cudaStream_t stream, bool pack) {
     }
   }
   if (p.splits > p.total_groups) { p.splits = p.total_groups; splits = p.splits; }
+}
+
+void GemmOp::upload(cudaStream_t stream) {
+  for (size_t i = 0; i < amaps_.size(); ++i) {
+    const MapDesc& m = amaps_[i];
+    encode_map(&p.amap[i], prec, m.rank, m.base, m.dims, m.strides, m.box);
+  }
+  MDB_CUDA_CHECK(cudaMalloc(&d_loads, loads.size() * sizeof(LoadEntry)));
+  MDB_CUDA_CHECK(cudaMemcpyAsync(d_loads, loads.data(), loads.size() * sizeof(LoadEntry), cudaMemcpyHostToDevice, stream));
+  p.loads = d_loads;
   if (!b_from_act) {
     const long long ktot = 1LL * ksteps * kb_elems(prec) * parts(prec);
     const long long bytes = ktot * p.N * esize(prec);
     MDB_CUDA_CHECK(cudaMalloc(&d_wpacked, bytes));
     owns_w = true;
-    p.b_batched = 0;
-    encode_bmap(d_wpacked, (int)ktot, p.N, 1, ktot * esize(prec), bytes);
-    if (pack) repack(stream);
+    bmap_ = b_desc(d_wpacked, ktot, p.N, 1, ktot * esize(prec), bytes);
   }
+  encode_map(&p.bmap, prec, bmap_.rank, bmap_.base, bmap_.dims, bmap_.strides, bmap_.box);
   MDB_CUDA_CHECK(cudaStreamSynchronize(stream));
 }
 

@@ -48,6 +48,17 @@ struct WSrc {
 struct Geometry { int bx, by, bz, bb; };
 Geometry pick_geometry(int X, int Y, int Z);
 
+// A TMA tensor map as described on the host (encode_map's arguments), encoded by GemmOp::upload
+struct MapDesc {
+  void* base = nullptr;
+  int rank = 0;
+  uint64_t dims[5] = {}, strides[4] = {};  // strides in bytes, rank - 1 of them
+  uint32_t box[5] = {};
+};
+
+// Built in three steps: the add_* / set_* calls and finalize() describe the op on the host (no GPU needed: flops,
+// fill_bytes and the launch geometry are then known); upload() encodes the tensor maps and allocates the device tables;
+// repack() packs the weights.
 class GemmOp {
  public:
   GemmParams p{};
@@ -56,7 +67,6 @@ class GemmOp {
   int splits = 1;     // split-K factor (small problems: few tiles, long K)
   std::vector<LoadEntry> loads;
   std::vector<WSrc> wsrcs;
-  int n_amaps = 0;
   int ksteps = 0;  // k-steps of the load table (X3: each with a W_hi and a W_lo tile)
   // device-owned
   LoadEntry* d_loads = nullptr;
@@ -112,7 +122,7 @@ class GemmOp {
   void set_residual(const void* res, long long ldr, long long batch_stride, bool fp32);
   void set_stats(long long* stats) { p.stats = stats; }
   // GroupNorm-backward epilogue (training data gradients, bf16 or split bf16 with logical pitches): the GEMM result is dL/da of a GroupNorm(+SiLU)(+dropout)
-  // whose INPUT is the channel concatenation of x0 (c0 channels, row pitch ld0) and x1; `consts` = [B][N] float4 from
+  // whose INPUT is the channel concatenation of x0 (c0 channels, row pitch ld0) and x1 (ld1 = 0: none); `consts` = [B][N] float4 from
   // launch_gn_consts; `part` = [gnb_rows()][N][2] per-tile partials for launch_gnb_tile_reduce. Dropout of the layer is
   // supplied per launch through rt_drop_*.
   void set_gn_backward(const void* x0, long long ld0, int c0, const void* x1, long long ld1, const void* consts, int silu, float* part);
@@ -125,9 +135,12 @@ class GemmOp {
   // Split-K over `S` CTAs per tile; `scratch` holds S fp32 copies of the output ([B][V][N] each). Call before finalize.
   void enable_splits(int S, float* scratch);
 
-  // Packs weights (device gather kernel), uploads the table, encodes the B map. Call after all add_* calls.
-  void finalize(cudaStream_t stream, bool pack = true);
-  // Re-pack weights only (after a weight reload into the same source buffers).
+  // Host only, after all add_* / set_* calls: checks the load table and derives the pipeline segments, the operand slot
+  // sizes and the final split-K factor.
+  void finalize();
+  // After finalize: encodes the tensor maps, uploads the load table and allocates the packed-weight buffer.
+  void upload(cudaStream_t stream);
+  // Packs the weights (device gather kernel) into the uploaded buffer; again after every weight reload.
   void repack(cudaStream_t stream);
   // B <= the batch the op was built for; out_override replaces the output pointer (user buffers).
   void launch(cudaStream_t stream, int B = -1, void* out_override = nullptr) const;
@@ -141,7 +154,9 @@ class GemmOp {
   int nk_max = 0;       // most k-steps of one entry
   void pick_slots(GemmParams& q) const;
   long long b_lo_off = 0;  // X3 activation-B: K coordinate of the lo parts
-  void encode_bmap(void* ptr, int K, int N, int batch, long long row_stride_bytes, long long batch_stride_bytes);
+  std::vector<MapDesc> amaps_;  // p.amap[i] once uploaded
+  MapDesc bmap_;                // p.bmap once uploaded (packed weights: described by upload itself)
+  MapDesc b_desc(void* ptr, long long K, int N, int batch, long long row_stride_bytes, long long batch_stride_bytes) const;
 };
 
 int sm_count();

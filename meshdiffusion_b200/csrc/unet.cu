@@ -59,6 +59,7 @@ void Arena::release(size_t off) {
 
 // ------------------------------------------------------------------ UNet plumbing
 void* UNet::dmalloc(size_t bytes, bool zero) {
+  if (dry_) return nullptr;
   void* p = nullptr;
   MDB_CUDA_CHECK(cudaMalloc(&p, bytes ? bytes : 16));
   if (zero) MDB_CUDA_CHECK(cudaMemset(p, 0, bytes ? bytes : 16));
@@ -66,19 +67,19 @@ void* UNet::dmalloc(size_t bytes, bool zero) {
   return p;
 }
 
-float* UNet::P(const std::string& name, std::vector<long long> shape, float* external) {
+float* UNet::P(const std::string& name, std::vector<long long> shape, bool external, float* slice) {
   auto it = pindex_.find(name);
   if (it == pindex_.end()) {
     ParamInfo pi;
     pi.name = name; pi.shape = shape; pi.numel = 1;
     for (auto d : shape) pi.numel *= d;
-    pi.external = external != nullptr;
+    pi.external = external;
     pindex_[name] = (int)params_.size();
     params_.push_back(pi);
     it = pindex_.find(name);
   }
   ParamInfo& pi = params_[it->second];
-  if (external) { pi.d = external; pi.external = true; }
+  if (external) pi.d = slice;
   return pi.d;
 }
 
@@ -87,7 +88,7 @@ TensP UNet::new_act(int C, int R, bool stats) {
   t->C = C; t->R = R;
   t->bytes = (size_t)cfg_.max_batch * R * R * R * C * esize(prec_) * parts(prec_);
   t->off = arena_.alloc(t->bytes);
-  t->ptr = dry_ ? nullptr : arena_base_ + t->off;
+  t->ptr = at(t->off);
   if (stats) {
     const size_t n = (size_t)cfg_.max_batch * C * kStatWords;
     t->stats = dry_ ? nullptr : stats_base_ + stats_cursor_;
@@ -119,7 +120,7 @@ UNet::Scratch UNet::split_begin(int R, int N, int cin_total, int taps) {
   if (s.S > 1) {
     const size_t bytes = (size_t)s.S * cfg_.max_batch * R * R * R * N * sizeof(float);
     s.off = arena_.alloc(bytes);
-    s.ptr = dry_ ? nullptr : reinterpret_cast<float*>(arena_base_ + s.off);
+    s.ptr = reinterpret_cast<float*>(at(s.off));
     s.active = true;
   }
   return s;
@@ -138,6 +139,13 @@ GemmOp* UNet::new_gemm(const std::string& name, bool commit_time) {
   return raw;
 }
 
+void UNet::gemm_step(std::vector<Step>& steps, GemmOp* g, std::function<void(cudaStream_t, int)> fn, int kind) {
+  g->finalize();
+  if (!dry_) g->upload(0);
+  if (!fn) fn = [g](cudaStream_t s, int B) { g->launch(s, B); };
+  steps.push_back({g->name, fn, kind});
+}
+
 // GroupNorm(32, eps 1e-6) + optional SiLU over the channel concatenation of `ins` (torch.cat is never materialised
 // in raw form: only this normalised copy, which is the conv's A operand, exists).
 TensP UNet::gn(const std::string& pname, const std::vector<TensP>& ins, bool silu, int drop_layer) {
@@ -147,7 +155,6 @@ TensP UNet::gn(const std::string& pname, const std::vector<TensP>& ins, bool sil
   float* gamma = P(pname + ".weight", {C});
   float* beta = P(pname + ".bias", {C});
   TensP y = new_act(C, R, false);
-  if (dry_) return y;
   NormActArgs na{};
   na.x0 = ins[0]->ptr; na.C0 = ins[0]->C; na.ld0 = ins[0]->C;
   na.x1 = ins.size() > 1 ? ins[1]->ptr : nullptr; na.C1 = ins.size() > 1 ? ins[1]->C : 0; na.ld1 = na.C1;
@@ -180,30 +187,27 @@ TensP UNet::resblock(const std::vector<TensP>& ins, int out_ch, int midx) {
   float* b0 = P(pre + "Conv_0.bias", {out_ch});
   const int doff = dense_cursor_;
   dense_cursor_ += out_ch;
-  P(pre + "Dense_0.weight", {out_ch, tdim}, dry_ ? nullptr : dense_w_ + (size_t)doff * tdim);
-  P(pre + "Dense_0.bias", {out_ch}, dry_ ? nullptr : dense_b_ + doff);
-  if (dry_) { params_[pindex_[pre + "Dense_0.weight"]].external = true; params_[pindex_[pre + "Dense_0.bias"]].external = true; }
+  P(pre + "Dense_0.weight", {out_ch, tdim}, true, dense_w_ + (size_t)doff * tdim);
+  P(pre + "Dense_0.bias", {out_ch}, true, dense_b_ + doff);
   TensP h = new_act(out_ch, R, true);
   Scratch sp0 = split_begin(R, out_ch, Cin, 27);
-  if (!dry_) {
-    GemmOp* g = new_gemm("res" + std::to_string(midx) + ".conv0");
-    g->set_output(prec_, R, R, R, mb, out_ch, h->ptr, out_ch, false);
-    g->add_conv({act_of(a)}, w0, 3, 1);
-    g->set_bias(b0);
-    g->set_rowbias(dense_out_ + doff, dense_total_);
-    g->set_stats(h->stats);
-    g->enable_splits(sp0.S, sp0.ptr);
-    g->finalize(0, false);
-    add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-  }
+  GemmOp* g0 = new_gemm("res" + std::to_string(midx) + ".conv0");
+  g0->set_output(prec_, R, R, R, mb, out_ch, h->ptr, out_ch, false);
+  g0->add_conv({act_of(a)}, w0, 3, 1);
+  g0->set_bias(b0);
+  g0->set_rowbias(dense_out_ + doff, dense_total_);
+  g0->set_stats(h->stats);
+  g0->enable_splits(sp0.S, sp0.ptr);
+  gemm_step(steps_, g0);
   split_end(sp0);
   release(a);
   TensP a2 = gn(pre + "GroupNorm_1", {h}, true, midx);
   release(h);
   float* w1 = P(pre + "Conv_1.weight", {out_ch, out_ch, 3, 3, 3});
   float* b1 = P(pre + "Conv_1.bias", {out_ch});
+  const bool nin = Cin != out_ch;
   float* wn = nullptr; float* bn = nullptr;
-  if (Cin != out_ch) {
+  if (nin) {
     wn = P(pre + "NIN_0.W", {Cin, out_ch});
     bn = P(pre + "NIN_0.b", {out_ch});
   } else if (ins.size() != 1) {
@@ -211,26 +215,23 @@ TensP UNet::resblock(const std::vector<TensP>& ins, int out_ch, int midx) {
   }
   TensP out = new_act(out_ch, R, true);
   Scratch sp1 = split_begin(R, out_ch, out_ch, 27);
-  if (!dry_) {
-    GemmOp* g = new_gemm("res" + std::to_string(midx) + ".conv1");
-    g->set_output(prec_, R, R, R, mb, out_ch, out->ptr, out_ch, false);
-    g->add_conv({act_of(a2)}, w1, 3, 1);
-    if (wn) {
-      std::vector<Act> raw;
-      for (auto& t : ins) raw.push_back(act_of(t));
-      g->add_pointwise(raw, wn, true);
-      float* bsum = (float*)dmalloc(out_ch * 4);
-      commit_steps_.push_back({"bias:" + pre, [=](cudaStream_t s, int) { launch_add_vec(b1, bn, bsum, out_ch, s); }});
-      g->set_bias(bsum);
-    } else {
-      g->set_bias(b1);
-      g->set_residual(ins[0]->ptr, out_ch, (long long)R * R * R * out_ch, false);
-    }
-    g->set_stats(out->stats);
-    g->enable_splits(sp1.S, sp1.ptr);
-    g->finalize(0, false);
-    add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
+  GemmOp* g1 = new_gemm("res" + std::to_string(midx) + ".conv1");
+  g1->set_output(prec_, R, R, R, mb, out_ch, out->ptr, out_ch, false);
+  g1->add_conv({act_of(a2)}, w1, 3, 1);
+  if (nin) {
+    std::vector<Act> raw;
+    for (auto& t : ins) raw.push_back(act_of(t));
+    g1->add_pointwise(raw, wn, true);
+    float* bsum = (float*)dmalloc(out_ch * 4);
+    commit_steps_.push_back({"bias:" + pre, [=](cudaStream_t s, int) { launch_add_vec(b1, bn, bsum, out_ch, s); }});
+    g1->set_bias(bsum);
+  } else {
+    g1->set_bias(b1);
+    g1->set_residual(ins[0]->ptr, out_ch, (long long)R * R * R * out_ch, false);
   }
+  g1->set_stats(out->stats);
+  g1->enable_splits(sp1.S, sp1.ptr);
+  gemm_step(steps_, g1);
   split_end(sp1);
   if (train_) tape_resblock(ins, a, h, a2, out, out_ch, midx, doff);
   release(a2);
@@ -250,21 +251,18 @@ TensP UNet::attn(const TensP& x, int midx) {
     Bv[i] = P(pre + "NIN_" + std::to_string(i) + ".b", {C});
   }
   TensP qkv = new_act(3 * C, R, false);
-  if (!dry_) {
-    for (int i = 0; i < 3; ++i) {
-      GemmOp* g = new_gemm("attn" + std::to_string(midx) + ".nin" + std::to_string(i));
-      g->set_output(prec_, R, R, R, mb, C, (char*)qkv->ptr + (size_t)i * C * es, 3 * C, false);
-      g->add_pointwise({act_of(hn)}, W[i], true);
-      g->set_bias(Bv[i]);
-      g->finalize(0, false);
-      add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-    }
+  for (int i = 0; i < 3; ++i) {
+    GemmOp* g = new_gemm("attn" + std::to_string(midx) + ".nin" + std::to_string(i));
+    g->set_output(prec_, R, R, R, mb, C, (char*)qkv->ptr + (size_t)i * C * es, 3 * C, false);
+    g->add_pointwise({act_of(hn)}, W[i], true);
+    g->set_bias(Bv[i]);
+    gemm_step(steps_, g);
   }
   release(hn);
   // v^T [B][C][V] so that P.V has a K-major B operand
   TensP vT = new_act(C, R, false);
-  if (!dry_) {
-    const void* src = qkv->ptr; void* dst = vT->ptr; const int es = esize(prec_);
+  {
+    const void* src = qkv->ptr; void* dst = vT->ptr;
     if (prec_ == kBF16X3) {
       // qkv rows are [3C hi | 3C lo]; v^T rows become [V hi | V lo]
       add_step("attn" + std::to_string(midx) + ".vT", [=](cudaStream_t s, int B) {
@@ -278,41 +276,34 @@ TensP UNet::attn(const TensP& x, int midx) {
   auto S = std::make_shared<Tens>();
   S->bytes = (size_t)mb * V * V * 4;
   S->off = arena_.alloc(S->bytes);
-  S->ptr = dry_ ? nullptr : arena_base_ + S->off;
+  S->ptr = at(S->off);
   TensP O = new_act(C, R, false);
-  if (!dry_) {
-    GemmOp* g = new_gemm("attn" + std::to_string(midx) + ".qk");
-    g->set_output_strided(prec_, V, 1, 1, mb, V, S->ptr, V, 0, 0, (long long)V * V, true);
-    Act q; q.ptr = qkv->ptr; q.C = C; q.ld = 3 * C; q.X = V; q.Y = 1; q.Z = 1; q.B = mb;
-    g->add_pointwise({q}, nullptr, true);
-    g->set_b_activation((char*)qkv->ptr + (size_t)C * es, C, V, mb, 3 * C, (long long)V * 3 * C);
-    g->set_alpha(1.0f / std::sqrt((float)C));
-    g->finalize(0, false);
-    add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-    float* sp = (float*)S->ptr; const Precision pr = prec_;
-    add_step("attn" + std::to_string(midx) + ".softmax", [=](cudaStream_t s, int B) { launch_softmax_rows(sp, (long long)B * V, V, pr, s); });
-    GemmOp* g2 = new_gemm("attn" + std::to_string(midx) + ".pv");
-    g2->set_output_strided(prec_, V, 1, 1, mb, C, O->ptr, C, 0, 0, (long long)V * C, false);
-    Act pa; pa.ptr = S->ptr; pa.C = V; pa.ld = (prec_ == kBF16) ? 2 * V : V; pa.X = V; pa.Y = 1; pa.Z = 1; pa.B = mb;
-    g2->add_pointwise({pa}, nullptr, true);
-    g2->set_b_activation(vT->ptr, V, C, mb, V, (long long)C * V);
-    g2->finalize(0, false);
-    add_step(g2->name, [g2](cudaStream_t s, int B) { g2->launch(s, B); });
-  }
+  GemmOp* gqk = new_gemm("attn" + std::to_string(midx) + ".qk");
+  gqk->set_output_strided(prec_, V, 1, 1, mb, V, S->ptr, V, 0, 0, (long long)V * V, true);
+  Act q; q.ptr = qkv->ptr; q.C = C; q.ld = 3 * C; q.X = V; q.Y = 1; q.Z = 1; q.B = mb;
+  gqk->add_pointwise_w({q}, nullptr);
+  gqk->set_b_activation((char*)qkv->ptr + (size_t)C * es, C, V, mb, 3 * C, (long long)V * 3 * C);
+  gqk->set_alpha(1.0f / std::sqrt((float)C));
+  gemm_step(steps_, gqk);
+  float* sp = (float*)S->ptr; const Precision pr = prec_;
+  add_step("attn" + std::to_string(midx) + ".softmax", [=](cudaStream_t s, int B) { launch_softmax_rows(sp, (long long)B * V, V, pr, s); });
+  GemmOp* gpv = new_gemm("attn" + std::to_string(midx) + ".pv");
+  gpv->set_output_strided(prec_, V, 1, 1, mb, C, O->ptr, C, 0, 0, (long long)V * C, false);
+  Act pa; pa.ptr = S->ptr; pa.C = V; pa.ld = (prec_ == kBF16) ? 2 * V : V; pa.X = V; pa.Y = 1; pa.Z = 1; pa.B = mb;
+  gpv->add_pointwise_w({pa}, nullptr);
+  gpv->set_b_activation(vT->ptr, V, C, mb, V, (long long)C * V);
+  gemm_step(steps_, gpv);
   if (!train_) arena_.release(S->off);
   { arena_.release(vT->off); vT->live = false; }  // backward multiplies by v itself (K-major there), not by v^T
   release(qkv);
   TensP out = new_act(C, R, true);
-  if (!dry_) {
-    GemmOp* g = new_gemm("attn" + std::to_string(midx) + ".nin3");
-    g->set_output(prec_, R, R, R, mb, C, out->ptr, C, false);
-    g->add_pointwise({act_of(O)}, W[3], true);
-    g->set_bias(Bv[3]);
-    g->set_residual(x->ptr, C, (long long)V * C, false);
-    g->set_stats(out->stats);
-    g->finalize(0, false);
-    add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-  }
+  GemmOp* g3 = new_gemm("attn" + std::to_string(midx) + ".nin3");
+  g3->set_output(prec_, R, R, R, mb, C, out->ptr, C, false);
+  g3->add_pointwise({act_of(O)}, W[3], true);
+  g3->set_bias(Bv[3]);
+  g3->set_residual(x->ptr, C, (long long)V * C, false);
+  g3->set_stats(out->stats);
+  gemm_step(steps_, g3);
   if (train_) tape_attn(x, hn, qkv, S, O, out, midx);
   release(O);
   return out;
@@ -325,16 +316,13 @@ TensP UNet::downsample(const TensP& x, int midx) {
   float* b = P(pre + "Conv_0.bias", {C});
   TensP out = new_act(C, R, true);
   Scratch sp = split_begin(R, C, C, 27);
-  if (!dry_) {
-    GemmOp* g = new_gemm("down" + std::to_string(midx));
-    g->set_output(prec_, R, R, R, cfg_.max_batch, C, out->ptr, C, false);
-    g->add_conv({act_of(x)}, w, 3, 2);
-    g->set_bias(b);
-    g->set_stats(out->stats);
-    g->enable_splits(sp.S, sp.ptr);
-    g->finalize(0, false);
-    add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-  }
+  GemmOp* g = new_gemm("down" + std::to_string(midx));
+  g->set_output(prec_, R, R, R, cfg_.max_batch, C, out->ptr, C, false);
+  g->add_conv({act_of(x)}, w, 3, 2);
+  g->set_bias(b);
+  g->set_stats(out->stats);
+  g->enable_splits(sp.S, sp.ptr);
+  gemm_step(steps_, g);
   split_end(sp);
   if (train_) tape_downsample(x, out, midx);
   return out;
@@ -350,43 +338,37 @@ TensP UNet::upsample(const TensP& x, int midx) {
     // (8/27 of the FLOPs) writing its strided share of the output; the upsampled tensor never exists. The training plan
     // keeps the materialised form below (its backward differentiates exactly that graph).
     TensP out = new_act(C, R, true);
-    if (!dry_) {
-      const int r = x->R, mb = cfg_.max_batch;
-      float* w8 = (float*)dmalloc((size_t)64 * C * C * sizeof(float));
-      commit_steps_.push_back({"upw:" + pre, [=](cudaStream_t s, int) { launch_upconv_weights(w, w8, C, C, s); }});
-      const long long es = esize(prec_) * parts(prec_);
-      for (int par = 0; par < 8; ++par) {
-        const int px = par & 1, py = (par >> 1) & 1, pz = par >> 2;
-        GemmOp* g = new_gemm("up" + std::to_string(midx) + ".conv.p" + std::to_string(par));
-        char* base = (char*)out->ptr + (((long long)pz * R + py) * R + px) * C * es;
-        g->set_output_strided(prec_, r, r, r, mb, C, base, 2LL * C, 2LL * R * C, 2LL * R * R * C, (long long)R * R * R * C, false, C);
-        g->add_conv_up2(act_of(x), w8 + (size_t)par * C * C * 8, px, py, pz);
-        g->set_bias(b);
-        g->set_stats(out->stats);
-        g->finalize(0, false);
-        add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-      }
+    const int r = x->R, mb = cfg_.max_batch;
+    float* w8 = (float*)dmalloc((size_t)64 * C * C * sizeof(float));
+    commit_steps_.push_back({"upw:" + pre, [=](cudaStream_t s, int) { launch_upconv_weights(w, w8, C, C, s); }});
+    const long long es = esize(prec_) * parts(prec_);
+    for (int par = 0; par < 8; ++par) {
+      const int px = par & 1, py = (par >> 1) & 1, pz = par >> 2;
+      GemmOp* g = new_gemm("up" + std::to_string(midx) + ".conv.p" + std::to_string(par));
+      char* base = (char*)out->ptr + (((long long)pz * R + py) * R + px) * C * es;
+      g->set_output_strided(prec_, r, r, r, mb, C, base, 2LL * C, 2LL * R * C, 2LL * R * R * C, (long long)R * R * R * C, false, C);
+      g->add_conv_up2(act_of(x), w8 + (size_t)par * C * C * 8, px, py, pz);
+      g->set_bias(b);
+      g->set_stats(out->stats);
+      gemm_step(steps_, g);
     }
     return out;
   }
   TensP up = new_act(C, R, false);
-  if (!dry_) {
+  {
     const void* src = x->ptr; void* dst = up->ptr; const int r = x->R; const int es = esize(prec_);
     const int Cp = C * parts(prec_);  // X3: a row is 2C bf16 (hi | lo), copied as it is
     add_step("up" + std::to_string(midx) + ".nearest", [=](cudaStream_t s, int B) { launch_upsample2x(src, dst, B, r, r, r, Cp, es, s); });
   }
   TensP out = new_act(C, R, true);
   Scratch sp = split_begin(R, C, C, 27);
-  if (!dry_) {
-    GemmOp* g = new_gemm("up" + std::to_string(midx) + ".conv");
-    g->set_output(prec_, R, R, R, cfg_.max_batch, C, out->ptr, C, false);
-    g->add_conv({act_of(up)}, w, 3, 1);
-    g->set_bias(b);
-    g->set_stats(out->stats);
-    g->enable_splits(sp.S, sp.ptr);
-    g->finalize(0, false);
-    add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-  }
+  GemmOp* g = new_gemm("up" + std::to_string(midx) + ".conv");
+  g->set_output(prec_, R, R, R, cfg_.max_batch, C, out->ptr, C, false);
+  g->add_conv({act_of(up)}, w, 3, 1);
+  g->set_bias(b);
+  g->set_stats(out->stats);
+  g->enable_splits(sp.S, sp.ptr);
+  gemm_step(steps_, g);
   split_end(sp);
   if (train_) tape_upsample(x, up, out, midx);
   release(up);
@@ -401,6 +383,9 @@ void UNet::build() {
   arena_.reset();
   stats_cursor_ = 0;
   dense_cursor_ = 0;
+  steps_.clear(); commit_steps_.clear(); bwd_steps_.clear();
+  gemms_.clear(); commit_gemms_.clear(); bwd_gemms_.clear(); wgrads_.clear();
+  grad_ready_.clear();
   auto is_attn = [&](int r) { for (int i = 0; i < cfg_.n_attn; ++i) if (cfg_.attn_resolutions[i] == r) return true; return false; };
   auto blocks_at = [&](int lvl) { return (lvl == 0 && cfg_.level0_blocks > 0) ? cfg_.level0_blocks : cfg_.num_res_blocks; };
 
@@ -411,13 +396,10 @@ void UNet::build() {
   float* tw1 = P("all_modules.1.weight", {tdim, tdim});
   float* tb1 = P("all_modules.1.bias", {tdim});
   m = 2;
-  if (!dry_) {
-    float* ta = temb_act_; float* dw = dense_w_; float* db = dense_b_; float* dout = dense_out_; const int dt = dense_total_;
-    add_step("temb", [=](cudaStream_t s, int B) {
-      launch_temb(rt_labels_, tw0, tb0, tw1, tb1, ta, B, nf, s);
-      launch_dense(ta, dw, db, dout, B, tdim, dt, s);
-    });
-  }
+  add_step("temb", [=](cudaStream_t s, int B) {
+    launch_temb(rt_labels_, tw0, tb0, tw1, tb1, temb_act_, B, nf, s);
+    launch_dense(temb_act_, dense_w_, dense_b_, dense_out_, B, tdim, dense_total_, s);
+  });
   if (train_) tape_temb();
   // --- non-trainable tensors carried by the checkpoint
   float* mask = P("mask", {1, 1, R0, R0, R0});
@@ -437,40 +419,35 @@ void UNet::build() {
   auto A0 = std::make_shared<Tens>();
   A0->bytes = (size_t)mb * V0 * Kpad * esize(prec_) * parts(prec_);
   A0->off = arena_.alloc(A0->bytes);
-  A0->ptr = dry_ ? nullptr : arena_base_ + A0->off;
+  A0->ptr = at(A0->off);
   TensP h0 = new_act(nf, R0, true);
-  void* Am = nullptr;
-  if (!dry_) {
-    // constant field (fp32 [V][nf]) computed once per commit with the same kernels
-    float* field = (float*)dmalloc(V0 * nf * 4);
-    Am = dmalloc(V0 * Kpad_m * esize(prec_) * parts(prec_));
-    float* fbias = (float*)dmalloc(nf * 4);
-    const Precision pr = prec_;
-    const bool use_pos = cfg_.use_pos_bias != 0;
-    commit_steps_.push_back({"field.bias", [=](cudaStream_t s, int) { launch_add_vec(mbias, use_pos ? posb : nullptr, fbias, nf, s); }});
-    commit_steps_.push_back({"field.im2col", [=](cudaStream_t s, int) { launch_im2col(mask, Am, 1, 1, R0, k, Kpad_m, pr, s); }});
-    GemmOp* gf = new_gemm("stem.field", true);
-    gf->set_output(prec_, R0, R0, R0, 1, nf, field, nf, true);
-    Act am; am.ptr = Am; am.C = Kpad_m; am.X = am.Y = am.Z = R0; am.B = 1;
-    WSrc wm{mw, (long long)T, 1, 0, T};
-    gf->add_pointwise_w({am}, &wm);
-    gf->set_bias(fbias);
-    gf->finalize(0, false);
-    commit_steps_.push_back({"field.gemm", [gf](cudaStream_t s, int) { gf->repack(s); gf->launch(s, 1); }});
+  // constant field (fp32 [V][nf]) computed once per commit with the same kernels
+  float* field = (float*)dmalloc(V0 * nf * 4);
+  void* Am = dmalloc(V0 * Kpad_m * esize(prec_) * parts(prec_));
+  float* fbias = (float*)dmalloc(nf * 4);
+  const Precision pr = prec_;
+  const bool use_pos = cfg_.use_pos_bias != 0;
+  commit_steps_.push_back({"field.bias", [=](cudaStream_t s, int) { launch_add_vec(mbias, use_pos ? posb : nullptr, fbias, nf, s); }});
+  commit_steps_.push_back({"field.im2col", [=](cudaStream_t s, int) { launch_im2col(mask, Am, 1, 1, R0, k, Kpad_m, pr, s); }});
+  GemmOp* gf = new_gemm("stem.field", true);
+  gf->set_output(prec_, R0, R0, R0, 1, nf, field, nf, true);
+  Act am; am.ptr = Am; am.C = Kpad_m; am.X = am.Y = am.Z = R0; am.B = 1;
+  WSrc wm{mw, (long long)T, 1, 0, T};
+  gf->add_pointwise_w({am}, &wm);
+  gf->set_bias(fbias);
+  gemm_step(commit_steps_, gf, [gf](cudaStream_t s, int) { gf->repack(s); gf->launch(s, 1); });
 
-    void* a0 = A0->ptr;
-    add_step("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, pr, s); });
-    GemmOp* g = new_gemm("stem.gemm");
-    g->set_output(prec_, R0, R0, R0, mb, nf, h0->ptr, nf, false);
-    Act a; a.ptr = a0; a.C = Kpad; a.X = a.Y = a.Z = R0; a.B = mb;
-    WSrc ws{sw, (long long)Cin * T, 1, 0, Cin * T};
-    g->add_pointwise_w({a}, &ws);
-    g->set_bias(sb);
-    g->set_residual(field, nf, 0, true);
-    g->set_stats(h0->stats);
-    g->finalize(0, false);
-    add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-  }
+  void* a0 = A0->ptr;
+  add_step("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, pr, s); });
+  GemmOp* gs = new_gemm("stem.gemm");
+  gs->set_output(prec_, R0, R0, R0, mb, nf, h0->ptr, nf, false);
+  Act ax; ax.ptr = a0; ax.C = Kpad; ax.X = ax.Y = ax.Z = R0; ax.B = mb;
+  WSrc ws{sw, (long long)Cin * T, 1, 0, Cin * T};
+  gs->add_pointwise_w({ax}, &ws);
+  gs->set_bias(sb);
+  gs->set_residual(field, nf, 0, true);
+  gs->set_stats(h0->stats);
+  gemm_step(steps_, gs);
   arena_.release(A0->off);
   if (train_) tape_stem(h0, Am, Kpad, Kpad_m);
 
@@ -544,44 +521,45 @@ void UNet::build() {
     auto Pt = std::make_shared<Tens>();
     Pt->bytes = (size_t)mb * V0 * Np * (pf32 ? 4 : 2);
     Pt->off = arena_.alloc(Pt->bytes);
-    Pt->ptr = dry_ ? nullptr : arena_base_ + Pt->off;
-    if (!dry_) {
-      GemmOp* g = new_gemm("head.proj");
-      g->set_output(prec_, R0, R0, R0, mb, T * Cin, Pt->ptr, Np, pf32);
-      WSrc ws{hw, (long long)nf * T, (long long)T, 0, nf, Cin, 1};
-      g->add_pointwise_w({act_of(a)}, &ws);
-      g->finalize(0, false);
-      add_step(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-      const void* pp = Pt->ptr;
-      add_step("head.shift_sum", [=](cudaStream_t s, int B) { launch_tap_shift_sum(pp, Np, pf32 ? 1 : 0, hb, rt_out_, B, R0, k, Cin, s); });
-    }
+    Pt->ptr = at(Pt->off);
+    GemmOp* g = new_gemm("head.proj");
+    g->set_output(prec_, R0, R0, R0, mb, T * Cin, Pt->ptr, Np, pf32);
+    WSrc wh{hw, (long long)nf * T, (long long)T, 0, nf, Cin, 1};
+    g->add_pointwise_w({act_of(a)}, &wh);
+    gemm_step(steps_, g);
+    const void* pp = Pt->ptr;
+    add_step("head.shift_sum", [=](cudaStream_t s, int B) { launch_tap_shift_sum(pp, Np, pf32 ? 1 : 0, hb, rt_out_, B, R0, k, Cin, s); });
     arena_.release(Pt->off);
-  } else if (!dry_) {
+  } else {
     GemmOp* g = new_gemm("head.conv");
     g->set_output_strided(prec_, R0, R0, R0, mb, Cin, nullptr, 1, R0, (long long)R0 * R0, (long long)Cin * V0, true);
     g->set_out_col_stride(V0);
     g->add_conv({act_of(a)}, hw, k, 1);
     g->set_bias(hb);
-    g->finalize(0, false);
-    add_step(g->name, [g, this](cudaStream_t s, int B) { g->launch(s, B, rt_out_); });
+    gemm_step(steps_, g, [g, this](cudaStream_t s, int B) { g->launch(s, B, rt_out_); });
   }
   if (train_) tape_head(head_in, a, head_gn, "all_modules." + std::to_string(m - 1));
   release(a);
   dense_total_ = dense_cursor_;
-  stats_doubles_ = stats_cursor_;
+  // every parameter is registered by now: the offsets of their gradients in the flat buffer
+  long long off = 0;
+  for (auto& p : params_) { goff_[p.name] = off; off += p.numel; }
   if (train_) {
     // emit the backward plan: the emitters recorded during the forward pass, in reverse order
-    bwd_count_ = 0;
     for (auto it = tape_.rbegin(); it != tape_.rend(); ++it) {
       touched_.clear();
       (*it)();
-      // every gradient this emitter writes is final once all of its launches have run (the dry pass counts the same
-      // launches, so a GPU-less plan answers mdb_unet_grad_ready too)
-      for (auto& n : touched_) grad_ready_[n] = bwd_count_;
+      // every gradient this emitter writes is final once all of its launches have run
+      for (auto& n : touched_) grad_ready_[n] = (int)bwd_steps_.size();
     }
     tape_.clear();
     if (arena_.in_use() != 0) throw std::runtime_error("mdb: training plan leaked " + std::to_string(arena_.in_use()) + " arena bytes");
   }
+  flops_ = 0;
+  for (auto& g : gemms_) flops_ += g->flops;
+  bwd_flops_ = 0;
+  for (auto& g : bwd_gemms_) bwd_flops_ += g->flops;
+  for (auto& g : wgrads_) bwd_flops_ += g->flops;
 }
 
 UNet::UNet(const UNetConfig& cfg, bool dry_only) : cfg_(cfg), prec_(precision_from_int(cfg.precision)) {
@@ -592,13 +570,12 @@ UNet::UNet(const UNetConfig& cfg, bool dry_only) : cfg_(cfg), prec_(precision_fr
   if (train_ && prec_ == kTF32) throw std::runtime_error("mdb: the training plan is built for bf16 or bf16x3 (split bf16) operands");
   dry_ = true;
   build();
-  // allocate everything the dry run sized
+  // allocate everything the dry pass sized
   arena_bytes_ = arena_.peak();
-  {
-    long long off = 0;
-    for (auto& p : params_) { goff_[p.name] = off; off += p.numel; }
-  }
+  stats_doubles_ = stats_cursor_;
   if (dry_only) return;
+  const size_t n_fwd = steps_.size(), n_commit = commit_steps_.size(), n_bwd = bwd_steps_.size();
+  dry_ = false;
   arena_base_ = (char*)dmalloc(arena_bytes_, false);
   stats_base_ = (long long*)dmalloc(stats_doubles_ * sizeof(long long));
   const int tdim = 4 * cfg_.nf;
@@ -609,11 +586,10 @@ UNet::UNet(const UNetConfig& cfg, bool dry_only) : cfg_(cfg), prec_(precision_fr
   if (train_) d_dense_out_ = (float*)dmalloc((size_t)cfg_.max_batch * dense_total_ * 4);
   for (auto& p : params_)
     if (!p.external) p.d = (float*)dmalloc(p.numel * 4);
-  dry_ = false;
   build();
-  for (auto& g : gemms_) flops_ += g->flops;
-  for (auto& g : bwd_gemms_) bwd_flops_ += g->flops;
-  for (auto& g : wgrads_) bwd_flops_ += g->flops;
+  if (arena_.peak() != arena_bytes_ || stats_cursor_ != stats_doubles_ || steps_.size() != n_fwd ||
+      commit_steps_.size() != n_commit || bwd_steps_.size() != n_bwd)
+    throw std::runtime_error("mdb: the plan built over the arena differs from the dry plan that sized it");
   MDB_CUDA_CHECK(cudaDeviceSynchronize());
 }
 
@@ -628,6 +604,7 @@ UNet::~UNet() {
 }
 
 void UNet::set_param(const std::string& name, const float* src, long long numel, bool dev, cudaStream_t s) {
+  check_runnable();
   auto it = pindex_.find(name);
   if (it == pindex_.end()) throw std::runtime_error("mdb: unknown parameter " + name);
   ParamInfo& p = params_[it->second];
@@ -637,6 +614,7 @@ void UNet::set_param(const std::string& name, const float* src, long long numel,
 }
 
 void UNet::get_param(const std::string& name, float* dst, long long numel, bool dev, cudaStream_t s) {
+  check_runnable();
   auto it = pindex_.find(name);
   if (it == pindex_.end()) throw std::runtime_error("mdb: unknown parameter " + name);
   ParamInfo& p = params_[it->second];
@@ -646,6 +624,7 @@ void UNet::get_param(const std::string& name, float* dst, long long numel, bool 
 }
 
 void UNet::commit(cudaStream_t s) {
+  check_runnable();
   drop_graphs();  // packed weights are rewritten in place, but derived pointers are only guaranteed per commit
   for (auto& st : commit_steps_) st.fn(s, 1);
   for (auto& g : gemms_) g->repack(s);
@@ -660,6 +639,7 @@ void UNet::drop_graphs() {
 }
 
 void UNet::forward(const float* x, const float* labels, float* out, int B, cudaStream_t s, bool allow_graph) {
+  check_runnable();
   if (!committed_) throw std::runtime_error("mdb: parameters changed, call commit() before forward()");
   if (B < 1 || B > cfg_.max_batch) throw std::runtime_error("mdb: batch out of range");
   rt_x_ = x; rt_labels_ = labels; rt_out_ = out;
@@ -698,6 +678,7 @@ void UNet::forward(const float* x, const float* labels, float* out, int B, cudaS
 }
 
 std::vector<std::pair<std::string, float>> UNet::profile(const float* x, const float* labels, float* out, int B, cudaStream_t s) {
+  check_runnable();
   if (!committed_) throw std::runtime_error("mdb: commit() first");
   rt_x_ = x; rt_labels_ = labels; rt_out_ = out;
   std::vector<std::pair<std::string, float>> res;

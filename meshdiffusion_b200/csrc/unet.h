@@ -45,7 +45,7 @@ class Arena {
   void release(size_t off);
   size_t peak() const { return peak_; }
   size_t in_use() const { size_t n = 0; for (auto& b : blocks_) if (!b.free) n += b.size; return n; }
-  void reset() { blocks_.clear(); end_ = 0; }
+  void reset() { blocks_.clear(); end_ = 0; peak_ = 0; }
  private:
   struct Block { size_t off, size; bool free; };
   std::vector<Block> blocks_;
@@ -77,7 +77,9 @@ typedef std::shared_ptr<Tens> TensP;
 
 class UNet {
  public:
-  // dry_only: size the plan and enumerate parameters without touching the GPU (host-side tests)
+  // The plan is built twice by the same code: a dry pass without the GPU (it sizes the arena; the pointers it records
+  // are null) and, unless dry_only, a real pass over the allocated arena that must reproduce the dry pass exactly.
+  // A dry_only plan answers every host-side query (parameters, arena, steps, GEMM ops, FLOPs, grad_ready) but cannot run.
   explicit UNet(const UNetConfig& cfg, bool dry_only = false);
   ~UNet();
   const std::vector<ParamInfo>& params() const { return params_; }
@@ -158,13 +160,19 @@ class UNet {
   int dense_total_ = 0, dense_cursor_ = 0;
 
   void build();
-  float* P(const std::string& name, std::vector<long long> shape, float* external = nullptr);
+  void check_runnable() const { if (dry_) throw std::runtime_error("mdb: a dry plan cannot run"); }
+  // external: the storage is `slice`, a part of a larger buffer (null in the dry pass), instead of a buffer of its own
+  float* P(const std::string& name, std::vector<long long> shape, bool external = false, float* slice = nullptr);
+  // the allocation layer is the only code that knows the pass: in the dry pass both return nullptr
   void* dmalloc(size_t bytes, bool zero = true);
+  char* at(size_t arena_off) const { return dry_ ? nullptr : arena_base_ + arena_off; }
   TensP new_act(int C, int R, bool stats);
   void release(TensP& t);
   Act act_of(const TensP& t) const;
   GemmOp* new_gemm(const std::string& name, bool commit_time = false);
-  void add_step(const std::string& name, std::function<void(cudaStream_t, int)> fn) { if (!dry_) steps_.push_back({name, fn}); }
+  void add_step(const std::string& name, std::function<void(cudaStream_t, int)> fn) { steps_.push_back({name, fn}); }
+  // finalizes g, uploads it (real pass), and appends its launch (fn, default g->launch(s, B)) to `steps` under its name
+  void gemm_step(std::vector<Step>& steps, GemmOp* g, std::function<void(cudaStream_t, int)> fn = {}, int kind = kAlways);
   struct Scratch { int S = 1; size_t off = 0; float* ptr = nullptr; bool active = false; };
   Scratch split_begin(int R, int N, int cin_total, int taps);
   void split_end(Scratch& s);
@@ -184,10 +192,8 @@ class UNet {
   bool has_input_grad_ = false;  // the plan carries the stem's data gradient (4 input channels, as the head's shift-sum)
   int rt_drop_thresh_ = 0; float rt_drop_scale_ = 1.f; unsigned long long rt_seed_ = 0;
   float* d_dense_out_ = nullptr;  // [mb][dense_total] gradient of the time-embedding projections
-  int bwd_count_ = 0;  // launches of the backward plan emitted so far (counted in the dry pass too)
   void add_bwd(const std::string& name, std::function<void(cudaStream_t, int)> fn, int kind = kAlways) {
-    ++bwd_count_;
-    if (!dry_) bwd_steps_.push_back({name, fn, kind});
+    bwd_steps_.push_back({name, fn, kind});
   }
   void run_backward(const float* dout, float* grads, float* dx, int B, bool accumulate, cudaStream_t s, const int* mark_steps,
                     void* const* mark_events, int n_marks);

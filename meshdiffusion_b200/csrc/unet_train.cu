@@ -23,7 +23,7 @@ GradView UNet::new_grad(int C, int R) {
   g.buf = std::make_shared<GradBuf>();
   g.buf->off = arena_.alloc((size_t)cfg_.max_batch * R * R * R * C * esize(prec_) * parts(prec_));
   g.buf->refs = 1;
-  g.ptr = dry_ ? nullptr : arena_base_ + g.buf->off;
+  g.ptr = at(g.buf->off);
   g.ld = C; g.C = C;
   return g;
 }
@@ -31,7 +31,7 @@ GradView UNet::new_grad(int C, int R) {
 GradView UNet::grad_view(const GradView& g, int c0, int C) {
   GradView v = g;
   v.buf->refs++;
-  v.ptr = dry_ ? nullptr : (char*)g.ptr + (size_t)c0 * esize(prec_);  // (X3: offset into the hi parts; lo parts follow at ld)
+  v.ptr = at(g.buf->off + (size_t)c0 * esize(prec_));  // g is a whole buffer (X3: offset into the hi parts; lo parts follow at ld)
   v.C = C;
   if (g.colsum) v.colsum = g.colsum + c0;
   return v;
@@ -56,7 +56,6 @@ Act UNet::act_of_grad(const GradView& g, int R) const {
 
 long long UNet::G(const std::string& name) const {
   touched_.push_back(name);
-  if (dry_) return 0;
   auto it = goff_.find(name);
   if (it == goff_.end()) throw std::runtime_error("mdb: no gradient slot for " + name);
   return it->second;
@@ -80,7 +79,7 @@ long long UNet::total_param_numel() const {
 UNet::Tmp UNet::tmp_alloc(size_t bytes) {
   Tmp t;
   t.off = arena_.alloc(bytes ? bytes : 16);
-  t.ptr = dry_ ? nullptr : arena_base_ + t.off;
+  t.ptr = at(t.off);
   return t;
 }
 void UNet::tmp_free(Tmp& t) { arena_.release(t.off); t.ptr = nullptr; }
@@ -115,6 +114,7 @@ void UNet::backward_input(const float* dout, float* dx, float* grads, int B, boo
 
 void UNet::run_backward(const float* dout, float* grads, float* dx, int B, bool accumulate, cudaStream_t s, const int* mark_steps,
                         void* const* mark_events, int n_marks) {
+  check_runnable();
   if (!train_) throw std::runtime_error("mdb: backward() needs an engine created with training = 1");
   if (!committed_) throw std::runtime_error("mdb: parameters changed, call commit() before backward()");
   if (B < 1 || B > cfg_.max_batch) throw std::runtime_error("mdb: batch out of range");
@@ -136,6 +136,7 @@ void UNet::run_backward(const float* dout, float* grads, float* dx, int B, bool 
 }
 
 std::vector<std::pair<std::string, float>> UNet::profile_backward(const float* dout, float* grads, int B, cudaStream_t s) {
+  check_runnable();
   if (!train_) throw std::runtime_error("mdb: profile_backward() needs a training engine");
   rt_dout_ = dout; rt_grads_ = grads; rt_accum_ = false;
   std::vector<std::pair<std::string, float>> res;
@@ -163,21 +164,19 @@ void UNet::emit_colsum(const std::string& name, const GradView& t, int R, float*
   // when the producing GroupNorm-backward kernel already left per-sample column sums, only the batch sum remains
   const bool have = t.buf && t.buf->has_cs;
   Tmp part = tmp_alloc(have ? 16 : (size_t)kBwdPartRows(cfg_.max_batch) * t.C * sizeof(float));
-  if (!dry_) {
-    ColsumArgs a{};
-    a.t = t.ptr; a.ld = t.ld; a.C = t.C; a.voxels = (long long)R * R * R;
-    a.part = (float*)part.ptr; a.per = per; a.per_ld = per_ld;
-    a.from_per = t.colsum; a.from_ld = t.cs_ld;
-    a.prec = prec_;
-    add_bwd(name, [=](cudaStream_t s, int B) {
-      ColsumArgs c = a;
-      c.total0 = g0 >= 0 ? rt_grads_ + g0 : nullptr;
-      c.total1 = g1 >= 0 ? rt_grads_ + g1 : nullptr;
-      c.total2 = g2 >= 0 ? rt_grads_ + g2 : nullptr;
-      c.accumulate = rt_accum_ ? 1 : 0;
-      launch_colsum(c, B, s);
-    }, kParamGradOnly);
-  }
+  ColsumArgs a{};
+  a.t = t.ptr; a.ld = t.ld; a.C = t.C; a.voxels = (long long)R * R * R;
+  a.part = (float*)part.ptr; a.per = per; a.per_ld = per_ld;
+  a.from_per = t.colsum; a.from_ld = t.cs_ld;
+  a.prec = prec_;
+  add_bwd(name, [=](cudaStream_t s, int B) {
+    ColsumArgs c = a;
+    c.total0 = g0 >= 0 ? rt_grads_ + g0 : nullptr;
+    c.total1 = g1 >= 0 ? rt_grads_ + g1 : nullptr;
+    c.total2 = g2 >= 0 ? rt_grads_ + g2 : nullptr;
+    c.accumulate = rt_accum_ ? 1 : 0;
+    launch_colsum(c, B, s);
+  }, kParamGradOnly);
   tmp_free(part);
 }
 
@@ -186,15 +185,13 @@ void UNet::emit_wgrad(const std::string& name, const Act& dy, const Act& x, int 
                       const WgradOut& layout) {
   const WgradPlan pl = plan_wgrad(dy.X, dy.Y, dy.Z, dy.B, dy.C, x.C, ksize, stride, prec_ == kBF16X3);
   Tmp sc = tmp_alloc(pl.scratch_bytes);
-  if (!dry_) {
-    auto op = std::make_unique<WgradOp>();
-    op->name = name;
-    op->init(dy, x, ksize, stride, layout, (float*)sc.ptr, prec_);
-    WgradOp* raw = op.get();
-    wgrads_.push_back(std::move(op));
-    const bool fixed = dy.B == 1 && cfg_.max_batch != 1;  // batch-reduced operand (mask_layer)
-    add_bwd(name, [=](cudaStream_t s, int B) { raw->launch(s, fixed ? 1 : B, rt_accum_, rt_grads_ + goff); }, kParamGradOnly);
-  }
+  auto op = std::make_unique<WgradOp>();
+  op->name = name;
+  op->init(dy, x, ksize, stride, layout, (float*)sc.ptr, prec_);
+  WgradOp* raw = op.get();
+  wgrads_.push_back(std::move(op));
+  const bool fixed = dy.B == 1 && cfg_.max_batch != 1;  // batch-reduced operand (mask_layer)
+  add_bwd(name, [=](cudaStream_t s, int B) { raw->launch(s, fixed ? 1 : B, rt_accum_, rt_grads_ + goff); }, kParamGradOnly);
   tmp_free(sc);
 }
 
@@ -205,8 +202,7 @@ static bool gnb_enabled() {
   return !(e && e[0] == '0');
 }
 
-// Sizes and attaches the GroupNorm-backward epilogue of a data-gradient GEMM (same decisions in the sizing pass, where
-// g == nullptr, and the real pass).
+// Sizes and attaches the GroupNorm-backward epilogue of a data-gradient GEMM.
 void UNet::gn_fuse_attach(GnFuse& f, GemmOp* g, int N, int R) {
   const int mb = cfg_.max_batch;
   const Geometry geo = pick_geometry(R, R, R);
@@ -216,7 +212,6 @@ void UNet::gn_fuse_attach(GnFuse& f, GemmOp* g, int N, int R) {
   f.consts = tmp_alloc((size_t)mb * N * 4 * sizeof(float));
   f.part = tmp_alloc((size_t)rows * N * 2 * sizeof(float));
   f.on = true;
-  if (dry_) return;
   GnBwdArgs a{};
   a.C0 = f.ins[0]->C; a.C1 = f.ins.size() > 1 ? f.ins[1]->C : 0;
   a.stats0 = f.ins[0]->stats; a.stats1 = f.ins.size() > 1 ? f.ins[1]->stats : nullptr;
@@ -236,26 +231,20 @@ GradView UNet::emit_conv_dgrad(const std::string& name, const GradView& dy, int 
   Scratch sp;
   if (can_split) sp = split_begin(R, cin_total, dy.C, 27);
   const bool fused = fuse && gnb_enabled() && !addend && sp.S <= 1 && cin_total % 32 == 0;
-  GemmOp* g = nullptr;
-  if (!dry_) {
-    g = new_bwd_gemm(name);
-    g->set_output(prec_, R, R, R, cfg_.max_batch, cin_total, dx.ptr, cin_total, false);
-    g->add_conv_dgrad(act_of_grad(dy, R), w, cin_total, 3);
-    if (addend) g->set_residual(addend->ptr, addend->ld, (long long)R * R * R * addend->ld, false);
-    g->enable_splits(sp.S, sp.ptr);
-  }
+  GemmOp* g = new_bwd_gemm(name);
+  g->set_output(prec_, R, R, R, cfg_.max_batch, cin_total, dx.ptr, cin_total, false);
+  g->add_conv_dgrad(act_of_grad(dy, R), w, cin_total, 3);
+  if (addend) g->set_residual(addend->ptr, addend->ld, (long long)R * R * R * addend->ld, false);
+  g->enable_splits(sp.S, sp.ptr);
   if (fused) gn_fuse_attach(*fuse, g, cin_total, R);
-  if (!dry_) {
-    g->finalize(0, false);
-    const int dl = fused ? fuse->drop_layer : -1;
-    add_bwd(name, [g, this, dl](cudaStream_t s, int B) {
-      if (dl >= 0) {
-        g->rt_drop_thresh = rt_drop_thresh_; g->rt_drop_scale = rt_drop_scale_;
-        g->rt_seed = dropout_layer_seed(rt_seed_, dl);
-      }
-      g->launch(s, B);
-    });
-  }
+  const int dl = fused ? fuse->drop_layer : -1;
+  gemm_step(bwd_steps_, g, [g, this, dl](cudaStream_t s, int B) {
+    if (dl >= 0) {
+      g->rt_drop_thresh = rt_drop_thresh_; g->rt_drop_scale = rt_drop_scale_;
+      g->rt_seed = dropout_layer_seed(rt_seed_, dl);
+    }
+    g->launch(s, B);
+  });
   split_end(sp);
   return dx;
 }
@@ -265,18 +254,12 @@ GradView UNet::emit_pointwise(const std::string& name, const std::vector<Act>& s
                               const GradView* addend, GnFuse* fuse) {
   GradView dx = new_grad(N, R);
   const bool fused = fuse && gnb_enabled() && !addend && N % 32 == 0;
-  GemmOp* g = nullptr;
-  if (!dry_) {
-    g = new_bwd_gemm(name);
-    g->set_output(prec_, R, R, R, cfg_.max_batch, N, dx.ptr, N, false);
-    for (size_t i = 0; i < srcs.size(); ++i) g->add_pointwise_w({srcs[i]}, &ws[i]);
-    if (addend) g->set_residual(addend->ptr, addend->ld, (long long)R * R * R * addend->ld, false);
-  }
+  GemmOp* g = new_bwd_gemm(name);
+  g->set_output(prec_, R, R, R, cfg_.max_batch, N, dx.ptr, N, false);
+  for (size_t i = 0; i < srcs.size(); ++i) g->add_pointwise_w({srcs[i]}, &ws[i]);
+  if (addend) g->set_residual(addend->ptr, addend->ld, (long long)R * R * R * addend->ld, false);
   if (fused) gn_fuse_attach(*fuse, g, N, R);
-  if (!dry_) {
-    g->finalize(0, false);
-    add_bwd(name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-  }
+  gemm_step(bwd_steps_, g);
   return dx;
 }
 
@@ -296,42 +279,40 @@ GradView UNet::emit_gn_backward(const std::string& pname, const std::vector<Tens
   // whichever op produced the tensor this is the gradient of
   dx.buf->has_cs = true;
   dx.buf->cs_off = arena_.alloc((size_t)mb * C * sizeof(float));
-  dx.colsum = dry_ ? nullptr : reinterpret_cast<float*>(arena_base_ + dx.buf->cs_off);
+  dx.colsum = reinterpret_cast<float*>(at(dx.buf->cs_off));
   dx.cs_ld = C;
   Tmp cs_part = tmp_alloc((size_t)kBwdPartRows(mb) * C * sizeof(float));
-  if (!dry_) {
-    GnBwdArgs a{};
-    a.x0 = ins[0]->ptr; a.C0 = ins[0]->C; a.ld0 = ins[0]->C;
-    a.x1 = ins.size() > 1 ? ins[1]->ptr : nullptr; a.C1 = ins.size() > 1 ? ins[1]->C : 0; a.ld1 = a.C1;
-    a.stats0 = ins[0]->stats; a.stats1 = ins.size() > 1 ? ins[1]->stats : nullptr;
-    a.gamma = gamma; a.beta = beta; a.da = da.ptr;
-    a.voxels = (long long)R * R * R; a.silu = silu ? 1 : 0; a.groups = 32; a.eps = 1e-6f;
-    a.part = (float*)part.ptr; a.sums = (float*)sums.ptr;
-    a.dx = dx.ptr;
-    a.add0 = add0 ? add0->ptr : nullptr; a.add0_ld = add0 ? add0->ld : 0;
-    a.add1 = add1 ? add1->ptr : nullptr; a.add1_ld = add1 ? add1->ld : 0;
-    a.cs_part = (float*)cs_part.ptr; a.cs_per = dx.colsum;
-    a.prec = prec_;
-    const long long gw = G(pname + ".weight"), gb = G(pname + ".bias");
-    auto with_rt = [this, a, gw, gb, drop_layer]() {
-      GnBwdArgs c = a;
-      if (drop_layer >= 0) {
-        c.drop_thresh = rt_drop_thresh_; c.drop_scale = rt_drop_scale_;
-        c.seed = dropout_layer_seed(rt_seed_, drop_layer);
-      }
-      // input gradient only: no gamma / beta gradient (the reduce launch then skips its parameter kernel)
-      c.dgamma = rt_grads_ ? rt_grads_ + gw : nullptr; c.dbeta = rt_grads_ ? rt_grads_ + gb : nullptr;
-      c.accumulate = rt_accum_ ? 1 : 0;
-      return c;
-    };
-    if (fused) {
-      const float* tp = (const float*)fuse->part.ptr; const int T = fuse->T, bb = fuse->bb;
-      add_bwd("gnb_tile_reduce:" + pname, [with_rt, tp, T, bb](cudaStream_t s, int B) { launch_gnb_tile_reduce(with_rt(), tp, T, bb, B, s); });
-    } else {
-      add_bwd("gn_bwd_reduce:" + pname, [with_rt](cudaStream_t s, int B) { launch_gn_bwd_reduce(with_rt(), B, s); });
+  GnBwdArgs a{};
+  a.x0 = ins[0]->ptr; a.C0 = ins[0]->C; a.ld0 = ins[0]->C;
+  a.x1 = ins.size() > 1 ? ins[1]->ptr : nullptr; a.C1 = ins.size() > 1 ? ins[1]->C : 0; a.ld1 = a.C1;
+  a.stats0 = ins[0]->stats; a.stats1 = ins.size() > 1 ? ins[1]->stats : nullptr;
+  a.gamma = gamma; a.beta = beta; a.da = da.ptr;
+  a.voxels = (long long)R * R * R; a.silu = silu ? 1 : 0; a.groups = 32; a.eps = 1e-6f;
+  a.part = (float*)part.ptr; a.sums = (float*)sums.ptr;
+  a.dx = dx.ptr;
+  a.add0 = add0 ? add0->ptr : nullptr; a.add0_ld = add0 ? add0->ld : 0;
+  a.add1 = add1 ? add1->ptr : nullptr; a.add1_ld = add1 ? add1->ld : 0;
+  a.cs_part = (float*)cs_part.ptr; a.cs_per = dx.colsum;
+  a.prec = prec_;
+  const long long gw = G(pname + ".weight"), gb = G(pname + ".bias");
+  auto with_rt = [this, a, gw, gb, drop_layer]() {
+    GnBwdArgs c = a;
+    if (drop_layer >= 0) {
+      c.drop_thresh = rt_drop_thresh_; c.drop_scale = rt_drop_scale_;
+      c.seed = dropout_layer_seed(rt_seed_, drop_layer);
     }
-    add_bwd("gn_bwd_apply:" + pname, [with_rt](cudaStream_t s, int B) { launch_gn_bwd_apply(with_rt(), B, s); });
+    // input gradient only: no gamma / beta gradient (the reduce launch then skips its parameter kernel)
+    c.dgamma = rt_grads_ ? rt_grads_ + gw : nullptr; c.dbeta = rt_grads_ ? rt_grads_ + gb : nullptr;
+    c.accumulate = rt_accum_ ? 1 : 0;
+    return c;
+  };
+  if (fused) {
+    const float* tp = (const float*)fuse->part.ptr; const int T = fuse->T, bb = fuse->bb;
+    add_bwd("gnb_tile_reduce:" + pname, [with_rt, tp, T, bb](cudaStream_t s, int B) { launch_gnb_tile_reduce(with_rt(), tp, T, bb, B, s); });
+  } else {
+    add_bwd("gn_bwd_reduce:" + pname, [with_rt](cudaStream_t s, int B) { launch_gn_bwd_reduce(with_rt(), B, s); });
   }
+  add_bwd("gn_bwd_apply:" + pname, [with_rt](cudaStream_t s, int B) { launch_gn_bwd_apply(with_rt(), B, s); });
   tmp_free(part);
   tmp_free(sums);
   tmp_free(cs_part);
@@ -381,14 +362,12 @@ void UNet::tape_resblock(const std::vector<TensP>& ins, TensP a, TensP h, TensP 
     GradView dh = emit_gn_backward(pre + "GroupNorm_1", {h}, da2, true, midx, nullptr, nullptr, &f1);
     unref(da2);
     // Conv_0 bias and the time-embedding projection: h += Dense_0(act(temb))[:, :, None, None, None]
-    emit_colsum(nm + ".conv0.dbias", dh, R, dry_ ? nullptr : d_dense_out_ + doff, dense_total_, G(pre + "Conv_0.bias"), -1, -1);
-    if (!dry_) {
-      const float* dd = d_dense_out_ + doff; const long long dt = dense_total_; const float* ta = temb_act_;
-      const long long gw = G(pre + "Dense_0.weight"), gb = G(pre + "Dense_0.bias");
-      add_bwd(nm + ".dense.wgrad", [=](cudaStream_t s, int B) {
-        launch_outer_sum(dd, dt, ta, tdim, rt_grads_ + gw, rt_grads_ + gb, B, out_ch, tdim, rt_accum_ ? 1 : 0, s);
-      }, kParamGradOnly);
-    }
+    emit_colsum(nm + ".conv0.dbias", dh, R, d_dense_out_ + doff, dense_total_, G(pre + "Conv_0.bias"), -1, -1);
+    const float* dd = d_dense_out_ + doff; const long long dt = dense_total_; const float* ta = temb_act_;
+    const long long gw = G(pre + "Dense_0.weight"), gb = G(pre + "Dense_0.bias");
+    add_bwd(nm + ".dense.wgrad", [=](cudaStream_t s, int B) {
+      launch_outer_sum(dd, dt, ta, tdim, rt_grads_ + gw, rt_grads_ + gb, B, out_ch, tdim, rt_accum_ ? 1 : 0, s);
+    }, kParamGradOnly);
     emit_wgrad(nm + ".conv0.wgrad", act_of_grad(dh, R), act_of(a), 3, 1, G(pre + "Conv_0.weight"), oidhw_layout(Cin));
     free_act(a);
     GnFuse f0; f0.pname = pre + "GroupNorm_0"; f0.ins = ins; f0.silu = true; f0.drop_layer = -1;
@@ -441,35 +420,29 @@ void UNet::tape_attn(TensP x, TensP hn, TensP qkv, TensP S, TensP O, TensP out, 
     GradView dqkv = new_grad(3 * C, R);
     // dP[q][k] = dOo[q][:] . v[k][:]   (fp32, softmax backward then runs in place)
     Tmp dS = tmp_alloc((size_t)mb * V * V * 4);
-    if (!dry_) {
-      GemmOp* g = new_bwd_gemm(nm + ".dP");
-      g->set_output_strided(prec_, V, 1, 1, mb, V, dS.ptr, V, 0, 0, (long long)V * V, true);
-      g->add_pointwise({mat(dOo.ptr, C, C)}, nullptr, true);
-      g->set_b_activation((char*)qkv->ptr + (size_t)2 * C * es, C, V, mb, 3 * C, (long long)V * 3 * C);
-      g->finalize(0, false);
-      add_bwd(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-    }
+    GemmOp* gdp = new_bwd_gemm(nm + ".dP");
+    gdp->set_output_strided(prec_, V, 1, 1, mb, V, dS.ptr, V, 0, 0, (long long)V * V, true);
+    gdp->add_pointwise_w({mat(dOo.ptr, C, C)}, nullptr);
+    gdp->set_b_activation((char*)qkv->ptr + (size_t)2 * C * es, C, V, mb, 3 * C, (long long)V * 3 * C);
+    gemm_step(bwd_steps_, gdp);
     // dv[k][c] = sum_q P[q][k] dOo[q][c]
     // (X3: P rows hold V hi then V lo parts; transposed rows are [V hi | V lo] again, one transpose per part)
     Tmp PT = tmp_alloc((size_t)mb * V * V * es * P);
     Tmp dOT = tmp_alloc((size_t)mb * C * V * es * P);
-    if (!dry_) {
-      const void* sp = S->ptr; char* pt = (char*)PT.ptr; const void* dop = dOo.ptr; char* dot = (char*)dOT.ptr;
-      add_bwd(nm + ".PT", [=](cudaStream_t s, int B) {
-        for (int part = 0; part < P; ++part) {
-          launch_transpose_vc(sp, 2 * V, part * V, pt + (size_t)part * V * es, B, V, V, es, s, (long long)P * V);
-          launch_transpose_vc(dop, (long long)P * C, part * C, dot + (size_t)part * V * es, B, V, C, es, s, (long long)P * V);
-        }
-      });
-      GemmOp* g = new_bwd_gemm(nm + ".dv");
-      g->set_output_strided(prec_, V, 1, 1, mb, C, (char*)dqkv.ptr + (size_t)2 * C * es, 3 * C, 0, 0, (long long)V * 3 * C, false);
-      g->add_pointwise({mat(PT.ptr, V, V)}, nullptr, true);
-      g->set_b_activation(dOT.ptr, V, C, mb, V, (long long)C * V);
-      g->finalize(0, false);
-      add_bwd(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-      float* dsp = (float*)dS.ptr; const float* pp = (const float*)S->ptr;
-      add_bwd(nm + ".softmax_bwd", [=](cudaStream_t s, int B) { launch_softmax_bwd_rows(pp, dsp, (long long)B * V, V, pr, s); });
-    }
+    const void* sp = S->ptr; char* pt = (char*)PT.ptr; const void* dop = dOo.ptr; char* dot = (char*)dOT.ptr;
+    add_bwd(nm + ".PT", [=](cudaStream_t s, int B) {
+      for (int part = 0; part < P; ++part) {
+        launch_transpose_vc(sp, 2 * V, part * V, pt + (size_t)part * V * es, B, V, V, es, s, (long long)P * V);
+        launch_transpose_vc(dop, (long long)P * C, part * C, dot + (size_t)part * V * es, B, V, C, es, s, (long long)P * V);
+      }
+    });
+    GemmOp* gdv = new_bwd_gemm(nm + ".dv");
+    gdv->set_output_strided(prec_, V, 1, 1, mb, C, (char*)dqkv.ptr + (size_t)2 * C * es, 3 * C, 0, 0, (long long)V * 3 * C, false);
+    gdv->add_pointwise_w({mat(PT.ptr, V, V)}, nullptr);
+    gdv->set_b_activation(dOT.ptr, V, C, mb, V, (long long)C * V);
+    gemm_step(bwd_steps_, gdv);
+    float* dsf = (float*)dS.ptr; const float* pp = (const float*)S->ptr;
+    add_bwd(nm + ".softmax_bwd", [=](cudaStream_t s, int B) { launch_softmax_bwd_rows(pp, dsf, (long long)B * V, V, pr, s); });
     tmp_free(PT);
     tmp_free(dOT);
     unref(dOo);
@@ -478,31 +451,27 @@ void UNet::tape_attn(TensP x, TensP hn, TensP qkv, TensP S, TensP O, TensP out, 
     Tmp kT = tmp_alloc((size_t)mb * C * V * es * P);
     Tmp qT = tmp_alloc((size_t)mb * C * V * es * P);
     Tmp dST = tmp_alloc((size_t)mb * V * V * es * P);
-    if (!dry_) {
-      const void* qp = qkv->ptr; char* ktp = (char*)kT.ptr; char* qtp = (char*)qT.ptr; const void* dsp = dS.ptr; char* dstp = (char*)dST.ptr;
-      add_bwd(nm + ".kT", [=](cudaStream_t s, int B) {
-        for (int part = 0; part < P; ++part) {  // qkv rows: [3C hi | 3C lo]; dS rows: V hi then V lo bf16
-          launch_transpose_vc(qp, 3LL * C * P, C + part * 3 * C, ktp + (size_t)part * V * es, B, V, C, es, s, (long long)P * V);
-          launch_transpose_vc(qp, 3LL * C * P, part * 3 * C, qtp + (size_t)part * V * es, B, V, C, es, s, (long long)P * V);
-          launch_transpose_vc(dsp, 2 * V, part * V, dstp + (size_t)part * V * es, B, V, V, es, s, (long long)P * V);
-        }
-      });
-      GemmOp* g = new_bwd_gemm(nm + ".dq");
-      g->set_output_strided(prec_, V, 1, 1, mb, C, dqkv.ptr, 3 * C, 0, 0, (long long)V * 3 * C, false);
-      // dS as the A operand: bf16 at the start of rows of V fp32 slots (logical pitch 2V), or X3 (hi | lo) rows filling them
-      g->add_pointwise({mat(dS.ptr, V, pr == kBF16X3 ? V : 2 * V)}, nullptr, true);
-      g->set_b_activation(kT.ptr, V, C, mb, V, (long long)C * V);
-      g->set_alpha(alpha);
-      g->finalize(0, false);
-      add_bwd(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); });
-      GemmOp* g2 = new_bwd_gemm(nm + ".dk");
-      g2->set_output_strided(prec_, V, 1, 1, mb, C, (char*)dqkv.ptr + (size_t)C * es, 3 * C, 0, 0, (long long)V * 3 * C, false);
-      g2->add_pointwise({mat(dST.ptr, V, V)}, nullptr, true);
-      g2->set_b_activation(qT.ptr, V, C, mb, V, (long long)C * V);
-      g2->set_alpha(alpha);
-      g2->finalize(0, false);
-      add_bwd(g2->name, [g2](cudaStream_t s, int B) { g2->launch(s, B); });
-    }
+    const void* qp = qkv->ptr; char* ktp = (char*)kT.ptr; char* qtp = (char*)qT.ptr; const void* dsp = dS.ptr; char* dstp = (char*)dST.ptr;
+    add_bwd(nm + ".kT", [=](cudaStream_t s, int B) {
+      for (int part = 0; part < P; ++part) {  // qkv rows: [3C hi | 3C lo]; dS rows: V hi then V lo bf16
+        launch_transpose_vc(qp, 3LL * C * P, C + part * 3 * C, ktp + (size_t)part * V * es, B, V, C, es, s, (long long)P * V);
+        launch_transpose_vc(qp, 3LL * C * P, part * 3 * C, qtp + (size_t)part * V * es, B, V, C, es, s, (long long)P * V);
+        launch_transpose_vc(dsp, 2 * V, part * V, dstp + (size_t)part * V * es, B, V, V, es, s, (long long)P * V);
+      }
+    });
+    GemmOp* gdq = new_bwd_gemm(nm + ".dq");
+    gdq->set_output_strided(prec_, V, 1, 1, mb, C, dqkv.ptr, 3 * C, 0, 0, (long long)V * 3 * C, false);
+    // dS as the A operand: bf16 at the start of rows of V fp32 slots (logical pitch 2V), or X3 (hi | lo) rows filling them
+    gdq->add_pointwise_w({mat(dS.ptr, V, pr == kBF16X3 ? V : 2 * V)}, nullptr);
+    gdq->set_b_activation(kT.ptr, V, C, mb, V, (long long)C * V);
+    gdq->set_alpha(alpha);
+    gemm_step(bwd_steps_, gdq);
+    GemmOp* gdk = new_bwd_gemm(nm + ".dk");
+    gdk->set_output_strided(prec_, V, 1, 1, mb, C, (char*)dqkv.ptr + (size_t)C * es, 3 * C, 0, 0, (long long)V * 3 * C, false);
+    gdk->add_pointwise_w({mat(dST.ptr, V, V)}, nullptr);
+    gdk->set_b_activation(qT.ptr, V, C, mb, V, (long long)C * V);
+    gdk->set_alpha(alpha);
+    gemm_step(bwd_steps_, gdk);
     tmp_free(kT);
     tmp_free(qT);
     tmp_free(dST);
@@ -546,11 +515,9 @@ void UNet::tape_downsample(TensP x, TensP out, int midx) {
     emit_wgrad(nm + ".wgrad", act_of_grad(dO, Ro), act_of(x), 3, 2, G(pre + "Conv_0.weight"), oidhw_layout(C));
     // transposed stride-2 convolution = zero-stuffed dY (odd sites) convolved with the mirrored, transposed kernel
     GradView z = new_grad(C, Ri);
-    if (!dry_) {
-      const void* src = dO.ptr; void* dst = z.ptr;
-      const int Cp = C * parts(prec_);  // X3: a row is 2C bf16 (hi | lo), moved as it is
-      add_bwd(nm + ".zero_stuff", [=](cudaStream_t s, int B) { launch_zero_stuff2x(src, dst, B, Ro, Cp, s); });
-    }
+    const void* src = dO.ptr; void* dst = z.ptr;
+    const int Cp = C * parts(prec_);  // X3: a row is 2C bf16 (hi | lo), moved as it is
+    add_bwd(nm + ".zero_stuff", [=](cudaStream_t s, int B) { launch_zero_stuff2x(src, dst, B, Ro, Cp, s); });
     GradView prev = x->grad;
     GradView dx = emit_conv_dgrad(nm + ".dgrad", z, Ri, w, C, prev.valid() ? &prev : nullptr);
     unref(z);
@@ -576,10 +543,8 @@ void UNet::tape_upsample(TensP x, TensP up, TensP out, int midx) {
     GradView dup = emit_conv_dgrad(nm + ".dgrad", dO, R, w, C, nullptr);
     unref(out->grad);
     GradView dx = new_grad(C, x->R);
-    if (!dry_) {
-      const void* src = dup.ptr; void* dst = dx.ptr; const int r = x->R; const Precision pr = prec_;
-      add_bwd(nm + ".downsum", [=](cudaStream_t s, int B) { launch_downsum2x(src, dst, B, r, C, pr, s); });
-    }
+    const void* src = dup.ptr; void* dst = dx.ptr; const int r = x->R; const Precision pr = prec_;
+    add_bwd(nm + ".downsum", [=](cudaStream_t s, int B) { launch_downsum2x(src, dst, B, r, C, pr, s); });
     unref(dup);
     if (x->grad.valid()) throw std::runtime_error("mdb: upsample input already has a gradient");
     x->grad = dx;
@@ -602,19 +567,16 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
       const int Np = ((T * Cin + 7) / 8) * 8;
       const bool pf32 = prec_ != kBF16;  // as the head: split bf16 keeps the per-tap projections fp32
       Tmp Pd = tmp_alloc((size_t)cfg_.max_batch * V0 * Np * (pf32 ? 4 : 2));
-      if (!dry_) {
-        const float* sw = P("all_modules.2.weight", {});
-        GemmOp* g = new_bwd_gemm("stem.dgrad.proj");
-        g->set_output(prec_, R0, R0, R0, cfg_.max_batch, T * Cin, Pd.ptr, Np, pf32);
-        WSrc wd{sw + (T - 1), (long long)T, (long long)Cin * T, 0, nf, Cin, -1};
-        g->add_pointwise_w({act_of_grad(dh, R0)}, &wd);
-        g->finalize(0, false);
-        add_bwd(g->name, [g](cudaStream_t s, int B) { g->launch(s, B); }, kInputGradOnly);
-        const float* zero = (const float*)dmalloc(Cin * sizeof(float));
-        const void* pp = Pd.ptr;
-        add_bwd("stem.dgrad.shift_sum", [=](cudaStream_t s, int B) { launch_tap_shift_sum(pp, Np, pf32 ? 1 : 0, zero, rt_dx_, B, R0, k, Cin, s); },
-                kInputGradOnly);
-      }
+      const float* sw = P("all_modules.2.weight", {});
+      GemmOp* g = new_bwd_gemm("stem.dgrad.proj");
+      g->set_output(prec_, R0, R0, R0, cfg_.max_batch, T * Cin, Pd.ptr, Np, pf32);
+      WSrc wd{sw + (T - 1), (long long)T, (long long)Cin * T, 0, nf, Cin, -1};
+      g->add_pointwise_w({act_of_grad(dh, R0)}, &wd);
+      gemm_step(bwd_steps_, g, {}, kInputGradOnly);
+      const float* zero = (const float*)dmalloc(Cin * sizeof(float));
+      const void* pp = Pd.ptr;
+      add_bwd("stem.dgrad.shift_sum", [=](cudaStream_t s, int B) { launch_tap_shift_sum(pp, Np, pf32 ? 1 : 0, zero, rt_dx_, B, R0, k, Cin, s); },
+              kInputGradOnly);
       tmp_free(Pd);
     }
     // h0 = conv(x) + b + pos_layer.bias + mask_layer(mask): the three biases receive the same column sum
@@ -623,10 +585,8 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
     const int es = esize(prec_), P = parts(prec_);
     const Precision pr = prec_;
     Tmp A0 = tmp_alloc((size_t)cfg_.max_batch * V0 * Kpad * es * P);
-    if (!dry_) {
-      void* a0 = A0.ptr;
-      add_bwd("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, pr, s); }, kParamGradOnly);
-    }
+    void* a0 = A0.ptr;
+    add_bwd("stem.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_x_, a0, B, Cin, R0, k, Kpad, pr, s); }, kParamGradOnly);
     {
       Act xa; xa.ptr = A0.ptr; xa.C = Kpad; xa.X = xa.Y = xa.Z = R0; xa.B = cfg_.max_batch;
       WgradOut o; o.sm = (long long)Cin * T; o.sn = 1; o.st = 0; o.n_valid = Cin * T;
@@ -635,10 +595,8 @@ void UNet::tape_stem(TensP h0, void* Am, int Kpad, int Kpad_m) {
     tmp_free(A0);
     // mask_layer weight: the mask is shared by the batch -> reduce dh over the batch first
     Tmp hs = tmp_alloc((size_t)V0 * nf * es * P);
-    if (!dry_) {
-      const void* src = dh.ptr; void* dst = hs.ptr;
-      add_bwd("stem.batch_sum", [=](cudaStream_t s, int B) { launch_batch_sum(src, dst, B, V0 * nf, nf, pr, s); }, kParamGradOnly);
-    }
+    const void* src = dh.ptr; void* dst = hs.ptr;
+    add_bwd("stem.batch_sum", [=](cudaStream_t s, int B) { launch_batch_sum(src, dst, B, V0 * nf, nf, pr, s); }, kParamGradOnly);
     {
       Act da; da.ptr = hs.ptr; da.C = nf; da.X = da.Y = da.Z = R0; da.B = 1;
       Act xa; xa.ptr = Am; xa.C = Kpad_m; xa.X = xa.Y = xa.Z = R0; xa.B = 1;
@@ -656,20 +614,16 @@ void UNet::tape_head(TensP h, TensP a, const std::string& gn_name, const std::st
     const int nf = cfg_.nf, R0 = cfg_.image_size, Cin = cfg_.num_channels, k = cfg_.stem_ksize, T = k * k * k;
     const long long V0 = (long long)R0 * R0 * R0;
     float* hw = P(conv_name + ".weight", {});
-    if (!dry_) {
-      const long long gb = G(conv_name + ".bias");
-      add_bwd("head.dbias", [=](cudaStream_t s, int B) { launch_rowsum_nc(rt_dout_, rt_grads_ + gb, B, Cin, V0, rt_accum_ ? 1 : 0, s); },
-              kParamGradOnly);
-    }
+    const long long gb = G(conv_name + ".bias");
+    add_bwd("head.dbias", [=](cudaStream_t s, int B) { launch_rowsum_nc(rt_dout_, rt_grads_ + gb, B, Cin, V0, rt_accum_ ? 1 : 0, s); },
+            kParamGradOnly);
     // im2col of dL/dout ([voxel][co*T + tap'], reading dout at v + off(tap')) serves both gradients:
     //   dW[co][c][T-1-tap'] = sum_v a[v][c] Ad[v][co*T + tap'],   da[v][c] = sum_k Ad[v][k] W[co][c][T-1-tap']
     const int Kp = ((Cin * T + 63) / 64) * 64;
     const Precision pr = prec_;
     Tmp Ad = tmp_alloc((size_t)cfg_.max_batch * V0 * Kp * esize(prec_) * parts(prec_));
-    if (!dry_) {
-      void* ad = Ad.ptr;
-      add_bwd("head.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_dout_, ad, B, Cin, R0, k, Kp, pr, s); });
-    }
+    void* ad = Ad.ptr;
+    add_bwd("head.im2col", [=](cudaStream_t s, int B) { launch_im2col(rt_dout_, ad, B, Cin, R0, k, Kp, pr, s); });
     Act ada; ada.ptr = Ad.ptr; ada.C = Kp; ada.X = ada.Y = ada.Z = R0; ada.B = cfg_.max_batch;
     {
       WgradOut o; o.sm = T; o.sn = -1; o.st = 0; o.ndiv = T; o.sn_hi = (long long)nf * T; o.n_valid = Cin * T;
@@ -690,7 +644,6 @@ void UNet::tape_head(TensP h, TensP a, const std::string& gn_name, const std::st
 // ------------------------------------------------------------------ time embedding (ddpm_res64.py:132-136, layers.py:680)
 void UNet::tape_temb() {
   tape_.push_back([=]() {
-    if (dry_) return;
     const int nf = cfg_.nf, tdim = 4 * nf, mb = cfg_.max_batch;
     float* tw0 = P("all_modules.0.weight", {}); float* tb0 = P("all_modules.0.bias", {});
     float* tw1 = P("all_modules.1.weight", {}); float* tb1 = P("all_modules.1.bias", {});

@@ -65,3 +65,35 @@ def grad_signature(name, g, seed=1234):
     r = torch.randn(4, g.numel(), generator=gen, dtype=torch.float64)
     gd = g.detach().double().reshape(-1).cpu()
     return np.concatenate([[gd.norm().item()], (r @ gd).numpy()])
+
+
+def engine_report(cfg, batch, precision, training, dry=True):
+    """What a score-network engine (or with dry=True its GPU-less plan) answers without running: mdb_unet_info, every
+    mdb_unet_gemm_ops row and, for a training plan, mdb_unet_train_info and mdb_unet_grad_ready of every parameter."""
+    import ctypes
+    from meshdiffusion_b200 import _native
+    from meshdiffusion_b200.diffusion.models import ddpm
+    L = _native.lib()
+    c = ddpm._config_c(ddpm.arch_from_config(cfg), batch, precision, training=training)
+    h = ctypes.c_void_p()
+    _native.check((L.mdb_unet_create_dry if dry else L.mdb_unet_create)(ctypes.byref(c), ctypes.byref(h)))
+    try:
+        fl, ar, ng, ns = ctypes.c_double(), ctypes.c_longlong(), ctypes.c_int(), ctypes.c_int()
+        _native.check(L.mdb_unet_info(h, ctypes.byref(fl), ctypes.byref(ar), ctypes.byref(ng), ctypes.byref(ns)))
+        r = {"flops": fl.value, "arena": ar.value, "n_gemm": ng.value, "n_steps": ns.value, "gemm_ops": []}
+        for i in range(ng.value):
+            name, f, fb = ctypes.c_char_p(), ctypes.c_double(), ctypes.c_double()
+            _native.check(L.mdb_unet_gemm_ops(h, i, ctypes.byref(name), ctypes.byref(f), ctypes.byref(fb)))
+            r["gemm_ops"].append((name.value.decode(), f.value, fb.value))
+        if training:
+            bf, nb, nu = ctypes.c_double(), ctypes.c_int(), ctypes.c_longlong()
+            _native.check(L.mdb_unet_train_info(h, ctypes.byref(bf), ctypes.byref(nb), ctypes.byref(nu)))
+            r.update(bwd_flops=bf.value, n_bwd_steps=nb.value, numel=nu.value, grad_ready={})
+            for i in range(L.mdb_unet_num_params(h)):
+                name, step = ctypes.c_char_p(), ctypes.c_int()
+                _native.check(L.mdb_unet_param_info(h, i, ctypes.byref(name), None, None, None))
+                _native.check(L.mdb_unet_grad_ready(h, name.value, ctypes.byref(step)))
+                r["grad_ready"][name.value.decode()] = step.value
+        return r
+    finally:
+        L.mdb_unet_destroy(h)

@@ -3,7 +3,7 @@ import ctypes
 import os
 import re
 
-from helpers import ROOT
+from helpers import ROOT, tiny_config
 
 
 def _declared():
@@ -53,6 +53,24 @@ def test_dry_plan_errors_are_reported_not_thrown():
     h = ctypes.c_void_p()
     rc = L.mdb_unet_create_dry(ctypes.byref(cfg), ctypes.byref(h))
     assert rc != 0 and b"image_size" in L.mdb_last_error()
+
+
+def test_dry_plan_refuses_to_run():
+    """The steps of a dry plan hold null pointers: the entry points that would run it report an error before anything is
+    enqueued (so this needs no GPU)."""
+    from meshdiffusion_b200 import _native
+    from meshdiffusion_b200.diffusion.models import ddpm
+    L = _native.lib()
+    cfg = ddpm._config_c(ddpm.arch_from_config(tiny_config("res64", "bf16")), 1, "bf16")
+    h = ctypes.c_void_p()
+    _native.check(L.mdb_unet_create_dry(ctypes.byref(cfg), ctypes.byref(h)))
+    try:
+        assert L.mdb_unet_commit(h, None) != 0
+        assert b"a dry plan cannot run" in L.mdb_last_error()
+        assert L.mdb_unet_forward(h, None, None, None, 1, None) != 0
+        assert b"a dry plan cannot run" in L.mdb_last_error()
+    finally:
+        L.mdb_unet_destroy(h)
 
 
 def test_groupnorm_entry_points_refuse_null_stats():

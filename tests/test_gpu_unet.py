@@ -9,7 +9,7 @@ and printed next to ours in test_res64_full_vs_oracle). bf16 operands: 4e-2.
 import pytest
 import torch
 
-from helpers import build_model, full_config, load_golden, rel_l2, rel_max, tiny_config
+from helpers import build_model, engine_report, full_config, load_golden, rel_l2, rel_max, tiny_config
 from oracle import synth, unet_oracle
 
 pytestmark = pytest.mark.gpu
@@ -117,3 +117,14 @@ def test_full_size_determinism_and_batch_invariance():
     c = model(x[:3].contiguous(), labels[:3].contiguous())
     assert torch.equal(a[:3], c), "a sample's output depends on the rest of the batch"
     assert torch.isfinite(a).all()
+
+
+@pytest.mark.parametrize("precision,training", [("bf16", False), ("tf32", False), ("bf16x3", False), ("bf16", True),
+                                                ("bf16x3", True)])
+def test_dry_plan_matches_engine(precision, training):
+    """The dry plan and the engine are built by the same code: they report the same launches, GEMM accounting, FLOPs,
+    arena, backward plan and gradient readiness."""
+    cfg = tiny_config("res64", precision)
+    dry = engine_report(cfg, 2, precision, training, dry=True)
+    assert dry["n_gemm"] > 0
+    assert engine_report(cfg, 2, precision, training, dry=False) == dry

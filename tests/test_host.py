@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import GOLD, ROOT, full_config, tiny_config
+from helpers import GOLD, ROOT, engine_report, full_config, tiny_config
 
 
 @pytest.mark.parametrize("name", ["res64", "res128"])
@@ -363,3 +363,21 @@ def test_trainer_loop_bounds_checkpoint_names_and_resume(tmp_path, monkeypatch):
     trainer.train(cfg)
     assert [c[0] for c in calls] == [8, 9, 10, 11, 12, 13]
     assert "checkpoint_6.pth" in os.listdir(ck)
+
+
+@pytest.mark.parametrize("name", ["tiny", "res64"])
+def test_dry_inference_plan_accounting(name):
+    """A dry plan describes every GEMM launch of the engine without a GPU: the three operand modes run the same launches
+    and FLOPs, and split bf16 fills shared memory with exactly twice the bf16 bytes."""
+    reports = {}
+    for prec in ("bf16", "tf32", "bf16x3"):
+        cfg = tiny_config("res64", prec) if name == "tiny" else full_config("res64", prec)
+        reports[prec] = r = engine_report(cfg, 1, prec, training=False)
+        assert r["n_gemm"] > 0 and r["n_steps"] > r["n_gemm"] and r["flops"] > 0
+    ops = {prec: r["gemm_ops"] for prec, r in reports.items()}
+    assert [o[:2] for o in ops["bf16"]] == [o[:2] for o in ops["tf32"]] == [o[:2] for o in ops["bf16x3"]]
+    for (op, _, fb1), (_, _, fb3) in zip(ops["bf16"], ops["bf16x3"]):
+        assert fb1 > 0 and fb3 == 2 * fb1, op
+    if name == "res64":  # DESIGN section 3: 5.47 TFLOP per sample-evaluation over 142 GEMM launches
+        r = reports["bf16x3"]
+        assert (r["n_gemm"], r["n_steps"], r["flops"]) == (142, 235, 5_466_260_242_432)
