@@ -45,7 +45,7 @@ typedef struct mdb_unet_config {
 
 int mdb_unet_create(const mdb_unet_config* cfg, mdb_unet** out);
 /* Plan only, no GPU needed: built by the same code as mdb_unet_create, so it answers the parameter table, arena size,
- * step and GEMM counts, mdb_unet_gemm_ops, FLOPs, mdb_unet_train_info and mdb_unet_grad_ready. It cannot run:
+ * step and GEMM counts, mdb_unet_gemm_ops, mdb_unet_gemm_slots, FLOPs, mdb_unet_train_info and mdb_unet_grad_ready. It cannot run:
  * set/get_param, commit, forward, backward* and profile* return an error. */
 int mdb_unet_create_dry(const mdb_unet_config* cfg, mdb_unet** out);
 void mdb_unet_destroy(mdb_unet* net);
@@ -71,6 +71,9 @@ int mdb_unet_info(mdb_unet* net, double* flops_per_sample, long long* arena_byte
 /* Forward GEMM launch i (0 <= i < n_gemm_launches) at the engine's max batch: its step name (valid while the engine
  * lives), executed FLOPs and the bytes TMA writes into shared memory (A boxes + weight tiles, summed over output tiles). */
 int mdb_unet_gemm_ops(mdb_unet* net, int i, const char** name, double* flops, double* fill_bytes);
+/* Operand ring depth of forward GEMM launch i: the A slots (entries in flight) and B slots (k-steps of weight tiles in
+ * flight) it takes under the current MDB_MAX_STAGES / MDB_MAX_BSLOTS, and the dynamic shared memory it requests. */
+int mdb_unet_gemm_slots(mdb_unet* net, int i, int* a_slots, int* b_slots, int* smem_bytes);
 /* One profiled forward: per-step device milliseconds. names_buf receives '\n'-separated step names. Synchronises. */
 int mdb_unet_profile(mdb_unet* net, const float* x, const float* labels, float* out, int batch, void* stream,
                      char* names_buf, int names_len, float* ms, int max_steps, int* n_steps);

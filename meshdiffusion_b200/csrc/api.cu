@@ -119,6 +119,17 @@ int mdb_unet_gemm_ops(mdb_unet* n, int i, const char** name, double* flops, doub
   MDB_API_END
 }
 
+int mdb_unet_gemm_slots(mdb_unet* n, int i, int* a_slots, int* b_slots, int* smem_bytes) {
+  MDB_API_BEGIN
+  if (i < 0 || i >= n->net->num_gemm_launches()) throw std::runtime_error("mdb: GEMM launch index out of range");
+  int a = 0, b = 0, sm = 0;
+  n->net->gemm(i).slots(a, b, sm);
+  if (a_slots) *a_slots = a;
+  if (b_slots) *b_slots = b;
+  if (smem_bytes) *smem_bytes = sm;
+  MDB_API_END
+}
+
 int mdb_unet_profile(mdb_unet* n, const float* x, const float* labels, float* out, int B, void* stream, char* names,
                      int names_len, float* ms, int max_steps, int* nsteps) {
   MDB_API_BEGIN

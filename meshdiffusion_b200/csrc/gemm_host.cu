@@ -46,27 +46,39 @@ void encode_map(CUtensorMap* m, Precision prec, int rank, void* base, const uint
   }
 }
 
-void GemmOp::pick_slots(GemmParams& q) const {
+int GemmOp::pick_slots(GemmParams& q) const {
   // Operand rings of this op in the shared memory left next to the epilogue scratch: two slots of each at least (one
   // filling while one is read). Then B slots are added until they cover the k-steps of every A slot in flight, and A slots
-  // (entries in flight) up to MDB_MAX_STAGES (default 4), whichever is behind and still fits.
-  const int fixed = block_n == 32 ? GemmCfg<32>::kFixedBytes : GemmCfg<128>::kFixedBytes;
+  // (entries in flight) up to MDB_MAX_STAGES (default 4), whichever is behind and still fits. MDB_MAX_BSLOTS caps the B
+  // slots (weight lookahead) the same way; both change timing only, never results.
+  const int fixed = block_n == 32 ? GemmCfg<32>::kFixedBytes : gnb ? GemmCfg<128, true>::kFixedBytes : GemmCfg<128>::kFixedBytes;
   const int budget = kMaxDynSmem - fixed;
   q.a_slot_bytes = (a_slot_need + 1023) / 1024 * 1024;
   q.b_slot_bytes = parts(prec) * block_n * kRowBytes;
-  int cap = 4;
-  if (const char* e = getenv("MDB_MAX_STAGES")) { const int c = atoi(e); if (c >= 2) cap = c; }
-  if (cap > kMaxSlots) cap = kMaxSlots;
+  auto env_cap = [](const char* name, int def) {
+    int cap = def;
+    if (const char* e = getenv(name)) { const int c = atoi(e); if (c >= 2) cap = c; }
+    return cap < kMaxSlots ? cap : kMaxSlots;
+  };
+  const int cap = env_cap("MDB_MAX_STAGES", 4), bcap = env_cap("MDB_MAX_BSLOTS", kMaxSlots);
   int na = 2, nb = 2;
   int used = na * q.a_slot_bytes + nb * q.b_slot_bytes;
   if (used > budget) throw std::runtime_error("mdb: operand rings need at least two slots each");
   for (;;) {
-    if (nb < na * nk_max && nb < kMaxSlots && used + q.b_slot_bytes <= budget) { ++nb; used += q.b_slot_bytes; }
+    if (nb < na * nk_max && nb < bcap && used + q.b_slot_bytes <= budget) { ++nb; used += q.b_slot_bytes; }
     else if (na < cap && used + q.a_slot_bytes <= budget) { ++na; used += q.a_slot_bytes; }
     else break;
   }
   q.n_aslots = na;
   q.n_bslots = nb;
+  return fixed + used;
+}
+
+void GemmOp::slots(int& a_slots, int& b_slots, int& smem_bytes) const {
+  GemmParams q = p;
+  smem_bytes = pick_slots(q);
+  a_slots = q.n_aslots;
+  b_slots = q.n_bslots;
 }
 
 double GemmOp::fill_bytes(int B) const {
@@ -529,10 +541,9 @@ void GemmOp::upload(cudaStream_t stream) {
 }
 
 template <int BN, bool TF32, bool GNB = false, bool X3 = false>
-static void launch_impl(const GemmParams& p, int grid, cudaStream_t stream) {
+static void launch_impl(const GemmParams& p, int grid, int smem, cudaStream_t stream) {
   static bool configured[64] = {};  // the attribute is per device
   auto kern = gemm_tc_kernel<BN, TF32, GNB, X3>;
-  const int smem = GemmCfg<BN>::kFixedBytes + p.n_aslots * p.a_slot_bytes + p.n_bslots * p.b_slot_bytes;
   int dev = 0;
   MDB_CUDA_CHECK(cudaGetDevice(&dev));
   if (dev >= 64 || !configured[dev]) {
@@ -545,7 +556,7 @@ static void launch_impl(const GemmParams& p, int grid, cudaStream_t stream) {
 
 void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
   GemmParams p = this->p;
-  pick_slots(p);
+  const int smem = pick_slots(p);
   if (B > 0) {
     if (B > this->p.Bn) throw std::runtime_error("mdb: batch exceeds the batch the op was built for");
     p.Bn = B;
@@ -560,21 +571,21 @@ void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
     if (tf || p.splits > 1) throw std::runtime_error("mdb: GroupNorm-backward epilogue: bf16 or split bf16, no split-K");
     p.gnb_drop_thresh = rt_drop_thresh; p.gnb_drop_scale = rt_drop_scale; p.gnb_seed = rt_seed;
     if (prec == kBF16X3) {
-      if (block_n == 32) launch_impl<32, false, true, true>(p, grid, stream); else launch_impl<128, false, true, true>(p, grid, stream);
+      if (block_n == 32) launch_impl<32, false, true, true>(p, grid, smem, stream); else launch_impl<128, false, true, true>(p, grid, smem, stream);
     } else {
-      if (block_n == 32) launch_impl<32, false, true>(p, grid, stream); else launch_impl<128, false, true>(p, grid, stream);
+      if (block_n == 32) launch_impl<32, false, true>(p, grid, smem, stream); else launch_impl<128, false, true>(p, grid, smem, stream);
     }
     return;
   }
   const bool x3 = prec == kBF16X3;
   if (block_n == 32) {
-    if (tf) launch_impl<32, true>(p, grid, stream);
-    else if (x3) launch_impl<32, false, false, true>(p, grid, stream);
-    else launch_impl<32, false>(p, grid, stream);
+    if (tf) launch_impl<32, true>(p, grid, smem, stream);
+    else if (x3) launch_impl<32, false, false, true>(p, grid, smem, stream);
+    else launch_impl<32, false>(p, grid, smem, stream);
   } else {
-    if (tf) launch_impl<128, true>(p, grid, stream);
-    else if (x3) launch_impl<128, false, false, true>(p, grid, stream);
-    else launch_impl<128, false>(p, grid, stream);
+    if (tf) launch_impl<128, true>(p, grid, smem, stream);
+    else if (x3) launch_impl<128, false, false, true>(p, grid, smem, stream);
+    else launch_impl<128, false>(p, grid, smem, stream);
   }
   if (p.splits > 1) {
     SplitReduceArgs a{};

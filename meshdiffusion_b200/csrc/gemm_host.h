@@ -146,13 +146,16 @@ class GemmOp {
   void launch(cudaStream_t stream, int B = -1, void* out_override = nullptr) const;
   // bytes TMA writes into shared memory in one launch at batch B (<= 0: the batch the op was built for)
   double fill_bytes(int B = -1) const;
+  // After finalize (host only): the A and B slots a launch takes under the current MDB_MAX_STAGES / MDB_MAX_BSLOTS and
+  // the dynamic shared memory it requests
+  void slots(int& a_slots, int& b_slots, int& smem_bytes) const;
 
  private:
   Geometry geo{};
   bool b_from_act = false;
   int a_slot_need = 0;  // bytes of the largest A box (X3: both parts): the A slot size
   int nk_max = 0;       // most k-steps of one entry
-  void pick_slots(GemmParams& q) const;
+  int pick_slots(GemmParams& q) const;  // sets the ring depths of q; returns the dynamic shared memory bytes
   long long b_lo_off = 0;  // X3 activation-B: K coordinate of the lo parts
   std::vector<MapDesc> amaps_;  // p.amap[i] once uploaded
   MapDesc bmap_;                // p.bmap once uploaded (packed weights: described by upload itself)

@@ -12,9 +12,10 @@
 // * B is the packed weight matrix [N][Ktot] (K-major) whose K order is exactly the k-step order of the load
 //   table, fetched by TMA as (KB x BLOCK_N) tiles.
 // * Accumulators live in registers: each of the two consumer warpgroups owns 64 rows of the tile (wgmma m64nNk16 /
-//   m64nNk8). After the last k-step they are staged through shared memory, and the same 256 threads read them back one
-//   row per thread to add bias / time-embedding bias / residual, store NDHWC output and reduce per-(sample, channel)
-//   sum and sum-of-squares for the GroupNorm that follows (warp-shuffle butterfly + shared + one atomic per channel).
+//   m64nNk8). After the last k-step they are staged through shared memory (64 columns at a time), and the same 256
+//   threads read them back one row per thread to add bias / time-embedding bias / residual, store NDHWC output and
+//   reduce per-(sample, channel) sum and sum-of-squares for the GroupNorm that follows (warp-shuffle butterfly + shared
+//   + one atomic per channel).
 //
 // Warp roles (384 threads): warpgroup 0 = TMA producer (warp 0), warpgroups 1-2 = MMA + epilogue.
 #pragma once
@@ -121,12 +122,19 @@ struct GemmParams {
 
 constexpr int kMaxSlots = 8;  // per ring
 constexpr int kMaxDynSmem = 232448;  // 227 KB: the opt-in limit of dynamic shared memory per block on sm_90
-template <int BLOCK_N>
+// kWholeTile: stage all BLOCK_N columns in one round (the GroupNorm-backward epilogues: the split-bf16 one spills
+// registers when round 1's accumulators stay live through round 0, the bf16 one runs slower)
+template <int BLOCK_N, bool kWholeTile = false>
 struct GemmCfg {
   static constexpr int kBTileBytes = BLOCK_N * kRowBytes;  // weight tile bytes per k-step
   static constexpr int kStatsFloats = 24 * BLOCK_N;  // 2 x [4 warps][sum,sumsq][N] column partials + 2 x [4 segs][N] bias
-  // accumulator staging [128 rows][kAccPitch]: the 4-float pad keeps the row-per-lane float4 reads conflict-free
-  static constexpr int kAccPitch = BLOCK_N + 4;
+  // accumulator staging [128 rows][kAccPitch], in kStageRounds rounds of kStageCols columns: 64-column rounds leave the
+  // operand rings 32 KB more than staging all 128 columns at once would. The 4-float pad keeps the row-per-lane float4
+  // reads conflict-free.
+  static constexpr int kStageCols = (kWholeTile || BLOCK_N < 64) ? BLOCK_N : 64;
+  static constexpr int kStageRounds = BLOCK_N / kStageCols;
+  static_assert(kStageRounds <= 2, "the epilogue stages at most two rounds");
+  static constexpr int kAccPitch = kStageCols + 4;
   static constexpr int kAccFloats = kBlockM * kAccPitch;
   // everything but the operand rings: alignment slack, accumulator staging, epilogue scratch, mbarriers (full / empty of
   // both rings)
@@ -147,7 +155,7 @@ __device__ __forceinline__ uint64_t kdesc(uint32_t saddr) { return make_wgmma_de
 // would cap the gradient accuracy near 5e-4).
 template <int BLOCK_N, bool TF32, bool GNB = false, bool X3 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
-  using Cfg = GemmCfg<BLOCK_N>;
+  using Cfg = GemmCfg<BLOCK_N, GNB>;
   constexpr int kParts = X3 ? 2 : 1;  // operand parts per A box / per k-step of weights
   const int NA = p.n_aslots, NB = p.n_bslots;
   const uint32_t a_slot = (uint32_t)p.a_slot_bytes, b_slot = (uint32_t)p.b_slot_bytes;
@@ -351,16 +359,24 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
       const long long ooff = xg * p.osx + yg * p.osy + zg * p.osz + bg * p.osb;
       const long long roff = xg * p.rsx + yg * p.rsy + zg * p.rsz + bg * p.rsb;
 
-      // accumulators -> shared staging (the previous tile's epilogue must be done reading it first). wgmma layout:
-      // register 4j+{0,1} = (row l/4, cols 8j + 2(l%4) + {0,1}), 4j+{2,3} = the same columns 8 rows further down.
-      named_bar_sync(2, kEpiThreads);
-      {
+      // accumulators -> shared staging, one round of kStageCols columns at a time. wgmma layout: register 4j+{0,1} =
+      // (row l/4, cols 8j + 2(l%4) + {0,1}), 4j+{2,3} = the same columns 8 rows further down, so the columns of round r
+      // are acc[kRoundRegs * r, kRoundRegs * (r + 1)).
+      constexpr int kRoundRegs = Cfg::kStageCols / 2;
+      auto stage = [&]() {
         const int w4 = (warp & 3), srow = wg * 64 + w4 * 16 + (lane >> 2), scol = 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
+        for (int j = 0; j < Cfg::kStageCols / 8; ++j) {
           *reinterpret_cast<float2*>(s_acc + srow * Cfg::kAccPitch + 8 * j + scol) = make_float2(acc[4 * j], acc[4 * j + 1]);
           *reinterpret_cast<float2*>(s_acc + (srow + 8) * Cfg::kAccPitch + 8 * j + scol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
+      };
+      named_bar_sync(2, kEpiThreads);  // the previous tile's epilogue is done reading the staging
+      stage();
+      // round 1's registers take the place of round 0's, so that the (rolled) round loop below stages the same registers
+      if constexpr (Cfg::kStageRounds > 1) {
+#pragma unroll
+        for (int i = 0; i < kRoundRegs; ++i) acc[i] = acc[kRoundRegs + i];
       }
 
       // stage bias + per-sample (time-embedding) bias of this tile's columns, s_bias[seg][col] -- only when the tile's
@@ -422,183 +438,194 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
       const int ch0 = kChunkStep == 2 ? half : 0;
       const bool active = kChunkStep == 2 || half == 0;  // BLOCK_N == 32: one chunk, the second warp of a quarter idles
       if (active) prefetch_res(ch0);
-      named_bar_sync(2, kEpiThreads);  // staged accumulators (and bias) visible to every epilogue thread
+
+      // the chunks of round r are [kRoundChunks * r, kRoundChunks * (r + 1)); each warp takes its own in the same order
+      // (half, half + 2, ...) as from a single round
+      constexpr int kRoundChunks = Cfg::kStageCols / 32;
+#pragma unroll 1
+      for (int rnd = 0; rnd < Cfg::kStageRounds; ++rnd) {
+        if (rnd > 0) {
+          named_bar_sync(2, kEpiThreads);  // every warp is done reading the previous round
+          stage();
+        }
+        named_bar_sync(2, kEpiThreads);  // staged accumulators (and bias) visible to every epilogue thread
 
 #pragma unroll 1
-      for (int ch = ch0; ch < kChunks && active; ch += kChunkStep) {
-        uint32_t rr[32];
-        {
-          const float4* src = reinterpret_cast<const float4*>(s_acc + row * Cfg::kAccPitch + ch * 32);
+        for (int ch = ch0 + rnd * kRoundChunks; ch < (rnd + 1) * kRoundChunks && active; ch += kChunkStep) {
+          uint32_t rr[32];
+          {
+            const float4* src = reinterpret_cast<const float4*>(s_acc + row * Cfg::kAccPitch + (ch - rnd * kRoundChunks) * 32);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 t = src[i];
-            rr[4 * i] = __float_as_uint(t.x); rr[4 * i + 1] = __float_as_uint(t.y);
-            rr[4 * i + 2] = __float_as_uint(t.z); rr[4 * i + 3] = __float_as_uint(t.w);
-          }
-        }
-        const int nb = n0 + ch * 32;
-        if (nb >= p.N) continue;  // warp-uniform
-        if (splits > 1) {
-          // split-K: raw fp32 partial sums; bias / residual / statistics are applied by the reduction kernel
-          if (valid) {
-            // (X3: ooff is in physical bf16 elements, twice the logical row pitch the fp32 partials use)
-            float* pp = p.partial + (long long)(tile % splits) * p.split_stride + (X3 ? (ooff >> 1) : ooff) + nb;
-            if (nb + 32 <= p.N) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                reinterpret_cast<float4*>(pp)[i] = make_float4(__uint_as_float(rr[4 * i]), __uint_as_float(rr[4 * i + 1]),
-                                                               __uint_as_float(rr[4 * i + 2]), __uint_as_float(rr[4 * i + 3]));
-            } else {
-              for (int i = 0; i < 32; ++i) if (nb + i < p.N) pp[i] = __uint_as_float(rr[i]);
+            for (int i = 0; i < 8; ++i) {
+              const float4 t = src[i];
+              rr[4 * i] = __float_as_uint(t.x); rr[4 * i + 1] = __float_as_uint(t.y);
+              rr[4 * i + 2] = __float_as_uint(t.z); rr[4 * i + 3] = __float_as_uint(t.w);
             }
           }
-          continue;
-        }
-        const bool full = (nb + 32 <= p.N) && (p.ocs == 1);
-        float v[32];
-        const float mbias = (p.bias && p.bias_on_m && valid) ? __ldg(p.bias + xg) : 0.f;
-        const float* sb = s_bias + (seg < 4 ? seg : 0) * BLOCK_N + ch * 32;
+          const int nb = n0 + ch * 32;
+          if (nb >= p.N) continue;  // warp-uniform
+          if (splits > 1) {
+            // split-K: raw fp32 partial sums; bias / residual / statistics are applied by the reduction kernel
+            if (valid) {
+              // (X3: ooff is in physical bf16 elements, twice the logical row pitch the fp32 partials use)
+              float* pp = p.partial + (long long)(tile % splits) * p.split_stride + (X3 ? (ooff >> 1) : ooff) + nb;
+              if (nb + 32 <= p.N) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rr[i]) * p.alpha + mbias + sb[i];
-        float q2[GNB ? 32 : 1];  // dy * xhat (GNB)
-        if constexpr (GNB) {
-          if (valid) {
-            const float4* cc = p.gnb_c + static_cast<long long>(bg) * p.N + nb;
-            // dropout mask of act_format.cuh (apply_dropout, interleaved with the loop below: the helper's separate pass
-            // changes this instantiation's register allocation)
-            unsigned long long hsh[8];
-            if (p.gnb_drop_thresh > 0) {
-              const unsigned long long e4 = (unsigned long long)((((static_cast<long long>(bg) * p.Z + zg) * p.Y + yg) * p.X + xg) * p.N + nb) >> 2;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) hsh[i] = drop_hash64(p.gnb_seed, e4 + i);
+                for (int i = 0; i < 8; ++i)
+                  reinterpret_cast<float4*>(pp)[i] = make_float4(__uint_as_float(rr[4 * i]), __uint_as_float(rr[4 * i + 1]),
+                                                                 __uint_as_float(rr[4 * i + 2]), __uint_as_float(rr[4 * i + 3]));
+              } else {
+                for (int i = 0; i < 32; ++i) if (nb + i < p.N) pp[i] = __uint_as_float(rr[i]);
+              }
             }
+            continue;
+          }
+          const bool full = (nb + 32 <= p.N) && (p.ocs == 1);
+          float v[32];
+          const float mbias = (p.bias && p.bias_on_m && valid) ? __ldg(p.bias + xg) : 0.f;
+          const float* sb = s_bias + (seg < 4 ? seg : 0) * BLOCK_N + ch * 32;
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const float4 kc = __ldg(cc + i);
-              const __nv_bfloat16 xb = reinterpret_cast<const __nv_bfloat16*>(rbuf)[i];
-              float xv = __bfloat162float(xb);
-              if constexpr (X3) xv += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(rbuf + 4)[i]);
-              float d = v[i];
+          for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rr[i]) * p.alpha + mbias + sb[i];
+          float q2[GNB ? 32 : 1];  // dy * xhat (GNB)
+          if constexpr (GNB) {
+            if (valid) {
+              const float4* cc = p.gnb_c + static_cast<long long>(bg) * p.N + nb;
+              // dropout mask of act_format.cuh (apply_dropout, interleaved with the loop below: the helper's separate pass
+              // changes this instantiation's register allocation)
+              unsigned long long hsh[8];
               if (p.gnb_drop_thresh > 0) {
-                const unsigned r16 = (unsigned)((hsh[i >> 2] >> (16 * (i & 3))) & 0xFFFFu);
-                d = r16 >= (unsigned)p.gnb_drop_thresh ? d * p.gnb_drop_scale : 0.f;
+                const unsigned long long e4 = (unsigned long long)((((static_cast<long long>(bg) * p.Z + zg) * p.Y + yg) * p.X + xg) * p.N + nb) >> 2;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) hsh[i] = drop_hash64(p.gnb_seed, e4 + i);
               }
-              if (p.gnb_silu) {
-                const float h = fmaf(xv, kc.x, kc.y);
-                d *= X3 ? dsilu_ex2_half(h) : dsilu_tanh_half(h);
-              }
-              v[i] = d;
-              q2[i] = d * fmaf(xv, kc.z, kc.w);
-            }
-          } else {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) q2[i] = 0.f;
-          }
-        }
-        if (!GNB && p.res && valid) {
-          if (TF32 || p.res_fp32) {
-            if (full) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 t = *reinterpret_cast<const float4*>(&rbuf[i]);
-                v[4 * i] += t.x; v[4 * i + 1] += t.y; v[4 * i + 2] += t.z; v[4 * i + 3] += t.w;
-              }
-            } else {
-              const float* rp = reinterpret_cast<const float*>(p.res) + roff + nb;
-              for (int i = 0; i < 32; ++i) if (nb + i < p.N) v[i] += rp[i];
-            }
-          } else {
-            if (full) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&rbuf[i]);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  float2 f = __bfloat1622float2(h[j]);
-                  if constexpr (X3) {
-                    const float2 l = __bfloat1622float2(reinterpret_cast<const __nv_bfloat162*>(&rbuf[4 + i])[j]);
-                    f.x += l.x; f.y += l.y;
-                  }
-                  v[8 * i + 2 * j] += f.x; v[8 * i + 2 * j + 1] += f.y;
+              for (int i = 0; i < 32; ++i) {
+                const float4 kc = __ldg(cc + i);
+                const __nv_bfloat16 xb = reinterpret_cast<const __nv_bfloat16*>(rbuf)[i];
+                float xv = __bfloat162float(xb);
+                if constexpr (X3) xv += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(rbuf + 4)[i]);
+                float d = v[i];
+                if (p.gnb_drop_thresh > 0) {
+                  const unsigned r16 = (unsigned)((hsh[i >> 2] >> (16 * (i & 3))) & 0xFFFFu);
+                  d = r16 >= (unsigned)p.gnb_drop_thresh ? d * p.gnb_drop_scale : 0.f;
                 }
+                if (p.gnb_silu) {
+                  const float h = fmaf(xv, kc.x, kc.y);
+                  d *= X3 ? dsilu_ex2_half(h) : dsilu_tanh_half(h);
+                }
+                v[i] = d;
+                q2[i] = d * fmaf(xv, kc.z, kc.w);
               }
             } else {
-              const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.res) + roff + nb;
-              for (int i = 0; i < 32; ++i)
-                if (nb + i < p.N) v[i] += __bfloat162float(rp[i]) + (X3 ? __bfloat162float(rp[i + p.res_lo_off]) : 0.f);
+#pragma unroll
+              for (int i = 0; i < 32; ++i) q2[i] = 0.f;
             }
           }
-        }
-        if (ch + kChunkStep < kChunks) prefetch_res(ch + kChunkStep);  // lands while this chunk is stored / reduced
-        if (valid) {
-          if (TF32 || p.out_fp32) {
-            float* op = reinterpret_cast<float*>(p.out) + ooff + nb;
-            if (full) {
+          if (!GNB && p.res && valid) {
+            if (TF32 || p.res_fp32) {
+              if (full) {
 #pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                float4 t = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-                if (p.round_out) { t.x = to_tf32_rna(t.x); t.y = to_tf32_rna(t.y); t.z = to_tf32_rna(t.z); t.w = to_tf32_rna(t.w); }
-                reinterpret_cast<float4*>(op)[i] = t;
+                for (int i = 0; i < 8; ++i) {
+                  const float4 t = *reinterpret_cast<const float4*>(&rbuf[i]);
+                  v[4 * i] += t.x; v[4 * i + 1] += t.y; v[4 * i + 2] += t.z; v[4 * i + 3] += t.w;
+                }
+              } else {
+                const float* rp = reinterpret_cast<const float*>(p.res) + roff + nb;
+                for (int i = 0; i < 32; ++i) if (nb + i < p.N) v[i] += rp[i];
               }
             } else {
-              for (int i = 0; i < 32; ++i) if (nb + i < p.N) op[i * p.ocs] = v[i];
-            }
-          } else {
-            __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + ooff + nb;
-            if (full) {
+              if (full) {
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                uint4 t;
-                __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&t);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) h[j] = __floats2bfloat162_rn(v[8 * i + 2 * j], v[8 * i + 2 * j + 1]);
-                reinterpret_cast<uint4*>(op)[i] = t;
-                if constexpr (X3) {  // lo parts: what the bf16 rounding of the hi parts lost
-                  uint4 tl;
-                  __nv_bfloat162* l = reinterpret_cast<__nv_bfloat162*>(&tl);
+                for (int i = 0; i < 4; ++i) {
+                  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&rbuf[i]);
 #pragma unroll
                   for (int j = 0; j < 4; ++j) {
-                    const float2 f = __bfloat1622float2(h[j]);
-                    l[j] = __floats2bfloat162_rn(v[8 * i + 2 * j] - f.x, v[8 * i + 2 * j + 1] - f.y);
+                    float2 f = __bfloat1622float2(h[j]);
+                    if constexpr (X3) {
+                      const float2 l = __bfloat1622float2(reinterpret_cast<const __nv_bfloat162*>(&rbuf[4 + i])[j]);
+                      f.x += l.x; f.y += l.y;
+                    }
+                    v[8 * i + 2 * j] += f.x; v[8 * i + 2 * j + 1] += f.y;
                   }
-                  reinterpret_cast<uint4*>(op + p.out_lo_off)[i] = tl;
                 }
+              } else {
+                const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.res) + roff + nb;
+                for (int i = 0; i < 32; ++i)
+                  if (nb + i < p.N) v[i] += __bfloat162float(rp[i]) + (X3 ? __bfloat162float(rp[i + p.res_lo_off]) : 0.f);
+              }
+            }
+          }
+          if (ch + kChunkStep < kChunks) prefetch_res(ch + kChunkStep);  // lands while this chunk is stored / reduced
+          if (valid) {
+            if (TF32 || p.out_fp32) {
+              float* op = reinterpret_cast<float*>(p.out) + ooff + nb;
+              if (full) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                  float4 t = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+                  if (p.round_out) { t.x = to_tf32_rna(t.x); t.y = to_tf32_rna(t.y); t.z = to_tf32_rna(t.z); t.w = to_tf32_rna(t.w); }
+                  reinterpret_cast<float4*>(op)[i] = t;
+                }
+              } else {
+                for (int i = 0; i < 32; ++i) if (nb + i < p.N) op[i * p.ocs] = v[i];
               }
             } else {
-              for (int i = 0; i < 32; ++i)
-                if (nb + i < p.N) {
-                  const __nv_bfloat16 hb = __float2bfloat16(v[i]);
-                  op[i * p.ocs] = hb;
-                  if constexpr (X3) op[i * p.ocs + p.out_lo_off] = __float2bfloat16(v[i] - __bfloat162float(hb));
+              __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + ooff + nb;
+              if (full) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                  uint4 t;
+                  __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&t);
+#pragma unroll
+                  for (int j = 0; j < 4; ++j) h[j] = __floats2bfloat162_rn(v[8 * i + 2 * j], v[8 * i + 2 * j + 1]);
+                  reinterpret_cast<uint4*>(op)[i] = t;
+                  if constexpr (X3) {  // lo parts: what the bf16 rounding of the hi parts lost
+                    uint4 tl;
+                    __nv_bfloat162* l = reinterpret_cast<__nv_bfloat162*>(&tl);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                      const float2 f = __bfloat1622float2(h[j]);
+                      l[j] = __floats2bfloat162_rn(v[8 * i + 2 * j] - f.x, v[8 * i + 2 * j + 1] - f.y);
+                    }
+                    reinterpret_cast<uint4*>(op + p.out_lo_off)[i] = tl;
+                  }
                 }
+              } else {
+                for (int i = 0; i < 32; ++i)
+                  if (nb + i < p.N) {
+                    const __nv_bfloat16 hb = __float2bfloat16(v[i]);
+                    op[i * p.ocs] = hb;
+                    if constexpr (X3) op[i * p.ocs + p.out_lo_off] = __float2bfloat16(v[i] - __bfloat162float(hb));
+                  }
+              }
             }
           }
-        }
-        if (GNB ? (want_cols != 0) : (p.stats != nullptr)) {  // (never reached in split-K mode)
-          // Column sums over the warp's 32 rows: butterfly transpose-reduce (31 shuffles per quantity);
-          // afterwards lane i holds the sum of column i.
-          float s[32], ss[32];
+          if (GNB ? (want_cols != 0) : (p.stats != nullptr)) {  // (never reached in split-K mode)
+            // Column sums over the warp's 32 rows: butterfly transpose-reduce (31 shuffles per quantity);
+            // afterwards lane i holds the sum of column i.
+            float s[32], ss[32];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float t = valid ? v[i] : 0.f;
-            s[i] = t; ss[i] = GNB ? q2[GNB ? i : 0] : t * t;
-          }
-#pragma unroll
-          for (int off = 16; off >= 1; off >>= 1) {
-            const bool hi = (lane & off) != 0;
-#pragma unroll
-            for (int i = 0; i < off; ++i) {
-              const float send_s = hi ? s[i] : s[i + off];
-              const float send_q = hi ? ss[i] : ss[i + off];
-              const float keep_s = hi ? s[i + off] : s[i];
-              const float keep_q = hi ? ss[i + off] : ss[i];
-              s[i] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, off);
-              ss[i] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, off);
+            for (int i = 0; i < 32; ++i) {
+              const float t = valid ? v[i] : 0.f;
+              s[i] = t; ss[i] = GNB ? q2[GNB ? i : 0] : t * t;
             }
+#pragma unroll
+            for (int off = 16; off >= 1; off >>= 1) {
+              const bool hi = (lane & off) != 0;
+#pragma unroll
+              for (int i = 0; i < off; ++i) {
+                const float send_s = hi ? s[i] : s[i + off];
+                const float send_q = hi ? ss[i] : ss[i + off];
+                const float keep_s = hi ? s[i + off] : s[i];
+                const float keep_q = hi ? ss[i + off] : ss[i];
+                s[i] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, off);
+                ss[i] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, off);
+              }
+            }
+            // per-warp slot, no atomics: the cross-warp sum below runs in a fixed order (deterministic results)
+            s_part[(q * 2 + 0) * BLOCK_N + ch * 32 + lane] = s[0];
+            s_part[(q * 2 + 1) * BLOCK_N + ch * 32 + lane] = ss[0];
           }
-          // per-warp slot, no atomics: the cross-warp sum below runs in a fixed order (deterministic results)
-          s_part[(q * 2 + 0) * BLOCK_N + ch * 32 + lane] = s[0];
-          s_part[(q * 2 + 1) * BLOCK_N + ch * 32 + lane] = ss[0];
         }
       }
       if constexpr (GNB) {

@@ -569,6 +569,17 @@ class ScoreNet(nn.Module):
             rows.append((name.value.decode(), fl.value, fb.value))
         return rows
 
+    def gemm_slots(self):
+        """Per forward GEMM launch: (A slots, B slots, dynamic shared memory bytes) under the current MDB_MAX_STAGES /
+        MDB_MAX_BSLOTS."""
+        L = _native.lib()
+        rows = []
+        for i in range(self.engine_info()["gemm_launches"]):
+            a, b, sm = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+            _native.check(L.mdb_unet_gemm_slots(self._handle, i, ctypes.byref(a), ctypes.byref(b), ctypes.byref(sm)))
+            rows.append((a.value, b.value, sm.value))
+        return rows
+
     def profile(self, x, labels):
         """One profiled forward: [(step name, device ms)]."""
         L = _native.lib()

@@ -5,7 +5,8 @@ One forward at batch 32 (synthetic weights, seeded input) in the given operand m
 (`ScoreNet.profile`, best of --reps forwards per launch after --warmup forwards). For every GEMM launch it prints the
 time, the issued TFLOP/s (executed FLOPs x tensor instructions per product: 1 bf16, 2 tf32, 3 bf16x3, over the time)
 and the fill rate (bytes TMA writes into shared memory, from `mdb_unet_gemm_ops`, over the time), then the ten
-slowest launches. The card's name, power limit and SM clock are read in the same process.
+slowest launches with their operand ring depth (A / B slots from `mdb_unet_gemm_slots`: MDB_MAX_STAGES and MDB_MAX_BSLOTS
+cap them). The card's name, power limit and SM clock are read in the same process.
 
     python tools/bench_gemm_ops.py --precision bf16x3 [--batch 32] [--json out.json]
 """
@@ -56,10 +57,11 @@ def run(precision, batch=32, warmup=2, reps=3):
     ops = net.gemm_ops()
     per = MMA_PER_PRODUCT[precision]
     rows = []
-    for name, flops, fill in ops:
+    for (name, flops, fill), (a_slots, b_slots, smem) in zip(ops, net.gemm_slots()):
         ms = best[name]
         rows.append({"name": name, "ms": ms, "flops": flops, "fill_bytes": fill,
-                     "issued_tflops": flops * per / (ms * 1e-3) / 1e12, "fill_gbs": fill / (ms * 1e-3) / 1e9})
+                     "issued_tflops": flops * per / (ms * 1e-3) / 1e12, "fill_gbs": fill / (ms * 1e-3) / 1e9,
+                     "a_slots": a_slots, "b_slots": b_slots, "smem_bytes": smem})
     forward_ms = sum(best.values())
     gemm_ms = sum(r["ms"] for r in rows)
     net.release_engine()
@@ -79,9 +81,10 @@ def main():
     print(f"card (name, power limit, SM clock, max SM clock): {r['card']}")
     print(f"{a.precision} res64 batch {a.batch}: forward {r['forward_ms']:.1f} ms, GEMM launches {r['gemm_ms']:.1f} ms "
           f"({len(r['ops'])} launches, {r['gemm_flops'] / 1e12:.1f} TFLOP, {r['gemm_fill_bytes'] / 1e9:.1f} GB filled)")
-    print(f"{'launch':<16}{'ms':>9}{'issued TFLOP/s':>16}{'fill GB/s':>11}")
+    print(f"{'launch':<16}{'ms':>9}{'issued TFLOP/s':>16}{'fill GB/s':>11}{'slots A/B':>11}")
     for o in sorted(r["ops"], key=lambda o: -o["ms"])[:10]:
-        print(f"{o['name']:<16}{o['ms']:>9.2f}{o['issued_tflops']:>16.1f}{o['fill_gbs']:>11.0f}")
+        slots = f"{o['a_slots']}/{o['b_slots']}"
+        print(f"{o['name']:<16}{o['ms']:>9.2f}{o['issued_tflops']:>16.1f}{o['fill_gbs']:>11.0f}{slots:>11}")
     if a.json:
         with open(a.json, "w") as f:
             json.dump(r, f, indent=1)
