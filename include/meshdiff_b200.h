@@ -45,7 +45,7 @@ typedef struct mdb_unet_config {
 
 int mdb_unet_create(const mdb_unet_config* cfg, mdb_unet** out);
 /* Plan only, no GPU needed: built by the same code as mdb_unet_create, so it answers the parameter table, arena size,
- * step and GEMM counts, mdb_unet_gemm_ops, mdb_unet_gemm_slots, FLOPs, mdb_unet_train_info and mdb_unet_grad_ready. It cannot run:
+ * step and GEMM counts, mdb_unet_gemm_ops, mdb_unet_gemm_slots, mdb_unet_gemm_tiles, FLOPs, mdb_unet_train_info and mdb_unet_grad_ready. It cannot run:
  * set/get_param, commit, forward, backward* and profile* return an error. */
 int mdb_unet_create_dry(const mdb_unet_config* cfg, mdb_unet** out);
 void mdb_unet_destroy(mdb_unet* net);
@@ -74,6 +74,10 @@ int mdb_unet_gemm_ops(mdb_unet* net, int i, const char** name, double* flops, do
 /* Operand ring depth of forward GEMM launch i: the A slots (entries in flight) and B slots (k-steps of weight tiles in
  * flight) it takes under the current MDB_MAX_STAGES / MDB_MAX_BSLOTS, and the dynamic shared memory it requests. */
 int mdb_unet_gemm_slots(mdb_unet* net, int i, int* a_slots, int* b_slots, int* smem_bytes);
+/* Tile shape of forward GEMM launch i at the engine's max batch: the work items its persistent CTAs share (output tiles
+ * times the split-K factor), the split-K factor, the k-steps of one output tile, the most k-steps of one load-table entry
+ * (3 or 5 for a halo convolution) and the tile width BLOCK_N. A launch runs on min(work items, SMs) CTAs. */
+int mdb_unet_gemm_tiles(mdb_unet* net, int i, int* work_items, int* splits, int* ksteps, int* entry_ksteps, int* block_n);
 /* One profiled forward: per-step device milliseconds. names_buf receives '\n'-separated step names. Synchronises. */
 int mdb_unet_profile(mdb_unet* net, const float* x, const float* labels, float* out, int batch, void* stream,
                      char* names_buf, int names_len, float* ms, int max_steps, int* n_steps);

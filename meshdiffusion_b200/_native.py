@@ -62,6 +62,8 @@ SIGNATURES = {
     "mdb_unet_info": (_i, [_vp, ctypes.POINTER(_d), ctypes.POINTER(_ll), ctypes.POINTER(_i), ctypes.POINTER(_i)]),
     "mdb_unet_gemm_ops": (_i, [_vp, _i, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(_d), ctypes.POINTER(_d)]),
     "mdb_unet_gemm_slots": (_i, [_vp, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i)]),
+    "mdb_unet_gemm_tiles": (_i, [_vp, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i),
+                                 ctypes.POINTER(_i)]),
     "mdb_unet_profile": (_i, [_vp, _vp, _vp, _vp, _i, _vp, ctypes.c_char_p, _i, ctypes.POINTER(_f), _i, ctypes.POINTER(_i)]),
     "mdb_unet_set_dropout": (_i, [_vp, _f, _u64]),
     "mdb_unet_backward": (_i, [_vp, _vp, _vp, _ll, _i, _i, _vp]),

@@ -1,5 +1,6 @@
 """In-tree build of the sm_90a shared library (no JIT cache: the .so must travel with the repo snapshot)."""
 import os
+import re
 import subprocess
 import sys
 
@@ -17,6 +18,27 @@ NVCC_FLAGS = ARCH_FLAGS + [
 # ptxas reports that make a wgmma kernel issue one MMA at a time (it waits for each to finish before the next): a build that
 # would silently lose the MMA pipelining fails instead
 SERIALISED_WGMMA = ("C7510", "C7520")
+# Kernels that must keep every value in registers. Their shared-memory rings leave L1 about 28 KB, so a stack frame (an
+# array indexed by a lane-dependent value, which ptxas does not count as a spill) or a spill goes to L2, on the
+# critical path of the epilogue or the MMA loop. No kernel here needs a stack.
+NO_STACK_KERNELS = ("gemm_tc_kernel", "wgrad_tc_kernel")
+_PROPS = re.compile(r"Function properties for (\S+)")
+_FRAME = re.compile(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads")
+
+
+def local_memory_violations(ptxas_report):
+    """Lines of a `-Xptxas -v` report where a NO_STACK_KERNELS function has a stack frame or spills."""
+    bad, fn = [], None
+    for line in ptxas_report.splitlines():
+        m = _PROPS.search(line)
+        if m:
+            fn = m.group(1)
+            continue
+        m = _FRAME.search(line)
+        if m and fn and any(k in fn for k in NO_STACK_KERNELS) and any(int(g) for g in m.groups()):
+            bad.append(f"{fn}: {line.strip()}")
+        fn = None
+    return bad
 
 
 def _newest_mtime(paths):
@@ -59,6 +81,9 @@ def _build_locked(force, verbose):
         serialised = [line for line in out.splitlines() if any(code in line for code in SERIALISED_WGMMA)]
         if serialised:
             raise RuntimeError("ptxas serialised wgmma in " + cmd[-3] + ":\n" + "\n".join(serialised))
+        local = local_memory_violations(out)
+        if local:
+            raise RuntimeError("local memory in a register-only kernel of " + cmd[-3] + ":\n" + "\n".join(local))
     cmd = [nvcc] + ARCH_FLAGS + ["-shared", "-o", LIB] + objs + ["-lcudart", "-ldl"]
     subprocess.check_call(cmd)
     return LIB

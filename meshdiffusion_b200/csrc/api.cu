@@ -130,6 +130,21 @@ int mdb_unet_gemm_slots(mdb_unet* n, int i, int* a_slots, int* b_slots, int* sme
   MDB_API_END
 }
 
+int mdb_unet_gemm_tiles(mdb_unet* n, int i, int* work_items, int* splits, int* ksteps, int* entry_ksteps, int* block_n) {
+  MDB_API_BEGIN
+  if (i < 0 || i >= n->net->num_gemm_launches()) throw std::runtime_error("mdb: GEMM launch index out of range");
+  const GemmOp& g = n->net->gemm(i);
+  const int s = g.p.splits > 1 ? g.p.splits : 1;
+  int nk = 0;
+  for (const LoadEntry& e : g.loads) nk = e.nk > nk ? e.nk : nk;
+  if (work_items) *work_items = g.p.tx * g.p.ty * g.p.tz * g.p.tb * g.p.n_tiles_n * s;
+  if (splits) *splits = s;
+  if (ksteps) *ksteps = g.ksteps;
+  if (entry_ksteps) *entry_ksteps = nk;
+  if (block_n) *block_n = g.block_n;
+  MDB_API_END
+}
+
 int mdb_unet_profile(mdb_unet* n, const float* x, const float* labels, float* out, int B, void* stream, char* names,
                      int names_len, float* ms, int max_steps, int* nsteps) {
   MDB_API_BEGIN

@@ -145,6 +145,27 @@ constexpr int kRegsProducer = 40, kRegsConsumer = 232;  // 128 x 40 + 256 x 232 
 // K-major 128B-swizzled operand at `saddr` (SBO = 1024 B)
 __device__ __forceinline__ uint64_t kdesc(uint32_t saddr) { return make_wgmma_desc(saddr, 16, 1024); }
 
+// Column sums over a warp's 32 rows, two quantities at once: butterfly transpose-reduce (31 shuffles per quantity); on
+// return lane i holds the sums of column i in s[0] / ss[0]. Level OFF halves the live columns [0, 2 OFF): a lane sends the
+// half its partner keeps and adds the received values to the half it keeps. The levels are template recursion so that
+// every array index is a compile-time constant and the lane select is a select between two registers: nvcc leaves an
+// inner loop bounded by an outer loop's OFF rolled, and its lane-dependent indices put both arrays in local memory
+// (build.py fails a build that gives this kernel a stack frame).
+template <int OFF>
+__device__ __forceinline__ void colsum_butterfly(float (&s)[32], float (&ss)[32], int lane) {
+  const bool hi = (lane & OFF) != 0;
+#pragma unroll
+  for (int i = 0; i < OFF; ++i) {
+    const float send_s = hi ? s[i] : s[i + OFF];
+    const float send_q = hi ? ss[i] : ss[i + OFF];
+    const float keep_s = hi ? s[i + OFF] : s[i];
+    const float keep_q = hi ? ss[i + OFF] : ss[i];
+    s[i] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, OFF);
+    ss[i] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, OFF);
+  }
+  if constexpr (OFF > 1) colsum_butterfly<OFF / 2>(s, ss, lane);
+}
+
 // GNB: GroupNorm-backward epilogue (see GemmParams::gnb_c) -- a separate instantiation, so the inference kernels'
 // code is untouched.
 // X3: split-bf16 operands (see Precision::kBF16X3): an entry loads the hi and lo parts of its A box, a k-step the W_hi and
@@ -601,27 +622,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
             }
           }
           if (GNB ? (want_cols != 0) : (p.stats != nullptr)) {  // (never reached in split-K mode)
-            // Column sums over the warp's 32 rows: butterfly transpose-reduce (31 shuffles per quantity);
-            // afterwards lane i holds the sum of column i.
             float s[32], ss[32];
 #pragma unroll
             for (int i = 0; i < 32; ++i) {
               const float t = valid ? v[i] : 0.f;
               s[i] = t; ss[i] = GNB ? q2[GNB ? i : 0] : t * t;
             }
-#pragma unroll
-            for (int off = 16; off >= 1; off >>= 1) {
-              const bool hi = (lane & off) != 0;
-#pragma unroll
-              for (int i = 0; i < off; ++i) {
-                const float send_s = hi ? s[i] : s[i + off];
-                const float send_q = hi ? ss[i] : ss[i + off];
-                const float keep_s = hi ? s[i + off] : s[i];
-                const float keep_q = hi ? ss[i + off] : ss[i];
-                s[i] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, off);
-                ss[i] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, off);
-              }
-            }
+            colsum_butterfly<16>(s, ss, lane);
             // per-warp slot, no atomics: the cross-warp sum below runs in a fixed order (deterministic results)
             s_part[(q * 2 + 0) * BLOCK_N + ch * 32 + lane] = s[0];
             s_part[(q * 2 + 1) * BLOCK_N + ch * 32 + lane] = ss[0];

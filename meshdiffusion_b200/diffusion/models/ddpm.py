@@ -580,6 +580,17 @@ class ScoreNet(nn.Module):
             rows.append((a.value, b.value, sm.value))
         return rows
 
+    def gemm_tiles(self):
+        """Per forward GEMM launch at the engine's batch: (work items, split-K factor, k-steps per output tile, most k-steps
+        of one load-table entry, BLOCK_N)."""
+        L = _native.lib()
+        rows = []
+        for i in range(self.engine_info()["gemm_launches"]):
+            v = [ctypes.c_int() for _ in range(5)]
+            _native.check(L.mdb_unet_gemm_tiles(self._handle, i, *[ctypes.byref(x) for x in v]))
+            rows.append(tuple(x.value for x in v))
+        return rows
+
     def profile(self, x, labels):
         """One profiled forward: [(step name, device ms)]."""
         L = _native.lib()
