@@ -8,6 +8,7 @@
 #include <cmath>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 namespace mdb {
 
@@ -17,7 +18,9 @@ namespace mdb {
 // dropped lo*lo term is 2^-16 relative) -- fp32-class results (the mode that meets the 1e-3 parity contract) at
 // one third of the bf16 tensor rate. An X3 tensor with a logical row pitch of `ld` channels occupies 2*ld bf16 per
 // voxel: hi parts at [0, ld), lo parts at [ld, 2*ld). All pitches handed to GemmOp / Act and to the launchers stay
-// LOGICAL. kTF32 tensors are fp32, rounded to tf32 (rna) wherever a kernel stores an operand.
+// LOGICAL. kTF32 tensors are fp32, rounded to tf32 (rna) wherever a kernel stores an operand: tensor cores truncate fp32
+// inputs to 10 mantissa bits, and rounding to nearest instead removes that systematic bias (full res64 net: rel-L2 vs
+// fp32 2.5e-3 -> 1.5e-3).
 enum Precision { kBF16 = 0, kTF32 = 1, kBF16X3 = 2 };
 constexpr int esize(Precision p) { return p == kTF32 ? 4 : 2; }
 constexpr int parts(Precision p) { return p == kBF16X3 ? 2 : 1; }
@@ -31,14 +34,29 @@ __device__ __forceinline__ float to_tf32_rna(float x) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
   return __uint_as_float(u);
 }
-// lo part of a split-bf16 value whose hi part is `hi`: what the bf16 rounding of v lost
-__device__ __forceinline__ __nv_bfloat16 bf16_lo(float v, __nv_bfloat16 hi) { return __float2bfloat16(v - __bfloat162float(hi)); }
-// scalar store in the activation format of bf16 (lo_off unused) or split bf16 (lo part lo_off elements behind)
+// element type of an activation tensor in mode P
+template <Precision P> using ActElem = std::conditional_t<P == kTF32, float, __nv_bfloat16>;
+// scalar load / store in the activation format of mode P: tf32 (rounded on store) and bf16 ignore lo_off, split bf16 has
+// its lo part lo_off elements behind the hi part
 template <Precision P>
-__device__ __forceinline__ void store_split(__nv_bfloat16* hi, long long lo_off, float v) {
-  const __nv_bfloat16 hb = __float2bfloat16(v);
-  hi[0] = hb;
-  if constexpr (P == kBF16X3) hi[lo_off] = bf16_lo(v, hb);
+__device__ __forceinline__ float load_split(const ActElem<P>* hi, long long lo_off) {
+  if constexpr (P == kTF32) {
+    return hi[0];
+  } else {
+    float x = __bfloat162float(hi[0]);
+    if constexpr (P == kBF16X3) x += __bfloat162float(hi[lo_off]);
+    return x;
+  }
+}
+template <Precision P>
+__device__ __forceinline__ void store_split(ActElem<P>* hi, long long lo_off, float v) {
+  if constexpr (P == kTF32) {
+    hi[0] = to_tf32_rna(v);
+  } else {
+    const __nv_bfloat16 hb = __float2bfloat16(v);
+    hi[0] = hb;
+    if constexpr (P == kBF16X3) hi[lo_off] = __float2bfloat16(v - __bfloat162float(hb));  // what the bf16 rounding lost
+  }
 }
 
 // 8 bf16 in a 16-byte vector

@@ -367,7 +367,7 @@ int mdb_conv3d_backward_prec(const void* dy, const void* x, const float* w, int 
   Act ax; ax.ptr = const_cast<void*>(x); ax.C = cin; ax.X = x_; ax.Y = y_; ax.Z = z; ax.B = B;
   if (dw) {
     const int T = ksize * ksize * ksize;
-    const WgradPlan pl = plan_wgrad(xo, yo, zo, B, cout, cin, ksize, stride, pr == kBF16X3);
+    const WgradPlan pl = plan_wgrad(xo, yo, zo, B, cout, cin, ksize, stride, pr);
     float* scratch = nullptr;
     MDB_CUDA_CHECK(cudaMalloc(&scratch, pl.scratch_bytes));
     WgradOut o; o.ptr = dw; o.sm = (long long)cin * T; o.sn = T; o.st = 1;

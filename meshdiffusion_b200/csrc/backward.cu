@@ -593,7 +593,6 @@ void launch_rowsum_nc(const float* t, float* out, int B, int C, long long V, int
 // ------------------------------------------------------------------ attention softmax backward (layers.py:604)
 template <Precision PR>
 __global__ void __launch_bounds__(256) softmax_bwd_rows_kernel(const float* __restrict__ P, float* __restrict__ dP, long long rows, int L) {
-  constexpr bool X3 = PR == kBF16X3;
   __shared__ float red[8];
   for (long long row = blockIdx.x; row < rows; row += gridDim.x) {
     const __nv_bfloat16* p = reinterpret_cast<const __nv_bfloat16*>(P + row * L);
@@ -603,7 +602,7 @@ __global__ void __launch_bounds__(256) softmax_bwd_rows_kernel(const float* __re
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       const int i = threadIdx.x + j * 256;
-      pv[j] = i < L ? __bfloat162float(p[i]) + (X3 ? __bfloat162float(p[L + i]) : 0.f) : 0.f;
+      pv[j] = i < L ? load_split<PR>(p + i, L) : 0.f;
       dv[j] = i < L ? d[i] : 0.f;
       dot = fmaf(pv[j], dv[j], dot);
     }

@@ -223,8 +223,7 @@ __global__ void softmax_rows_kernel(float* __restrict__ s, long long rows, int L
     for (int j = 0; j < 16; ++j) {
       const int i = threadIdx.x + j * 256;
       if (i < L) {
-        if constexpr (P == kTF32) p[i] = to_tf32_rna(vals[j] * inv);
-        else store_split<P>((__nv_bfloat16*)p + i, L, vals[j] * inv);
+        store_split<P>(reinterpret_cast<ActElem<P>*>(p) + i, L, vals[j] * inv);
       }
     }
   }
@@ -401,7 +400,6 @@ void launch_tap_shift_sum(const void* P, long long ldp, int p_fp32, const float*
 // integer atomic per (block, channel).
 template <Precision P>  // split bf16: out / res rows are [N hi | N lo]
 __global__ void __launch_bounds__(256) split_reduce_kernel(SplitReduceArgs a, int vchunk) {
-  constexpr bool TF32 = P == kTF32;
   const int b = blockIdx.y;
   const long long v0 = (long long)blockIdx.x * vchunk;
   const long long v1 = v0 + vchunk < a.voxels ? v0 + vchunk : a.voxels;
@@ -413,18 +411,10 @@ __global__ void __launch_bounds__(256) split_reduce_kernel(SplitReduceArgs a, in
       const long long idx = ((long long)b * a.voxels + v) * a.N + n;
       float acc = add;
       for (int sp = 0; sp < a.splits; ++sp) acc += a.partial[sp * a.split_stride + idx];
-      if (a.res) {
-        const long long ridx = (long long)b * a.res_batch_stride + v * a.N + n;
-        if constexpr (P == kBF16X3) {
-          const __nv_bfloat16* rp = (const __nv_bfloat16*)a.res + 2 * ((long long)b * a.res_batch_stride + v * a.N) + n;
-          acc += __bfloat162float(rp[0]) + __bfloat162float(rp[a.N]);
-        } else {
-          acc += TF32 ? ((const float*)a.res)[ridx] : __bfloat162float(((const __nv_bfloat16*)a.res)[ridx]);
-        }
-      }
+      if (a.res)
+        acc += load_split<P>((const ActElem<P>*)a.res + parts(P) * ((long long)b * a.res_batch_stride + v * a.N) + n, a.N);
       s1 += acc; s2 += acc * acc;
-      if constexpr (TF32) ((float*)a.out)[idx] = to_tf32_rna(acc);
-      else store_split<P>((__nv_bfloat16*)a.out + parts(P) * (idx - n) + n, a.N, acc);
+      store_split<P>((ActElem<P>*)a.out + parts(P) * (idx - n) + n, a.N, acc);
     }
     if (a.stats) {
       long long* dst = a.stats + ((long long)b * a.N + n) * kStatWords;

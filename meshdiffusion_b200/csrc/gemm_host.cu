@@ -26,24 +26,57 @@ static PFN_encodeTiled get_encode() {
   return fn;
 }
 
-void encode_map(CUtensorMap* m, Precision prec, int rank, void* base, const uint64_t* dims,
-                const uint64_t* strides_bytes /*rank-1*/, const uint32_t* box) {
+void encode_map(CUtensorMap* m, Precision prec, const MapDesc& d) {
   cuuint64_t gd[5], gs[4];
   cuuint32_t bd[5], es[5];
-  for (int i = 0; i < rank; ++i) { gd[i] = dims[i]; bd[i] = box[i]; es[i] = 1; }
-  for (int i = 0; i + 1 < rank; ++i) gs[i] = strides_bytes[i];
+  for (int i = 0; i < d.rank; ++i) { gd[i] = d.dims[i]; bd[i] = d.box[i]; es[i] = 1; }
+  for (int i = 0; i + 1 < d.rank; ++i) gs[i] = d.strides[i];
   CUtensorMapDataType dt = prec == kTF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  CUresult r = get_encode()(m, dt, rank, base, gd, gs, bd, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = get_encode()(m, dt, d.rank, d.base, gd, gs, bd, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     std::string msg = "mdb: cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ") rank " +
-                      std::to_string(rank) + " dims";
-    for (int i = 0; i < rank; ++i) msg += " " + std::to_string(dims[i]);
+                      std::to_string(d.rank) + " dims";
+    for (int i = 0; i < d.rank; ++i) msg += " " + std::to_string(d.dims[i]);
     msg += " box";
-    for (int i = 0; i < rank; ++i) msg += " " + std::to_string(box[i]);
+    for (int i = 0; i < d.rank; ++i) msg += " " + std::to_string(d.box[i]);
     throw std::runtime_error(msg);
   }
+}
+
+// ------------------------------------------------------------------ kernel instantiations
+template <int BN, Precision P, bool GNB>
+static void launch_impl(const GemmParams& p, int grid, int smem, cudaStream_t stream) {
+  static bool configured[64] = {};  // the attribute is per device
+  auto kern = gemm_tc_kernel<BN, P, GNB>;
+  int dev = 0;
+  MDB_CUDA_CHECK(cudaGetDevice(&dev));
+  if (dev >= 64 || !configured[dev]) {
+    MDB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+    if (dev < 64) configured[dev] = true;
+  }
+  kern<<<grid, kGemmThreads, smem, stream>>>(p);
+  MDB_CUDA_CHECK(cudaGetLastError());
+}
+
+struct GemmVariant {
+  void (*launch)(const GemmParams&, int grid, int smem, cudaStream_t);
+  int fixed_bytes;  // GemmCfg::kFixedBytes: the shared memory next to the operand rings
+};
+template <int BN, Precision P, bool GNB>
+static GemmVariant variant() { return {launch_impl<BN, P, GNB>, GemmCfg<BN, GNB>::kFixedBytes}; }
+template <int BN>
+static GemmVariant variant(Precision prec, bool gnb) {
+  if (gnb) {
+    if (prec == kTF32) throw std::runtime_error("mdb: the GroupNorm-backward epilogue is built for bf16 / split-bf16 operands");
+    return prec == kBF16X3 ? variant<BN, kBF16X3, true>() : variant<BN, kBF16, true>();
+  }
+  return prec == kTF32 ? variant<BN, kTF32, false>() : prec == kBF16X3 ? variant<BN, kBF16X3, false>() : variant<BN, kBF16, false>();
+}
+// the one choice of kernel instantiation for (BLOCK_N, operand mode, GroupNorm-backward epilogue)
+static GemmVariant gemm_variant(int block_n, Precision prec, bool gnb) {
+  return block_n == 32 ? variant<32>(prec, gnb) : variant<128>(prec, gnb);
 }
 
 int GemmOp::pick_slots(GemmParams& q) const {
@@ -51,7 +84,7 @@ int GemmOp::pick_slots(GemmParams& q) const {
   // filling while one is read). Then B slots are added until they cover the k-steps of every A slot in flight, and A slots
   // (entries in flight) up to MDB_MAX_STAGES (default 4), whichever is behind and still fits. MDB_MAX_BSLOTS caps the B
   // slots (weight lookahead) the same way; both change timing only, never results.
-  const int fixed = block_n == 32 ? GemmCfg<32>::kFixedBytes : gnb ? GemmCfg<128, true>::kFixedBytes : GemmCfg<128>::kFixedBytes;
+  const int fixed = gemm_variant(block_n, prec, gnb).fixed_bytes;
   const int budget = kMaxDynSmem - fixed;
   q.a_slot_bytes = (a_slot_need + 1023) / 1024 * 1024;
   q.b_slot_bytes = parts(prec) * block_n * kRowBytes;
@@ -144,6 +177,14 @@ GemmOp::~GemmOp() {
   if (d_wpacked && owns_w) cudaFree(d_wpacked);
 }
 
+// Logical element strides (sx, sy, sz, sb) of an epilogue tensor -> physical ones; returns the offset of the lo parts.
+// Split-bf16 rows are (hi, lo) pairs: physical pitches twice the logical ones, lo parts lo_off (logical) elements behind.
+static long long physical_strides(bool split, long long lo_off, long long& sx, long long& sy, long long& sz, long long& sb) {
+  if (!split) return 0;
+  sx *= 2; sy *= 2; sz *= 2; sb *= 2;
+  return lo_off;
+}
+
 void GemmOp::set_output_strided(Precision pr, int X, int Y, int Z, int B, int N, void* out, long long osx,
                                 long long osy, long long osz, long long osb, bool out_fp32, long long lo_off) {
   prec = pr;
@@ -162,18 +203,7 @@ void GemmOp::set_output_strided(Precision pr, int X, int Y, int Z, int B, int N,
   p.out = out;
   p.osx = osx; p.osy = osy; p.osz = osz; p.osb = osb;
   p.out_fp32 = out_fp32 ? 1 : 0;
-  p.out_lo_off = 0;
-  if (prec == kBF16X3 && !out_fp32) {  // (hi, lo) rows: physical pitch 2x the logical one, lo parts one logical row behind
-    p.out_lo_off = lo_off >= 0 ? lo_off : osx;
-    p.osx *= 2; p.osy *= 2; p.osz *= 2; p.osb *= 2;
-  }
-  {
-    // TF32 operands: tensor cores truncate fp32 inputs to 10 mantissa bits; rounding the stored activations to
-    // nearest instead removes that systematic bias (measured on the full res64 net: rel-L2 vs fp32 2.5e-3 -> 1.5e-3,
-    // on par with stock cuDNN/cuBLAS TF32). MDB_TF32_ROUND_STORE=0 restores plain fp32 stores.
-    const char* e = getenv("MDB_TF32_ROUND_STORE");
-    p.round_out = (prec == kTF32 && !out_fp32 && !(e && e[0] == '0')) ? 1 : 0;
-  }
+  p.out_lo_off = physical_strides(prec == kBF16X3 && !out_fp32, lo_off >= 0 ? lo_off : osx, p.osx, p.osy, p.osz, p.osb);
   p.alpha = 1.f;
   p.ocs = 1;
   p.kb_elems = kb_elems(prec);
@@ -183,28 +213,23 @@ void GemmOp::set_output(Precision pr, int X, int Y, int Z, int B, int N, void* o
   set_output_strided(pr, X, Y, Z, B, N, out, ldc, ldc * X, ldc * X * Y, ldc * X * Y * Z, out_fp32);
 }
 
+MapDesc act_map(const Act& a, Precision prec, int part, Geometry box, int sub, int px, int py, int pz) {
+  const long long es = esize(prec);
+  const long long sx = a.row() * parts(prec) * es, sy = sx * a.X, sz = sy * a.Y, sb = sz * a.Z;  // physical, bytes
+  MapDesc m;
+  m.rank = 5;
+  m.base = static_cast<char*>(a.ptr) + (long long)part * a.row() * es + px * sx + py * sy + pz * sz;
+  m.dims[0] = a.C; m.dims[1] = (a.X - px + sub - 1) / sub; m.dims[2] = (a.Y - py + sub - 1) / sub;
+  m.dims[3] = (a.Z - pz + sub - 1) / sub; m.dims[4] = a.B;
+  m.strides[0] = sx * sub; m.strides[1] = sy * sub; m.strides[2] = sz * sub; m.strides[3] = sb;
+  m.box[0] = kb_elems(prec); m.box[1] = box.bx; m.box[2] = box.by; m.box[3] = box.bz; m.box[4] = box.bb;
+  return m;
+}
+
 int GemmOp::add_amap(const Act& a, int halo, int sub, int px, int py, int pz, int part) {
   if ((int)amaps_.size() >= kMaxAMaps) throw std::runtime_error("mdb: too many A tensor maps");
   if (halo > 0 && (geo.bz != 1 || geo.bb != 1)) throw std::runtime_error("mdb: halo needs a (bx,by,1,1) tile");
-  const long long es = esize(prec);
-  const long long prow = a.row() * parts(prec);  // physical row pitch in elements
-  MapDesc m;
-  m.rank = 5;
-  uint64_t* dims = m.dims; uint64_t* strides = m.strides; uint32_t* box = m.box;
-  char* base = static_cast<char*>(a.ptr) + (long long)part * a.row() * es;
-  if (sub == 1) {
-    dims[0] = a.C; dims[1] = a.X; dims[2] = a.Y; dims[3] = a.Z; dims[4] = a.B;
-    strides[0] = prow * es; strides[1] = strides[0] * a.X; strides[2] = strides[1] * a.Y; strides[3] = strides[2] * a.Z;
-  } else {
-    dims[0] = a.C; dims[1] = (a.X - px + sub - 1) / sub; dims[2] = (a.Y - py + sub - 1) / sub;
-    dims[3] = (a.Z - pz + sub - 1) / sub; dims[4] = a.B;
-    const long long sx = prow * es, sy = sx * a.X, sz = sy * a.Y, sb = sz * a.Z;
-    strides[0] = sx * sub; strides[1] = sy * sub; strides[2] = sz * sub; strides[3] = sb;
-    base += px * sx + py * sy + pz * sz;
-  }
-  box[0] = kb_elems(prec); box[1] = geo.bx; box[2] = geo.by + halo; box[3] = geo.bz; box[4] = geo.bb;
-  m.base = base;
-  amaps_.push_back(m);
+  amaps_.push_back(act_map(a, prec, part, {geo.bx, geo.by + halo, geo.bz, geo.bb}, sub, px, py, pz));
   return (int)amaps_.size() - 1;
 }
 
@@ -338,11 +363,7 @@ void GemmOp::set_residual(const void* res, long long ldr, long long batch_stride
   p.batch_fastest = batch_stride == 0 ? 1 : 0;  // a residual shared by every sample: keep its slice L2-resident
   p.rsx = ldr; p.rsy = ldr * p.X; p.rsz = ldr * p.X * p.Y; p.rsb = batch_stride;
   p.res_fp32 = fp32 ? 1 : 0;
-  p.res_lo_off = 0;
-  if (prec == kBF16X3 && !fp32) {
-    p.res_lo_off = ldr;
-    p.rsx *= 2; p.rsy *= 2; p.rsz *= 2; p.rsb *= 2;
-  }
+  p.res_lo_off = physical_strides(prec == kBF16X3 && !fp32, ldr, p.rsx, p.rsy, p.rsz, p.rsb);
 }
 
 void GemmOp::set_gn_backward(const void* x0, long long ld0, int c0, const void* x1, long long ld1, const void* consts, int silu,
@@ -356,12 +377,8 @@ void GemmOp::set_gn_backward(const void* x0, long long ld0, int c0, const void* 
   p.rsx = ld0; p.rsy = ld0 * p.X; p.rsz = ld0 * p.X * p.Y; p.rsb = ld0 * p.X * p.Y * p.Z;
   p.res1 = x1; p.res_c0 = ld1 > 0 ? c0 : p.N;
   p.r1sx = ld1; p.r1sy = ld1 * p.X; p.r1sz = ld1 * p.X * p.Y; p.r1sb = ld1 * p.X * p.Y * p.Z;
-  p.res_lo_off = 0; p.res1_lo_off = 0;
-  if (prec == kBF16X3) {  // (hi, lo) rows: physical pitches twice the logical ones, lo parts one logical row behind
-    p.res_lo_off = ld0; p.res1_lo_off = ld1;
-    p.rsx *= 2; p.rsy *= 2; p.rsz *= 2; p.rsb *= 2;
-    p.r1sx *= 2; p.r1sy *= 2; p.r1sz *= 2; p.r1sb *= 2;
-  }
+  p.res_lo_off = physical_strides(prec == kBF16X3, ld0, p.rsx, p.rsy, p.rsz, p.rsb);
+  p.res1_lo_off = physical_strides(prec == kBF16X3, ld1, p.r1sx, p.r1sy, p.r1sz, p.r1sb);
   p.gnb_c = reinterpret_cast<const float4*>(consts);
   p.gnb_silu = silu;
   p.gnb_part = part;
@@ -423,30 +440,16 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const LoadEntry* __re
       if (c < w.cvalid) valid |= 1u << i;
       coff[i] = noff + (w.cdiv ? (long long)(c % w.cdiv) * w.sc + (long long)(c / w.cdiv) * w.sc_hi : (long long)c * w.sc);
     }
-    constexpr int kParts = P == kBF16X3 ? 2 : 1;
-    const long long obase = ((long long)n * ksteps + load_ks0[l]) * kParts * KB + v8 * 8;
+    const long long obase = ((long long)n * ksteps + load_ks0[l]) * parts(P) * KB + v8 * 8;
     for (int j = 0; j < e.nk; ++j) {
       const long long toff = (long long)(e.tap0 + j * e.tapj) * w.st;
       float v[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = (valid >> i) & 1u ? __ldg(w.ptr + coff[i] + toff) : 0.f;
-      const long long o = obase + (long long)j * kParts * KB;
-      if (P == kTF32) {
-        float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + o);
-        op[0] = make_float4(to_tf32_rna(v[0]), to_tf32_rna(v[1]), to_tf32_rna(v[2]), to_tf32_rna(v[3]));
-        op[1] = make_float4(to_tf32_rna(v[4]), to_tf32_rna(v[5]), to_tf32_rna(v[6]), to_tf32_rna(v[7]));
-      } else {
-        uint4 pk, pl;
-        __nv_bfloat16* h = reinterpret_cast<__nv_bfloat16*>(&pk);
-        __nv_bfloat16* lo = reinterpret_cast<__nv_bfloat16*>(&pl);
+      ActElem<P>* op = reinterpret_cast<ActElem<P>*>(out) + obase + (long long)j * parts(P) * KB;
+      constexpr int E = kVecElems<P>;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          h[i] = __float2bfloat16(v[i]);
-          if (P == kBF16X3) lo[i] = bf16_lo(v[i], h[i]);
-        }
-        *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(out) + o) = pk;
-        if (P == kBF16X3) *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(out) + o + KB) = pl;
-      }
+      for (int i = 0; i < 8 / E; ++i) store_vec<P>(op + E * i, (long long)KB * sizeof(ActElem<P>), v + E * i);
     }
   }
 }
@@ -522,10 +525,7 @@ void GemmOp::finalize() {
 }
 
 void GemmOp::upload(cudaStream_t stream) {
-  for (size_t i = 0; i < amaps_.size(); ++i) {
-    const MapDesc& m = amaps_[i];
-    encode_map(&p.amap[i], prec, m.rank, m.base, m.dims, m.strides, m.box);
-  }
+  for (size_t i = 0; i < amaps_.size(); ++i) encode_map(&p.amap[i], prec, amaps_[i]);
   MDB_CUDA_CHECK(cudaMalloc(&d_loads, loads.size() * sizeof(LoadEntry)));
   MDB_CUDA_CHECK(cudaMemcpyAsync(d_loads, loads.data(), loads.size() * sizeof(LoadEntry), cudaMemcpyHostToDevice, stream));
   p.loads = d_loads;
@@ -536,22 +536,8 @@ void GemmOp::upload(cudaStream_t stream) {
     owns_w = true;
     bmap_ = b_desc(d_wpacked, ktot, p.N, 1, ktot * esize(prec), bytes);
   }
-  encode_map(&p.bmap, prec, bmap_.rank, bmap_.base, bmap_.dims, bmap_.strides, bmap_.box);
+  encode_map(&p.bmap, prec, bmap_);
   MDB_CUDA_CHECK(cudaStreamSynchronize(stream));
-}
-
-template <int BN, bool TF32, bool GNB = false, bool X3 = false>
-static void launch_impl(const GemmParams& p, int grid, int smem, cudaStream_t stream) {
-  static bool configured[64] = {};  // the attribute is per device
-  auto kern = gemm_tc_kernel<BN, TF32, GNB, X3>;
-  int dev = 0;
-  MDB_CUDA_CHECK(cudaGetDevice(&dev));
-  if (dev >= 64 || !configured[dev]) {
-    MDB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    if (dev < 64) configured[dev] = true;
-  }
-  kern<<<grid, kGemmThreads, smem, stream>>>(p);
-  MDB_CUDA_CHECK(cudaGetLastError());
 }
 
 void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
@@ -564,36 +550,20 @@ void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
   }
   if (out_override) p.out = out_override;
   const int tiles_m = p.tx * p.ty * p.tz * p.tb;
-  const bool tf = prec == kTF32;
   const int total = tiles_m * p.n_tiles_n * (p.splits > 1 ? p.splits : 1);
   const int grid = total < sm_count() ? total : sm_count();
   if (gnb) {
-    if (tf || p.splits > 1) throw std::runtime_error("mdb: GroupNorm-backward epilogue: bf16 or split bf16, no split-K");
+    if (p.splits > 1) throw std::runtime_error("mdb: GroupNorm-backward epilogue: no split-K");
     p.gnb_drop_thresh = rt_drop_thresh; p.gnb_drop_scale = rt_drop_scale; p.gnb_seed = rt_seed;
-    if (prec == kBF16X3) {
-      if (block_n == 32) launch_impl<32, false, true, true>(p, grid, smem, stream); else launch_impl<128, false, true, true>(p, grid, smem, stream);
-    } else {
-      if (block_n == 32) launch_impl<32, false, true>(p, grid, smem, stream); else launch_impl<128, false, true>(p, grid, smem, stream);
-    }
-    return;
   }
-  const bool x3 = prec == kBF16X3;
-  if (block_n == 32) {
-    if (tf) launch_impl<32, true>(p, grid, smem, stream);
-    else if (x3) launch_impl<32, false, false, true>(p, grid, smem, stream);
-    else launch_impl<32, false>(p, grid, smem, stream);
-  } else {
-    if (tf) launch_impl<128, true>(p, grid, smem, stream);
-    else if (x3) launch_impl<128, false, false, true>(p, grid, smem, stream);
-    else launch_impl<128, false>(p, grid, smem, stream);
-  }
+  gemm_variant(block_n, prec, gnb).launch(p, grid, smem, stream);
   if (p.splits > 1) {
     SplitReduceArgs a{};
     a.partial = p.partial; a.split_stride = p.split_stride; a.splits = p.splits;
     a.bias = p.bias; a.rowbias = p.rowbias; a.rowbias_ld = p.rowbias_ld;
     a.res = p.res; a.res_batch_stride = p.rsb;
     a.out = p.out; a.stats = p.stats; a.voxels = (long long)p.X * p.Y * p.Z; a.N = p.N; a.prec = prec;
-    if (x3) a.res_batch_stride = p.rsb / 2;  // the reduction kernel takes logical strides
+    if (prec == kBF16X3) a.res_batch_stride = p.rsb / 2;  // the reduction kernel takes logical strides
     launch_split_reduce(a, p.Bn, stream);
   }
 }

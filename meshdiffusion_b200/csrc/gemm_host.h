@@ -48,13 +48,17 @@ struct WSrc {
 struct Geometry { int bx, by, bz, bb; };
 Geometry pick_geometry(int X, int Y, int Z);
 
-// A TMA tensor map as described on the host (encode_map's arguments), encoded by GemmOp::upload
+// A TMA tensor map as described on the host (encode_map's arguments)
 struct MapDesc {
   void* base = nullptr;
   int rank = 0;
   uint64_t dims[5] = {}, strides[4] = {};  // strides in bytes, rank - 1 of them
   uint32_t box[5] = {};
 };
+// The 5-D map (channel, x, y, z, batch) over activation `a` in mode `prec`, with a box of one k-step of channels by `box`
+// voxels. part: 0 = the tensor itself / the hi parts of a split-bf16 tensor, 1 = its lo parts (one logical row in).
+// sub = 2: only the parity-(px, py, pz) sub-grid of a stride-2 access.
+MapDesc act_map(const Act& a, Precision prec, int part, Geometry box, int sub = 1, int px = 0, int py = 0, int pz = 0);
 
 // Built in three steps: the add_* / set_* calls and finalize() describe the op on the host (no GPU needed: flops,
 // fill_bytes and the launch geometry are then known); upload() encodes the tensor maps and allocates the device tables;
@@ -166,8 +170,7 @@ int sm_count();
 // SMs the split-K plans and grid caps are sized for (the H100 SXM's 132). A constant (not the device query) so that the
 // GPU-less sizing pass and the real pass agree on every scratch size.
 constexpr int kPlanSMs = 132;
-void encode_map(CUtensorMap* m, Precision prec, int rank, void* base, const uint64_t* dims,
-                const uint64_t* strides_bytes /*rank-1*/, const uint32_t* box);
+void encode_map(CUtensorMap* m, Precision prec, const MapDesc& d);
 // Split-K factor for a conv-like op (pure function of the shapes, so the dry planning pass and the real pass agree).
 int plan_splits(int X, int Y, int Z, int B, int N, int cin_total, int taps, Precision prec);
 

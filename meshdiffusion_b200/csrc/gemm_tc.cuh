@@ -95,8 +95,7 @@ struct GemmParams {
   void* out;
   long long osx, osy, osz, osb;  // output element strides per voxel axis
   long long ocs;                 // output column stride (1 = channels contiguous; else scalar store path)
-  int out_fp32;
-  int round_out;  // TF32 operands: round stored activations to tf32 (rna) so downstream MMAs do not truncate them
+  int out_fp32;  // plain fp32 output (attention logits, head projection, stem field); else the activation format
   const float* bias;
   int bias_on_m;
   const float* rowbias;  // [Bn][rowbias_ld] per-sample bias (time embedding projection) or null
@@ -166,18 +165,32 @@ __device__ __forceinline__ void colsum_butterfly(float (&s)[32], float (&ss)[32]
   if constexpr (OFF > 1) colsum_butterfly<OFF / 2>(s, ss, lane);
 }
 
+// v[0, 32) += the residual chunk prefetched as 16-byte vectors in mode P (split bf16: hi vectors in buf[0, 4), lo in [4, 8))
+template <Precision P>
+__device__ __forceinline__ void add_res_chunk(const uint4 (&buf)[8], float (&v)[32]) {
+  constexpr int E = kVecElems<P>, NV = 32 / E;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    float r[E];
+    decode_vec<P>(buf[i], buf[P == kBF16X3 ? NV + i : i], r);
+#pragma unroll
+    for (int j = 0; j < E; ++j) v[E * i + j] += r[j];
+  }
+}
+
+// P: the operand mode (act_format.cuh); the epilogue reads residuals and stores outputs in its row format.
 // GNB: GroupNorm-backward epilogue (see GemmParams::gnb_c) -- a separate instantiation, so the inference kernels'
 // code is untouched.
-// X3: split-bf16 operands (see Precision::kBF16X3): an entry loads the hi and lo parts of its A box, a k-step the W_hi and
-// W_lo tiles. Per k16 step, A_hi . [W_hi; W_lo] is one m64n(2 BLOCK_N) wgmma into acc[0, BLOCK_N) (first half: the W_hi
-// columns, second half: W_lo), then A_lo . W_hi an m64nBLOCK_N one into acc[0, BLOCK_N / 2); after the last k-step the
-// second half is folded into the first. The epilogue reads residuals and stores outputs as (hi, lo) bf16 pairs. GNB && X3 reads
-// the GroupNorm input as hi + lo, stores dy as (hi, lo) and takes the SiLU derivative from ex2/rcp (tanh.approx's 2^-11
-// would cap the gradient accuracy near 5e-4).
-template <int BLOCK_N, bool TF32, bool GNB = false, bool X3 = false>
+// kBF16X3 (split bf16): an entry loads the hi and lo parts of its A box, a k-step the W_hi and W_lo tiles. Per k16 step,
+// A_hi . [W_hi; W_lo] is one m64n(2 BLOCK_N) wgmma into acc[0, BLOCK_N) (first half: the W_hi columns, second half: W_lo),
+// then A_lo . W_hi an m64nBLOCK_N one into acc[0, BLOCK_N / 2); after the last k-step the second half is folded into the
+// first. GNB with kBF16X3 reads the GroupNorm input as hi + lo, stores dy as (hi, lo) and takes the SiLU derivative from
+// ex2/rcp (tanh.approx's 2^-11 would cap the gradient accuracy near 5e-4).
+template <int BLOCK_N, Precision P, bool GNB>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
+  static_assert(!(GNB && P == kTF32), "the GroupNorm-backward epilogue is built for bf16 / split-bf16 operands");
   using Cfg = GemmCfg<BLOCK_N, GNB>;
-  constexpr int kParts = X3 ? 2 : 1;  // operand parts per A box / per k-step of weights
+  constexpr int kParts = parts(P);  // operand parts per A box / per k-step of weights
   const int NA = p.n_aslots, NB = p.n_bslots;
   const uint32_t a_slot = (uint32_t)p.a_slot_bytes, b_slot = (uint32_t)p.b_slot_bytes;
   extern __shared__ uint8_t smem_raw[];
@@ -261,18 +274,18 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
               const uint32_t abase = a_ring + as * a_slot, bar = a_full + 8 * as;
               mbar_expect_tx(bar, kParts * seg.a_bytes);
               tma_load_5d(&p.amap[en.tmap], bar, abase, en.c0, x0 + en.dx, y0 + en.dy, z0 + en.dz, b0);
-              if constexpr (X3) tma_load_5d(&p.amap[en.tmap_lo], bar, abase + seg.a_stride, en.c0, x0 + en.dx, y0 + en.dy, z0 + en.dz, b0);
+              if constexpr (P == kBF16X3) tma_load_5d(&p.amap[en.tmap_lo], bar, abase + seg.a_stride, en.c0, x0 + en.dx, y0 + en.dy, z0 + en.dz, b0);
             }
             __syncwarp();
             if (++as == (uint32_t)NA) { as = 0; aph ^= 1; }
-            int kc = (X3 && p.b_explicit_k) ? (int)en.wc0 : kcol;
+            int kc = (P == kBF16X3 && p.b_explicit_k) ? (int)en.wc0 : kcol;
             for (int j = 0; j < seg.nk; ++j) {
               mbar_wait(b_empty + 8 * bs, bph ^ 1);
               if (elect_one()) {
                 const uint32_t bbase = b_ring + bs * b_slot, bar = b_full + 8 * bs;
                 mbar_expect_tx(bar, kParts * Cfg::kBTileBytes);
                 tma_load_3d(&p.bmap, bar, bbase, kc, n0, bcoord);
-                if constexpr (X3) tma_load_3d(&p.bmap, bar, bbase + Cfg::kBTileBytes, kc + p.b_lo_k, n0, bcoord);
+                if constexpr (P == kBF16X3) tma_load_3d(&p.bmap, bar, bbase + Cfg::kBTileBytes, kc + p.b_lo_k, n0, bcoord);
               }
               __syncwarp();
               kc += p.b_kstep;
@@ -311,7 +324,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
     for (int tile = first_tile; tile < total_tiles; tile += tile_step, ++it) {
       const int vit = it;
       // ---------------------------------------------------------------- main loop: wgmma over the k-step groups
-      constexpr int kAccRegs = X3 ? BLOCK_N : BLOCK_N / 2;  // X3: [W_hi columns | W_lo columns] until the fold
+      constexpr int kAccRegs = kParts * BLOCK_N / 2;  // split bf16: [W_hi columns | W_lo columns] until the fold
       float acc[kAccRegs];
       float (&acc_hi)[BLOCK_N / 2] = *reinterpret_cast<float (*)[BLOCK_N / 2]>(acc);
 #pragma unroll
@@ -334,7 +347,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
               const uint64_t ad = kdesc(abase + j * sgm.jbytes);
               const uint64_t bd = kdesc(b_ring + bs * b_slot);
               wgmma_fence();  // directly in front of the straight-line wgmmas: no branch between the fence and them
-              if constexpr (X3) {
+              if constexpr (P == kBF16X3) {
                 const uint64_t adl = kdesc(abase + sgm.a_stride + j * sgm.jbytes);
 #pragma unroll
                 for (int k = 0; k < kRowBytes / 32; ++k) wgmma_kmajor<2 * BLOCK_N, false>(acc, ad + 2 * k, bd + 2 * k, 1u);
@@ -343,7 +356,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
                 for (int k = 0; k < kRowBytes / 32; ++k) wgmma_kmajor<BLOCK_N, false>(acc_hi, adl + 2 * k, bd + 2 * k, 1u);
               } else {
 #pragma unroll
-                for (int k = 0; k < kRowBytes / 32; ++k) wgmma_kmajor<BLOCK_N, TF32>(acc, ad + 2 * k, bd + 2 * k, 1u);
+                for (int k = 0; k < kRowBytes / 32; ++k) wgmma_kmajor<BLOCK_N, P == kTF32>(acc, ad + 2 * k, bd + 2 * k, 1u);
               }
               wgmma_commit();
               wgmma_wait<1>();  // the previous k-step's wgmmas have retired: hand its slots back to the producer
@@ -364,7 +377,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
           if (prev_b >= 0) mbar_arrive(b_empty + 8 * prev_b);
           if (prev_a >= 0) mbar_arrive(a_empty + 8 * prev_a);
         }
-        if constexpr (X3) {
+        if constexpr (P == kBF16X3) {
 #pragma unroll
           for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] += acc[BLOCK_N / 2 + i];
         }
@@ -434,14 +447,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
           const uint4* rp = reinterpret_cast<const uint4*>(base + off);
 #pragma unroll
           for (int i = 0; i < 4; ++i) rbuf[i] = __ldg(rp + i);
-          if constexpr (X3) {
+          if constexpr (P == kBF16X3) {
             const uint4* rl = reinterpret_cast<const uint4*>(base + off + (second ? p.res1_lo_off : p.res_lo_off));
 #pragma unroll
             for (int i = 0; i < 4; ++i) rbuf[4 + i] = __ldg(rl + i);
           }
           return;
         }
-        if (TF32 || p.res_fp32) {
+        if (P == kTF32 || p.res_fp32) {
           const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(p.res) + roff + nbp);
 #pragma unroll
           for (int i = 0; i < 8; ++i) rbuf[i] = __ldg(rp + i);
@@ -449,7 +462,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
           const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + roff + nbp);
 #pragma unroll
           for (int i = 0; i < 4; ++i) rbuf[i] = __ldg(rp + i);
-          if constexpr (X3) {
+          if constexpr (P == kBF16X3) {
             const uint4* rl = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + roff + nbp + p.res_lo_off);
 #pragma unroll
             for (int i = 0; i < 4; ++i) rbuf[4 + i] = __ldg(rl + i);
@@ -488,8 +501,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
           if (splits > 1) {
             // split-K: raw fp32 partial sums; bias / residual / statistics are applied by the reduction kernel
             if (valid) {
-              // (X3: ooff is in physical bf16 elements, twice the logical row pitch the fp32 partials use)
-              float* pp = p.partial + (long long)(tile % splits) * p.split_stride + (X3 ? (ooff >> 1) : ooff) + nb;
+              // (split bf16: ooff is in physical bf16 elements, twice the logical row pitch the fp32 partials use)
+              float* pp = p.partial + (long long)(tile % splits) * p.split_stride + (P == kBF16X3 ? (ooff >> 1) : ooff) + nb;
               if (nb + 32 <= p.N) {
 #pragma unroll
                 for (int i = 0; i < 8; ++i)
@@ -524,7 +537,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
                 const float4 kc = __ldg(cc + i);
                 const __nv_bfloat16 xb = reinterpret_cast<const __nv_bfloat16*>(rbuf)[i];
                 float xv = __bfloat162float(xb);
-                if constexpr (X3) xv += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(rbuf + 4)[i]);
+                if constexpr (P == kBF16X3) xv += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(rbuf + 4)[i]);
                 float d = v[i];
                 if (p.gnb_drop_thresh > 0) {
                   const unsigned r16 = (unsigned)((hsh[i >> 2] >> (16 * (i & 3))) & 0xFFFFu);
@@ -532,7 +545,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
                 }
                 if (p.gnb_silu) {
                   const float h = fmaf(xv, kc.x, kc.y);
-                  d *= X3 ? dsilu_ex2_half(h) : dsilu_tanh_half(h);
+                  d *= P == kBF16X3 ? dsilu_ex2_half(h) : dsilu_tanh_half(h);
                 }
                 v[i] = d;
                 q2[i] = d * fmaf(xv, kc.z, kc.w);
@@ -543,81 +556,40 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
             }
           }
           if (!GNB && p.res && valid) {
-            if (TF32 || p.res_fp32) {
+            if (P == kTF32 || p.res_fp32) {  // plain fp32 (also the tf32 activation format, whose loads need no rounding)
               if (full) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const float4 t = *reinterpret_cast<const float4*>(&rbuf[i]);
-                  v[4 * i] += t.x; v[4 * i + 1] += t.y; v[4 * i + 2] += t.z; v[4 * i + 3] += t.w;
-                }
+                add_res_chunk<kTF32>(rbuf, v);
               } else {
                 const float* rp = reinterpret_cast<const float*>(p.res) + roff + nb;
                 for (int i = 0; i < 32; ++i) if (nb + i < p.N) v[i] += rp[i];
               }
             } else {
               if (full) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&rbuf[i]);
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-                    float2 f = __bfloat1622float2(h[j]);
-                    if constexpr (X3) {
-                      const float2 l = __bfloat1622float2(reinterpret_cast<const __nv_bfloat162*>(&rbuf[4 + i])[j]);
-                      f.x += l.x; f.y += l.y;
-                    }
-                    v[8 * i + 2 * j] += f.x; v[8 * i + 2 * j + 1] += f.y;
-                  }
-                }
+                add_res_chunk<P>(rbuf, v);
               } else {
-                const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.res) + roff + nb;
-                for (int i = 0; i < 32; ++i)
-                  if (nb + i < p.N) v[i] += __bfloat162float(rp[i]) + (X3 ? __bfloat162float(rp[i + p.res_lo_off]) : 0.f);
+                const ActElem<P>* rp = reinterpret_cast<const ActElem<P>*>(p.res) + roff + nb;
+                for (int i = 0; i < 32; ++i) if (nb + i < p.N) v[i] += load_split<P>(rp + i, p.res_lo_off);
               }
             }
           }
           if (ch + kChunkStep < kChunks) prefetch_res(ch + kChunkStep);  // lands while this chunk is stored / reduced
           if (valid) {
-            if (TF32 || p.out_fp32) {
+            if (p.out_fp32) {
               float* op = reinterpret_cast<float*>(p.out) + ooff + nb;
               if (full) {
 #pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  float4 t = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-                  if (p.round_out) { t.x = to_tf32_rna(t.x); t.y = to_tf32_rna(t.y); t.z = to_tf32_rna(t.z); t.w = to_tf32_rna(t.w); }
-                  reinterpret_cast<float4*>(op)[i] = t;
-                }
+                for (int i = 0; i < 8; ++i) reinterpret_cast<float4*>(op)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
               } else {
                 for (int i = 0; i < 32; ++i) if (nb + i < p.N) op[i * p.ocs] = v[i];
               }
             } else {
-              __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + ooff + nb;
+              ActElem<P>* op = reinterpret_cast<ActElem<P>*>(p.out) + ooff + nb;
               if (full) {
+                constexpr int E = kVecElems<P>;
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  uint4 t;
-                  __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&t);
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) h[j] = __floats2bfloat162_rn(v[8 * i + 2 * j], v[8 * i + 2 * j + 1]);
-                  reinterpret_cast<uint4*>(op)[i] = t;
-                  if constexpr (X3) {  // lo parts: what the bf16 rounding of the hi parts lost
-                    uint4 tl;
-                    __nv_bfloat162* l = reinterpret_cast<__nv_bfloat162*>(&tl);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                      const float2 f = __bfloat1622float2(h[j]);
-                      l[j] = __floats2bfloat162_rn(v[8 * i + 2 * j] - f.x, v[8 * i + 2 * j + 1] - f.y);
-                    }
-                    reinterpret_cast<uint4*>(op + p.out_lo_off)[i] = tl;
-                  }
-                }
+                for (int i = 0; i < 32 / E; ++i) store_vec<P>(op + E * i, p.out_lo_off * (long long)sizeof(ActElem<P>), v + E * i);
               } else {
-                for (int i = 0; i < 32; ++i)
-                  if (nb + i < p.N) {
-                    const __nv_bfloat16 hb = __float2bfloat16(v[i]);
-                    op[i * p.ocs] = hb;
-                    if constexpr (X3) op[i * p.ocs + p.out_lo_off] = __float2bfloat16(v[i] - __bfloat162float(hb));
-                  }
+                for (int i = 0; i < 32; ++i) if (nb + i < p.N) store_split<P>(op + i * p.ocs, p.out_lo_off, v[i]);
               }
             }
           }

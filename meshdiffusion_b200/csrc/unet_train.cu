@@ -183,7 +183,7 @@ void UNet::emit_colsum(const std::string& name, const GradView& t, int R, float*
 // G[tap][m][n] = sum_p dy[p][m] x[p+tap][n] scattered to the parameter gradient at `goff` with `layout` strides
 void UNet::emit_wgrad(const std::string& name, const Act& dy, const Act& x, int ksize, int stride, long long goff,
                       const WgradOut& layout) {
-  const WgradPlan pl = plan_wgrad(dy.X, dy.Y, dy.Z, dy.B, dy.C, x.C, ksize, stride, prec_ == kBF16X3);
+  const WgradPlan pl = plan_wgrad(dy.X, dy.Y, dy.Z, dy.B, dy.C, x.C, ksize, stride, prec_);
   Tmp sc = tmp_alloc(pl.scratch_bytes);
   auto op = std::make_unique<WgradOp>();
   op->name = name;

@@ -14,11 +14,11 @@ static Geometry half_geometry(Geometry g) {
   return g;
 }
 
-WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int stride, bool x3) {
+WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int stride, Precision prec) {
   WgradPlan pl;
   if (ksize != 1 && ksize != 3) throw std::runtime_error("mdb: wgrad supports 1x1x1 and 3x3x3 kernels");
   pl.flat = ksize == 1;
-  const int vox = x3 ? 64 : 128;
+  const int vox = 128 / parts(prec);
   long long tiles;
   if (pl.flat) {
     pl.geo = {vox, 1, 1, 1};
@@ -26,7 +26,7 @@ WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int st
     tiles = ((long long)B * X * Y * Z + vox - 1) / vox;
   } else {
     pl.geo = pick_geometry(X, Y, Z);
-    if (x3) pl.geo = half_geometry(pl.geo);
+    if (prec == kBF16X3) pl.geo = half_geometry(pl.geo);
     if (pl.geo.bx * pl.geo.by * pl.geo.bz * pl.geo.bb != vox) throw std::runtime_error("mdb: unsupported wgrad tile geometry");
     pl.n_groups = 27;
     pl.taps = 27;
@@ -47,9 +47,9 @@ WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int st
 void WgradOp::init(const Act& dy, const Act& x, int ksize, int stride, const WgradOut& out, float* scratch, Precision prec) {
   if (prec == kTF32) throw std::runtime_error("mdb: weight gradients are built for bf16 or split-bf16 operands");
   dy_ = dy; x_ = x; ksize_ = ksize; stride_ = stride; out_ = out;
-  x3_ = prec == kBF16X3;
+  prec_ = prec;
   M_ = dy.C; N_ = x.C;
-  plan_ = plan_wgrad(dy.X, dy.Y, dy.Z, dy.B, M_, N_, ksize, stride, x3_);
+  plan_ = plan_wgrad(dy.X, dy.Y, dy.Z, dy.B, M_, N_, ksize, stride, prec);
   if (ksize == 3 && stride == 1 && (x.X != dy.X || x.Y != dy.Y || x.Z != dy.Z)) throw std::runtime_error("mdb: wgrad extent mismatch");
   if (ksize == 3 && stride == 2 && (x.X != 2 * dy.X || x.Y != 2 * dy.Y || x.Z != 2 * dy.Z)) throw std::runtime_error("mdb: stride-2 wgrad extent mismatch");
   if (ksize == 1 && x.voxels() != dy.voxels()) throw std::runtime_error("mdb: pointwise wgrad extent mismatch");
@@ -79,49 +79,28 @@ const WgradParams& WgradOp::params_for(int B) {
   auto it = cache_.find(B);
   if (it != cache_.end()) return it->second;
   WgradParams p = base_;
-  const long long es = 2;
-  const long long parts = x3_ ? 2 : 1;  // X3: physical row = hi parts | lo parts; part 1 maps start one logical row in
-  uint64_t dims[5], strides[4];
-  uint32_t box[5];
+  Act dy = dy_, x = x_;
   if (plan_.flat) {
+    // one row axis over the voxels of every sample (pointwise: stride 1)
     const long long rows = (long long)B * dy_.voxels();
-    const int vox = p.bx;
-    p.tx = (int)((rows + vox - 1) / vox); p.ty = p.tz = p.tb = 1;
-    auto enc = [&](CUtensorMap* m, const Act& a, int part) {
-      dims[0] = a.C; dims[1] = rows; dims[2] = dims[3] = dims[4] = 1;
-      strides[0] = a.row() * es * parts; strides[1] = strides[0] * rows; strides[2] = strides[1]; strides[3] = strides[1];
-      box[0] = 64; box[1] = vox; box[2] = box[3] = box[4] = 1;
-      encode_map(m, kBF16, 5, static_cast<char*>(a.ptr) + part * a.row() * es, dims, strides, box);
-    };
-    enc(&p.ymap, dy_, 0);
-    enc(&p.xmap[0], x_, 0);
-    if (x3_) { enc(&p.ymap_lo, dy_, 1); enc(&p.xmap_lo[0], x_, 1); }
+    p.tx = (int)((rows + p.bx - 1) / p.bx); p.ty = p.tz = p.tb = 1;
+    dy.X = x.X = (int)rows;
+    dy.Y = dy.Z = dy.B = x.Y = x.Z = x.B = 1;
   } else {
     p.tx = (dy_.X + p.bx - 1) / p.bx; p.ty = (dy_.Y + p.by - 1) / p.by; p.tz = (dy_.Z + p.bz - 1) / p.bz;
     p.tb = (B + p.bb - 1) / p.bb;
-    auto enc = [&](CUtensorMap* m, const Act& a, int sub, int px, int py, int pz, int part) {
-      char* base = static_cast<char*>(a.ptr) + part * a.row() * es;
-      const long long sx = a.row() * es * parts, sy = sx * a.X, sz = sy * a.Y, sb = sz * a.Z;
-      dims[0] = a.C; dims[4] = B;
-      if (sub == 1) {
-        dims[1] = a.X; dims[2] = a.Y; dims[3] = a.Z;
-        strides[0] = sx; strides[1] = sy; strides[2] = sz; strides[3] = sb;
-      } else {
-        dims[1] = (a.X - px + sub - 1) / sub; dims[2] = (a.Y - py + sub - 1) / sub; dims[3] = (a.Z - pz + sub - 1) / sub;
-        strides[0] = sx * sub; strides[1] = sy * sub; strides[2] = sz * sub; strides[3] = sb;
-        base += px * sx + py * sy + pz * sz;
-      }
-      box[0] = 64; box[1] = p.bx; box[2] = p.by; box[3] = p.bz; box[4] = p.bb;
-      encode_map(m, kBF16, 5, base, dims, strides, box);
-    };
-    for (int part = 0; part < (int)parts; ++part) {
-      enc(part ? &p.ymap_lo : &p.ymap, dy_, 1, 0, 0, 0, part);
-      CUtensorMap* xm = part ? p.xmap_lo : p.xmap;
-      if (stride_ == 1) {
-        enc(&xm[0], x_, 1, 0, 0, 0, part);
-      } else {
-        for (int par = 0; par < 8; ++par) enc(&xm[par], x_, 2, par & 1, (par >> 1) & 1, (par >> 2) & 1, part);
-      }
+    dy.B = x.B = B;
+  }
+  auto enc = [&](CUtensorMap* m, const Act& a, int part, int sub = 1, int par = 0) {
+    encode_map(m, prec_, act_map(a, prec_, part, plan_.geo, sub, par & 1, (par >> 1) & 1, (par >> 2) & 1));
+  };
+  for (int part = 0; part < parts(prec_); ++part) {
+    enc(part ? &p.ymap_lo : &p.ymap, dy, part);
+    CUtensorMap* xm = part ? p.xmap_lo : p.xmap;
+    if (stride_ == 1) {
+      enc(&xm[0], x, part);
+    } else {
+      for (int par = 0; par < 8; ++par) enc(&xm[par], x, part, 2, par);
     }
   }
   const long long tiles = 1LL * p.tx * p.ty * p.tz * p.tb;
@@ -169,13 +148,13 @@ void WgradOp::launch(cudaStream_t s, int B, bool accumulate, float* out_ptr) {
   MDB_CUDA_CHECK(cudaGetDevice(&dev));
   bool& configured = configured_dev[dev < 64 ? dev : 63];
   if (!configured || dev >= 63) {
-    MDB_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes));
-    MDB_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes));
+    MDB_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel<kBF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes));
+    MDB_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel<kBF16X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemBytes));
     configured = true;
   }
   const int grid = p.m_tiles * p.n_tiles * p.n_groups * p.splits;
-  if (x3_) wgrad_tc_kernel<true><<<grid, kWgThreads, kWgSmemBytes, s>>>(p);
-  else wgrad_tc_kernel<false><<<grid, kWgThreads, kWgSmemBytes, s>>>(p);
+  if (prec_ == kBF16X3) wgrad_tc_kernel<kBF16X3><<<grid, kWgThreads, kWgSmemBytes, s>>>(p);
+  else wgrad_tc_kernel<kBF16><<<grid, kWgThreads, kWgSmemBytes, s>>>(p);
   MDB_CUDA_CHECK(cudaGetLastError());
   WgradReduceArgs r{};
   r.partial = p.partial; r.splits = p.splits; r.taps = p.taps; r.Mp = p.Mp; r.Np = p.Np; r.M = out_.m_valid ? out_.m_valid : M_; r.N = out_.n_valid ? out_.n_valid : N_;

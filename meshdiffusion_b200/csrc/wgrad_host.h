@@ -22,8 +22,8 @@ struct WgradPlan {
   size_t scratch_bytes = 0;
 };
 // dY extents (X,Y,Z,B) = output positions of the forward op; M = dY channels, N = X-operand channels.
-// x3: split-bf16 operands (64-voxel tiles).
-WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int stride, bool x3 = false);
+// prec: the operand mode (split-bf16 operands: 64-voxel tiles).
+WgradPlan plan_wgrad(int X, int Y, int Z, int B, int M, int N, int ksize, int stride, Precision prec);
 
 class WgradOp {
  public:
@@ -42,7 +42,7 @@ class WgradOp {
   WgradParams base_{};
   Act dy_, x_;
   int ksize_ = 1, stride_ = 1, M_ = 0, N_ = 0;
-  bool x3_ = false;
+  Precision prec_ = kBF16;
   WgradOut out_;
   std::map<int, WgradParams> cache_;  // tensor maps encoded for a given runtime batch
   const WgradParams& params_for(int B);

@@ -12,7 +12,7 @@
 // thread can hold next to its addressing.) Partials are summed in a fixed order by wgrad_reduce_kernel (deterministic
 // gradients), which also scatters into the reference's OIDHW layout.
 //
-// Split-bf16 operands (X3 instantiation, Precision::kBF16X3): dY and X are (hi, lo) bf16 pairs and the contraction is
+// Split-bf16 operands (the Precision::kBF16X3 instantiation): dY and X are (hi, lo) bf16 pairs and the contraction is
 // dYlo.Xhi + dYhi.Xlo + dYhi.Xhi into the same register accumulator (lo.lo dropped, 2^-16 relative). A stage then
 // carries the hi and lo parts of both operands for HALF the voxels (64-voxel boxes): still 64 KB, still three stages.
 //
@@ -55,10 +55,11 @@ struct WgradParams {
 };
 
 #ifdef MDB_WGRAD_KERNEL_IMPL  // the kernel itself is compiled in wgrad_host.cu only
-template <bool X3>
+template <Precision P>
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ WgradParams p) {
-  // one 64-channel block of one operand part; stage = [dY blocks][dY lo blocks][X blocks][X lo blocks] (lo: X3 only)
-  constexpr int CH = X3 ? kWgYChunkBytes / 2 : kWgYChunkBytes;
+  static_assert(P != kTF32, "weight gradients are built for bf16 / split-bf16 operands");
+  // one 64-channel block of one operand part; stage = [dY blocks][dY lo blocks][X blocks][X lo blocks] (lo: split bf16 only)
+  constexpr int CH = P == kBF16X3 ? kWgYChunkBytes / 2 : kWgYChunkBytes;
   constexpr int KS = CH / 2048;  // 16-voxel wgmma k-steps per stage
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -83,7 +84,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.ymap);
     tma_prefetch_desc(&p.xmap[grp.xmap]);
-    if (X3) { tma_prefetch_desc(&p.ymap_lo); tma_prefetch_desc(&p.xmap_lo[grp.xmap]); }
+    if (P == kBF16X3) { tma_prefetch_desc(&p.ymap_lo); tma_prefetch_desc(&p.xmap_lo[grp.xmap]); }
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kWgStages; ++i) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 2); }
@@ -111,14 +112,14 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
           mbar_expect_tx(bar, bytes);
           tma_load_5d(&p.ymap, bar, sbase, m0, x0, y0, z0, b0);
           tma_load_5d(&p.ymap, bar, sbase + CH, m0 + 64, x0, y0, z0, b0);
-          if (X3) {
+          if (P == kBF16X3) {
             tma_load_5d(&p.ymap_lo, bar, sbase + 2 * CH, m0, x0, y0, z0, b0);
             tma_load_5d(&p.ymap_lo, bar, sbase + 3 * CH, m0 + 64, x0, y0, z0, b0);
           }
-          const uint32_t xb = sbase + (X3 ? 4 : 2) * CH;
+          const uint32_t xb = sbase + (P == kBF16X3 ? 4 : 2) * CH;
           tma_load_5d(&p.xmap[grp.xmap], bar, xb, n0, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
           tma_load_5d(&p.xmap[grp.xmap], bar, xb + CH, n0 + 64, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
-          if (X3) {
+          if (P == kBF16X3) {
             tma_load_5d(&p.xmap_lo[grp.xmap], bar, xb + 2 * CH, n0, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
             tma_load_5d(&p.xmap_lo[grp.xmap], bar, xb + 3 * CH, n0 + 64, x0 + grp.dx, y0 + grp.dy, z0 + grp.dz, b0);
           }
@@ -140,12 +141,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
       mbar_wait(full + 8 * st, ph);
       const uint32_t sbase = stage0 + st * kWgStageBytes;
       // A = this warpgroup's 64-channel dY block (one MN block); B = both 64-channel X blocks, LBO apart
-      // (X3: hi blocks at 0 / 4 CH, lo blocks at 2 CH / 6 CH)
+      // (split bf16: hi blocks at 0 / 4 CH, lo blocks at 2 CH / 6 CH)
       const uint64_t a0 = make_wgmma_desc(sbase + wg * CH, CH, 1024);
-      const uint64_t b0 = make_wgmma_desc(sbase + (X3 ? 4 : 2) * CH, CH, 1024);
+      const uint64_t b0 = make_wgmma_desc(sbase + (P == kBF16X3 ? 4 : 2) * CH, CH, 1024);
       fence_operands(acc);
       wgmma_fence();
-      if constexpr (X3) {
+      if constexpr (P == kBF16X3) {
         // small terms first: dYlo.Xhi, dYhi.Xlo, then dYhi.Xhi
         const uint64_t al = make_wgmma_desc(sbase + (2 + wg) * CH, CH, 1024);
         const uint64_t bl = make_wgmma_desc(sbase + 6 * CH, CH, 1024);

@@ -86,6 +86,24 @@ def test_conv3d_epilogue_terms(precision):
     assert err < TOL[precision]
 
 
+def test_conv3d_tf32_stores_tf32_values_in_the_tail_chunk():
+    """tf32 activations are stored rounded to tf32 (rna) on every epilogue path: with 48 output channels each row is one
+    full 32-column chunk and a 16-column tail, and both keep the low 13 mantissa bits zero."""
+    from meshdiffusion_b200 import ops
+    _ref_setup()
+    B, Cin, Cout, R = 2, 64, 48, 16
+    g = torch.Generator(device="cuda").manual_seed(5)
+    x = torch.randn(B, Cin, R, R, R, device="cuda", generator=g)
+    w = torch.randn(Cout, Cin, 3, 3, 3, device="cuda", generator=g) / (Cin * 27) ** 0.5
+    b = torch.randn(Cout, device="cuda", generator=g)
+    y = ops.conv3d(ops.to_ndhwc(x, "tf32"), w, b, precision="tf32")
+    low = y.view(torch.int32) & 0x1FFF
+    assert (low[..., :32] == 0).all()
+    assert (low[..., 32:] == 0).all(), "tail chunk stored without tf32 rounding"
+    err = _rel(ops.from_ndhwc(y, "tf32"), F.conv3d(x, w, b, padding=1))
+    assert err < TOL["tf32"]
+
+
 @pytest.mark.parametrize("precision", ["tf32", "bf16", "bf16x3"])
 def test_groupnorm_silu(precision):
     from meshdiffusion_b200 import ops

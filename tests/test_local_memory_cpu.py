@@ -10,8 +10,8 @@ import subprocess
 import pytest
 
 CLEAN = """\
-ptxas info    : Compiling entry function '_ZN3mdb14gemm_tc_kernelILi128ELb0ELb0ELb1EEEvNS_10GemmParamsE' for 'sm_90a'
-ptxas info    : Function properties for _ZN3mdb14gemm_tc_kernelILi128ELb0ELb0ELb1EEEvNS_10GemmParamsE
+ptxas info    : Compiling entry function '_ZN3mdb14gemm_tc_kernelILi128ELNS_9PrecisionE2ELb0EEEvNS_10GemmParamsE' for 'sm_90a'
+ptxas info    : Function properties for _ZN3mdb14gemm_tc_kernelILi128ELNS_9PrecisionE2ELb0EEEvNS_10GemmParamsE
     0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads
 ptxas info    : Used 168 registers, used 3 barriers
 ptxas info    : Function properties for _ZN3mdb19pack_weights_kernelILNS_9PrecisionE0EEEvPKNS_9LoadEntryEPKiiNS_8PackArgsEiiiPv
@@ -29,8 +29,8 @@ def test_guard_passes_a_clean_report_and_other_kernels():
     assert build.local_memory_violations(CLEAN) == []
 
 
-@pytest.mark.parametrize("fn", ["_ZN3mdb14gemm_tc_kernelILi32ELb0ELb1ELb0EEEvNS_10GemmParamsE",
-                                "_ZN3mdb15wgrad_tc_kernelILb1EEEvNS_11WgradParamsE"])
+@pytest.mark.parametrize("fn", ["_ZN3mdb14gemm_tc_kernelILi32ELNS_9PrecisionE0ELb1EEEvNS_10GemmParamsE",
+                                "_ZN3mdb15wgrad_tc_kernelILNS_9PrecisionE2EEEvNS_11WgradParamsE"])
 @pytest.mark.parametrize("frame", [(256, 0, 0), (0, 8, 0), (0, 0, 8)])
 def test_guard_flags_stack_and_spills(fn, frame):
     from meshdiffusion_b200 import build
