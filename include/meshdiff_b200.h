@@ -158,6 +158,35 @@ int mdb_sampler_run(mdb_unet* net, float* x, float* x_mean, const float* mask, c
                     float* eps_buf, float* labels_buf, int step0, const mdb_sampler_cond* cond /* nullable */,
                     const float* cond_mean_coefs, const float* cond_stds, int cond_until, void* stream);
 
+/* Few-step sampling: DPM-Solver++(2M) (Lu et al. 2022), ODE or SDE form, on the same noise prediction as the sampler
+ * above (diffusion/sampling.py: get_dpm_solver_sampler, which computes the step table in float64 on the host).
+ * Step k runs the network at label n_k and moves x from n_k to n_{k+1}:
+ *   x0 = (x - sigma eps) inv_alpha;   x' = (c_x x + c_0 x0 + c_1 x0_prev + c_z z) g;   x0_prev <- x0
+ * with g the grid mask. c_1 = 0 marks a first-order step (x0_hist is not read); c_z = 0 one without noise. With `cond`,
+ * channel `channel` is then replaced: x_c <- (x_c (1 - pm) + (cond_coef partial + cond_std z') pm) g (the mean_coef / std
+ * fields of mdb_sampler_cond are ignored). */
+typedef struct mdb_solver_step {
+  float label;               /* network label n_k */
+  float sigma, inv_alpha;    /* x0 = (x - sigma*eps) * inv_alpha */
+  float c_x, c_0, c_1, c_z;  /* x' = c_x*x + c_0*x0 + c_1*x0_prev + c_z*z */
+  float cond_coef, cond_std; /* replacement after the step: alpha, sigma of n_{k+1} */
+} mdb_solver_step;
+
+/* One step, in place on x and x0_hist ([batch][channels][voxels] fp32; mask [voxels]). noise: z [batch][channels][voxels],
+ * or NULL for Philox(seed, element, offset) as in mdb_sampler_update (a loop passes offset = 4 * k); cond->noise likewise
+ * NULL for Philox(seed, element, offset + 2). */
+int mdb_solver_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_solver_step* step,
+                      long long voxels, int channels, int batch, const float* noise /* nullable */,
+                      unsigned long long seed, unsigned long long offset, const mdb_sampler_cond* cond /* nullable */,
+                      void* stream);
+/* The whole solver loop without host round trips: for i < n_steps: steps[i].label -> network -> mdb_solver_update with
+ * in-kernel Philox at offset 4 * (step0 + i), and the replacement while step0 + i < cond_until. `steps` is a HOST array of
+ * n_steps entries for the global steps step0 .. step0 + n_steps - 1. eps_buf: device scratch [B][C][V]; labels_buf: device
+ * scratch [B]. cond->noise must be NULL. The call only enqueues work. */
+int mdb_solver_run(mdb_unet* net, float* x, float* x0_hist, const float* mask, const mdb_solver_step* steps, int n_steps,
+                   int batch, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
+                   const mdb_sampler_cond* cond /* nullable */, int cond_until, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Training-step kernels (optimiser side). Replace get_ddpm_loss_fn's elementwise tail (lib/diffusion/losses.py:69-78),
  * torch.nn.utils.clip_grad_norm_ + torch.optim.Adam.step (losses.py:45-50, 26-35) and

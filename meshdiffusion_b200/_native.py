@@ -44,6 +44,12 @@ class SamplerCondC(ctypes.Structure):
     ]
 
 
+class SolverStepC(ctypes.Structure):
+    """mdb_solver_step (include/meshdiff_b200.h)."""
+    _fields_ = [(name, ctypes.c_float) for name in
+                ("label", "sigma", "inv_alpha", "c_x", "c_0", "c_1", "c_z", "cond_coef", "cond_std")]
+
+
 # name -> (restype, argtypes); the symbol list is checked against the header by tests/test_abi.py
 _vp, _i, _ll, _f, _u64, _d = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float, ctypes.c_ulonglong, ctypes.c_double
 SIGNATURES = {
@@ -78,6 +84,10 @@ SIGNATURES = {
     "mdb_sampler_update": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _f, _ll, _i, _i, _u64, _u64, ctypes.POINTER(SamplerCondC), _vp]),
     "mdb_sampler_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(_f), ctypes.POINTER(_f), ctypes.POINTER(_f), _i, _i, _u64, _vp, _vp,
                              _i, ctypes.POINTER(SamplerCondC), ctypes.POINTER(_f), ctypes.POINTER(_f), _i, _vp]),
+    "mdb_solver_update": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverStepC), _ll, _i, _i, _vp, _u64, _u64,
+                               ctypes.POINTER(SamplerCondC), _vp]),
+    "mdb_solver_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverStepC), _i, _i, _u64, _vp, _vp, _i,
+                            ctypes.POINTER(SamplerCondC), _i, _vp]),
     "mdb_ddpm_loss": (_i, [_vp, _vp, _vp, _d, _vp, _vp, _vp, _i, _i, _ll, _vp]),
     "mdb_ddpm_perturb": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _ll, _vp]),
     "mdb_chunk_elems": (_i, []),

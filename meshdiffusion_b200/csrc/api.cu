@@ -313,6 +313,55 @@ int mdb_sampler_run(mdb_unet* n, float* x, float* x_mean, const float* mask, con
   MDB_API_END
 }
 
+static SolverUpdateArgs solver_args(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_solver_step& st,
+                                    long long V, int C, const mdb_sampler_cond* c) {
+  SolverUpdateArgs a{};
+  a.eps = eps; a.x = x; a.x0_hist = x0_hist; a.mask = mask;
+  a.sigma = st.sigma; a.inv_alpha = st.inv_alpha; a.c_x = st.c_x; a.c_0 = st.c_0; a.c_1 = st.c_1; a.c_z = st.c_z;
+  a.V = V; a.C = C;
+  if (c && c->partial) {
+    if (!c->partial_mask) throw std::runtime_error("mdb: conditional sampling needs partial_mask");
+    if (c->channel < 0 || c->channel >= C) throw std::runtime_error("mdb: partial_channel out of range");
+    a.cond_partial = c->partial; a.cond_partial_bs = c->partial_bstride;
+    a.cond_pmask = c->partial_mask; a.cond_pmask_bs = c->mask_bstride;
+    a.cond_channel = c->channel; a.cond_coef = st.cond_coef; a.cond_std = st.cond_std; a.cond_noise = c->noise;
+  }
+  return a;
+}
+
+int mdb_solver_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_solver_step* step,
+                      long long V, int C, int B, const float* noise, unsigned long long seed, unsigned long long offset,
+                      const mdb_sampler_cond* cond, void* stream) {
+  MDB_API_BEGIN
+  if (!step) throw std::runtime_error("mdb: mdb_solver_update needs a step");
+  if (V <= 0 || C <= 0 || B <= 0) throw std::runtime_error("mdb: mdb_solver_update needs positive voxels, channels, batch");
+  SolverUpdateArgs a = solver_args(eps, x, x0_hist, mask, *step, V, C, cond);
+  a.noise = noise; a.seed = seed; a.offset = offset;
+  launch_solver_update(a, B, (cudaStream_t)stream);
+  MDB_API_END
+}
+
+int mdb_solver_run(mdb_unet* n, float* x, float* x0_hist, const float* mask, const mdb_solver_step* steps, int n_steps,
+                   int B, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
+                   const mdb_sampler_cond* cond, int cond_until, void* stream) {
+  MDB_API_BEGIN
+  cudaStream_t s = (cudaStream_t)stream;
+  const UNetConfig& c = n->net->cfg();
+  const long long V = (long long)c.image_size * c.image_size * c.image_size;
+  if (n_steps > 0 && !steps) throw std::runtime_error("mdb: mdb_solver_run needs the step table");
+  if (cond && cond->noise) throw std::runtime_error("mdb: mdb_solver_run draws its noise in-kernel (cond->noise must be NULL)");
+  for (int i = 0; i < n_steps; ++i) {
+    fill_kernel<<<(B + 127) / 128, 128, 0, s>>>(labels_buf, steps[i].label, B);
+    n->net->forward(x, labels_buf, eps_buf, B, s, /*allow_graph=*/true);
+    SolverUpdateArgs a = solver_args(eps_buf, x, x0_hist, mask, steps[i], V, c.num_channels,
+                                     step0 + i < cond_until ? cond : nullptr);
+    // the same Philox counter blocks as mdb_sampler_run: 4 outputs per step, the replacement draw at +2
+    a.noise = nullptr; a.seed = seed; a.offset = 4ull * (unsigned long long)(step0 + i);
+    launch_solver_update(a, B, s);
+  }
+  MDB_API_END
+}
+
 int mdb_conv3d(const void* x, int B, int cin, int z, int y_, int x_, const float* w, const float* bias, int cout,
                int ksize, int stride, void* out, const float* rowbias, const void* residual, long long* stats,
                int precision, void* stream) {

@@ -1,5 +1,5 @@
 // Bandwidth-bound kernels around the wgmma contractions: GroupNorm finalize/apply (+SiLU), nearest 2x upsample,
-// stem im2col, attention softmax / V transpose, time-embedding MLP, ancestral-sampling update.
+// stem im2col, attention softmax / V transpose, time-embedding MLP, ancestral-sampling and DPM-Solver updates.
 // All of these are HBM-roofline kernels: 16-byte vector accesses, grid-stride loops sized to the SM count.
 #pragma once
 #include "act_format.cuh"
@@ -83,5 +83,26 @@ struct SamplerUpdateArgs {
   const float* cond_noise;       // z' [B][V] or null (then Philox(seed, element, offset + 2))
 };
 void launch_sampler_update(const SamplerUpdateArgs& a, int B, cudaStream_t s);
+
+// One DPM-Solver++(2M) step (ODE or SDE form), in place, fp32 NCDHW [B][C][V]; mask [V]:
+//   x0 = (x - sigma eps) inv_alpha;  x' = (c_x x + c_0 x0 [+ c_1 x0_prev] [+ c_z z]) g;  x0_hist <- x0
+// then, when cond_partial != nullptr, on channel cond_channel: x_c <- (x_c (1-pm) + (coef partial + std z') pm) g.
+// The c_1 term is skipped when c_1 == 0 (first-order step: x0_hist is not read) and the noise term when c_z == 0.
+struct SolverUpdateArgs {
+  const float* eps;    // network output
+  float* x;            // in/out state
+  float* x0_hist;      // in: x0 of the previous step, out: x0 of this step
+  const float* mask;   // [V]
+  float sigma, inv_alpha, c_x, c_0, c_1, c_z;
+  long long V; int C;
+  const float* noise;               // z ~ N(0,1) [B][C][V] or null (then Philox(seed, element, offset))
+  unsigned long long seed, offset;
+  const float* cond_partial; long long cond_partial_bs;  // channel c of sample 0, sample stride (0 = shared grid)
+  const float* cond_pmask; long long cond_pmask_bs;
+  int cond_channel;
+  float cond_coef, cond_std;        // alpha, sigma of the label the step lands on
+  const float* cond_noise;          // z' [B][V] or null (then Philox(seed, element, offset + 2))
+};
+void launch_solver_update(const SolverUpdateArgs& a, int B, cudaStream_t s);
 
 }  // namespace mdb

@@ -6,7 +6,8 @@ freeze_iters)` (:357-487). The configured pair (ancestral_sampling + none, confi
 path: one native U-Net evaluation and ONE fused update kernel per step (score scaling, ancestral mean / noise and
 both grid-mask multiplies), with the state resident in HBM and no host synchronisation inside the loop. Other
 registered predictors / correctors use the same native network through `get_score_fn` with a few torch
-elementwise ops around it.
+elementwise ops around it. `method='dpm_solver'` (no working reference counterpart) is the few-step DPM-Solver++(2M)
+sampler at the end of this file.
 """
 import abc
 import ctypes
@@ -67,6 +68,12 @@ def get_sampling_fn(config, sde, shape, inverse_scaler, eps, grid_mask=None, ret
         return get_ddim_sampler(sde=sde, shape=shape, predictor=get_predictor("ddim"), inverse_scaler=inverse_scaler,
                                 n_steps=config.sampling.n_steps_each, denoise=config.sampling.noise_removal, eps=eps,
                                 device=config.device, grid_mask=grid_mask)
+    if method == "dpm_solver":
+        return get_dpm_solver_sampler(sde=sde, shape=shape, inverse_scaler=inverse_scaler,
+                                      n_steps=config.sampling.get("dpm_steps", 25),
+                                      stochastic=config.sampling.get("dpm_sde", False),
+                                      denoise=config.sampling.noise_removal, device=config.device, grid_mask=grid_mask,
+                                      native_rng=config.sampling.get("native_rng", False), seed=config.get("seed", 42))
     raise ValueError(f"Sampler name {method} unknown.")
 
 
@@ -204,7 +211,8 @@ def _native_net(model):
 class _Cond:
     """Replacement conditioning of the partial branch (sampling.py:453-467 of the reference) in the form the update kernel
     takes it: channel `c` of `partial` / `partial_mask` (batch 1 = one grid shared by all samples, or one per sample) and
-    the per-step marginal_prob scalars, computed with the reference's torch ops so they are bit-identical."""
+    the per-step marginal_prob scalars, computed with the reference's torch ops so they are bit-identical. The DPM-Solver
+    sampler passes timesteps=None: its per-step scalars are in the solver's step table."""
 
     def __init__(self, sde, partial, partial_mask, c, timesteps, B):
         V = partial[0, 0].numel()
@@ -216,6 +224,8 @@ class _Cond:
                 raise ValueError("partial / partial_mask must have batch 1 or the sampling batch")
         self.pb = V if self.partial.shape[0] == B and B > 1 else 0
         self.mb = V if self.pmask.shape[0] == B and B > 1 else 0
+        if timesteps is None:
+            return
         lmc = -0.25 * timesteps ** 2 * (sde.beta_1 - sde.beta_0) - 0.5 * timesteps * sde.beta_0  # sde_lib.py:211
         self.coefs = torch.exp(lmc).cpu().tolist()
         self.stds = torch.sqrt(1.0 - torch.exp(2.0 * lmc)).cpu().tolist()
@@ -445,3 +455,184 @@ def get_ddim_sampler(sde, shape, predictor, inverse_scaler, n_steps=1, denoise=F
             return inverse_scaler(x0_pred * grid_mask if denoise else x * grid_mask), sde.N * (n_steps + 1)
 
     return ddim_sampler
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# DPM-Solver++(2M) (Lu et al. 2022, "DPM-Solver++: Fast Solver for Guided Sampling of Diffusion Probabilistic Models"),
+# in its ODE form and in the SDE form of k-diffusion's sample_dpmpp_2m_sde: a second-order multistep exponential
+# integrator in log-SNR time on the same noise prediction as the samplers above, one network evaluation per step, so a
+# sample costs ~25 evaluations instead of 999.
+def dpm_solver_schedule(sde, n_steps, stochastic=False, denoise=True):
+    """Label grid and step table of DPM-Solver++(2M) with `n_steps` (K) log-SNR intervals.
+
+    With alpha_n = sqrt(alphas_cumprod[n]), sigma_n = sqrt(1 - alphas_cumprod[n]) and lambda_n = log alpha_n - log sigma_n
+    (float64), the labels are the ones whose lambda is nearest each of K + 1 equally spaced targets from lambda_{N-1} to
+    lambda_0, repeats dropped: labels[0] = N - 1, labels[-1] = 0, K_eff = len(labels) - 1 network evaluations (K_eff < K
+    only when two targets share a label, near label 0). Row k of the table (float64, mdb_solver_step field order: label,
+    sigma, inv_alpha, c_x, c_0, c_1, c_z, cond_coef, cond_std) moves x from labels[k] to labels[k + 1]:
+    x' = c_x x + c_0 x0_k + c_1 x0_{k-1} + c_z z with x0_k = (x - sigma eps) inv_alpha. Step 0 is first order (c_1 = 0);
+    with `denoise` the last SDE step adds no noise. Returns (labels, table)."""
+    if isinstance(n_steps, bool) or int(n_steps) != n_steps or n_steps < 2:
+        raise ValueError(f"sampling.dpm_steps must be an integer >= 2, got {n_steps!r}")
+    K = int(n_steps)
+    abar = sde.alphas_cumprod.detach().to("cpu", torch.float64).numpy()
+    N = abar.shape[0]
+    alpha, sigma = np.sqrt(abar), np.sqrt(1.0 - abar)
+    lam = np.log(alpha) - np.log(sigma)
+    targets = lam[N - 1] + np.arange(K + 1) * ((lam[0] - lam[N - 1]) / K)
+    labels = []
+    for t in targets:
+        n = int(np.argmin(np.abs(lam - t)))
+        if not labels or n != labels[-1]:
+            labels.append(n)
+    assert labels[0] == N - 1 and labels[-1] == 0 and all(a > b for a, b in zip(labels, labels[1:]))
+    K_eff = len(labels) - 1
+    table = np.zeros((K_eff, 9), dtype=np.float64)
+    h_prev = None
+    for k in range(K_eff):
+        s, t = labels[k], labels[k + 1]
+        h = lam[t] - lam[s]
+        if stochastic:
+            c_x = sigma[t] / sigma[s] * np.exp(-h)
+            b = -alpha[t] * np.expm1(-2.0 * h)
+            c_z = 0.0 if (denoise and k == K_eff - 1) else sigma[t] * np.sqrt(-np.expm1(-2.0 * h))
+        else:
+            c_x, b, c_z = sigma[t] / sigma[s], -alpha[t] * np.expm1(-h), 0.0
+        if h_prev is None:
+            c_0, c_1 = b, 0.0
+        else:
+            r = h_prev / h
+            c_0, c_1 = b * (1.0 + 1.0 / (2.0 * r)), -b / (2.0 * r)
+        table[k] = (s, sigma[s], 1.0 / alpha[s], c_x, c_0, c_1, c_z, alpha[t], sigma[t])
+        h_prev = h
+    return labels, table
+
+
+def _solver_steps_c(table):
+    """The step table as the float32 mdb_solver_step array the library takes."""
+    rows = table.astype(np.float32)
+    arr = (_native.SolverStepC * len(rows))()
+    for i, r in enumerate(rows):
+        arr[i] = _native.SolverStepC(*(float(v) for v in r))
+    return arr
+
+
+def _replace_channel(xc, partial, pmask, mask, coef, std, z):
+    """x_c <- (x_c (1 - pm) + (coef partial + std z) pm) g, fp32, in solver_update_kernel's operation order."""
+    sampled = partial * coef + z * std
+    return (xc * (1.0 - pmask) + sampled * pmask) * mask
+
+
+def _solver_update_eager(eps, x, x0_hist, mask, row, noise=None, cond=None, cond_noise=None):
+    """One solver step in torch fp32 ops, in place on x and x0_hist, with the operation order of solver_update_kernel (each
+    product and sum rounded on its own), so it is the kernel's bit-exact oracle. `row`: a float32 table row; `mask`
+    broadcasts over x; `cond`: a _Cond."""
+    label, sg, inv_a, c_x, c_0, c_1, c_z, coef, std = (float(v) for v in row)
+    x0 = (x - eps * sg) * inv_a
+    xn = x * c_x + x0 * c_0
+    if c_1 != 0.0:
+        xn = xn + x0_hist * c_1
+    if c_z != 0.0:
+        xn = xn + noise * c_z
+    xn = xn * mask
+    if cond is not None:
+        xn[:, cond.c] = _replace_channel(xn[:, cond.c], cond.partial, cond.pmask, mask, coef, std, cond_noise)
+    x0_hist.copy_(x0)
+    x.copy_(xn)
+    return x
+
+
+def _solver_update(eps, x, x0_hist, mask_flat, row_c, noise=None, cond=None, cond_noise=None, seed=0, offset=0):
+    """One step through mdb_solver_update, in place on x and x0_hist; noise=None draws it in-kernel."""
+    L = _native.lib()
+    B, C = x.shape[0], x.shape[1]
+    cs = cond.struct(noise=cond_noise) if cond is not None else None
+    _native.check(L.mdb_solver_update(_native.ptr(eps), _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat),
+                                      ctypes.byref(row_c), x[0, 0].numel(), C, B, _native.ptr(noise), int(seed),
+                                      int(offset), ctypes.byref(cs) if cs is not None else None,
+                                      _native.current_stream()))
+    return x
+
+
+def _native_solver_loop(net, x, x0_hist, mask_flat, steps_c, seed, step0=0, n=None, cond=None, cond_until=0):
+    """Steps step0 .. step0+n-1 of the solver loop inside the library (mdb_solver_run), in place on x and x0_hist.
+    `steps_c` is the whole table (_solver_steps_c), indexed by the GLOBAL step."""
+    L = _native.lib()
+    B = x.shape[0]
+    n = len(steps_c) - step0 if n is None else n
+    net._ensure_engine(B, x.device)
+    net.sync_parameters()
+    eps_buf = torch.empty_like(x)
+    labels_buf = torch.empty(B, device=x.device, dtype=torch.float32)
+    part = (_native.SolverStepC * n).from_buffer(steps_c, step0 * ctypes.sizeof(_native.SolverStepC))
+    cs = cond.struct() if cond is not None else None
+    _native.check(L.mdb_solver_run(net._handle, _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat), part, n, B,
+                                   int(seed), _native.ptr(eps_buf), _native.ptr(labels_buf), int(step0),
+                                   ctypes.byref(cs) if cs is not None else None, int(cond_until),
+                                   _native.current_stream()))
+    return x
+
+
+def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=False, denoise=True, device="cuda",
+                           grid_mask=None, native_rng=False, seed=42):
+    """Returns `dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None)` ->
+    (samples, number of network evaluations), the signature of pc_sampler.
+
+    The prior is pc_sampler's (sde.prior_sampling(shape) * grid_mask). With `partial`, channel c is replaced before step 0
+    (alpha, sigma of label N-1) and after every step k but the last whose label n_k has N-1-n_k < freeze_iters (alpha,
+    sigma of n_{k+1}), with fresh per-sample noise; the x0 history keeps the network's prediction. Paths: on CUDA with
+    `native_rng` and a native ScoreNet the whole loop runs in the library (mdb_solver_run, Philox noise keyed by
+    seed + rank and step); other CUDA states run model + mdb_solver_update per step with torch.randn_like noise; CPU
+    tensors run the eager fp32 update (_solver_update_eager), which is the kernel's oracle."""
+    labels, table = dpm_solver_schedule(sde, n_steps, stochastic, denoise)
+    rows32 = table.astype(np.float32)
+    steps_c = _solver_steps_c(table)
+    K_eff = len(labels) - 1
+    N = sde.N
+    abar_T = float(sde.alphas_cumprod[N - 1])
+    a_T, s_T = (float(np.float32(v)) for v in (np.sqrt(abar_T), np.sqrt(1.0 - abar_T)))  # alpha, sigma of label N - 1
+
+    def dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None):
+        with torch.no_grad():
+            if freeze_iters is None:
+                freeze_iters = N + 10
+            c = partial_channel
+            B = shape[0]
+            x = sde.prior_sampling(shape).to(device)
+            assert x.dim() == 5
+            x = (x * grid_mask).contiguous()
+            V = x[0, 0].numel()
+            if grid_mask.numel() != V:
+                raise ValueError("dpm_solver: grid_mask must hold one value per voxel")
+            mask_v = grid_mask.to(device=x.device, dtype=torch.float32).reshape(x.shape[2:]).contiguous()
+            cond, cond_until = None, 0
+            if partial is not None:
+                assert partial.dim() == 5
+                cond = _Cond(sde, partial.to(x.device), partial_mask.to(x.device), c, None, B)
+                z = torch.randn_like(x[:, c])
+                x[:, c] = _replace_channel(x[:, c], cond.partial, cond.pmask, mask_v, a_T, s_T, z)
+                cond_until = sum(1 for k in range(K_eff - 1) if N - 1 - labels[k] < freeze_iters)
+            x0_hist = torch.empty_like(x)
+            net = _native_net(model)
+            if x.is_cuda and native_rng and net is not None:
+                net._ensure_engine(B, x.device)
+                net.sync_parameters()
+                net._frozen = True  # nobody edits the weights inside the loop: skip per-step change detection
+                try:
+                    _native_solver_loop(net, x, x0_hist, mask_v.reshape(-1), steps_c, seed + _rank(), cond=cond,
+                                        cond_until=cond_until)
+                finally:
+                    net._frozen = False
+                return inverse_scaler(x), K_eff
+            for k in range(K_eff):
+                eps_out = model(x, torch.full((B,), float(labels[k]), device=x.device))
+                z = torch.randn_like(x) if rows32[k, 6] != 0 else None
+                ck = cond if k < cond_until else None
+                z2 = torch.randn_like(x[:, c]).contiguous() if ck is not None else None
+                if x.is_cuda:
+                    _solver_update(eps_out.float().contiguous(), x, x0_hist, mask_v.reshape(-1), steps_c[k], z, ck, z2)
+                else:
+                    _solver_update_eager(eps_out.float(), x, x0_hist, mask_v, rows32[k], z, ck, z2)
+            return inverse_scaler(x), K_eff
+
+    return dpm_solver_sampler
