@@ -355,6 +355,35 @@ int mdb_emd_matrix(const float* A, int nA, const float* B, int nB, int N, float 
 int mdb_pflow_drift_div(const float* x, const float* e, const float* h, const float* g, const float* mask, float beta, float std,
                         float* drift, double* div, int batch, int channels, long long voxels, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Single-view visibility for partial DMTets (nvdiffrec/lib/render/render.py:335-407, fit_singleview.py:783-827): a
+ * first-layer depth / face-id rasterization and the reference's visible-tet test on top of it. Every product, sum and
+ * quotient is rounded on its own (no FMA contraction), so a float32 restatement reproduces both bit for bit.
+ */
+/* Rasterizes n_jobs (mesh, view) jobs into res x res buffers. Meshes are packed like mdb_marching_tets_extract's output:
+ * verts fp32 [V][3], faces int64 [F][3] local to their mesh, vert_off device int64 [n_meshes], face_off device int64
+ * [n_meshes + 1]. job_mesh device int32 [n_jobs] (mesh of each job, not range-checked here), mvp device fp32 [n_jobs][16]
+ * (row-major). Per vertex clip = mvp [x, y, z, 1] (each row ((m0 x + m1 y) + m2 z) + m3); a face with a vertex at
+ * w <= 0 is not drawn and is counted in n_behind (device int32 [n_jobs], overwritten); so is a face with a non-finite
+ * screen coordinate or a zero area, uncounted. Screen X = (x / w * 0.5 + 0.5) * res (likewise Y); pixel (r, c) has its
+ * centre at (c + 0.5, r + 0.5), so row 0 is clip y = -1. A pixel is covered when its centre lies in the face's bounding
+ * box and every edge function has the sign of the area or is zero (both windings); depth = z / w interpolated with the
+ * edge-function weights, dropped outside [-1, 1]. The nearest fragment wins, ties to the lower face index (a 64-bit
+ * atomicMin on (depth key, face)). depth fp32 [n_jobs][res][res] (100 where empty), face_id int32 (-1 where empty; else
+ * the face's index within its mesh). scratch: device uint64 [n_jobs][res][res]. */
+int mdb_raster_depth(const float* verts, const long long* faces, const long long* vert_off, const long long* face_off,
+                     const int* job_mesh, const float* mvp, int n_jobs, int res, unsigned long long* scratch, float* depth,
+                     int* face_id, int* n_behind, void* stream);
+/* For every tet t and job j: centre c = (((p0 + p1) + p2) + p3) * 0.25 over pos + job_mesh[j] * pos_stride (fp32 [Nv][3];
+ * pos_stride in floats, 0 = shared), h = mvp c, n = h.xyz / h.w, q = rint((n * 0.5 + 0.5) * (res - 1)) (half to even).
+ * visible[j][t] = 1 when q is in [0, res - 1] in all three components and, over rows q.y +- 7 and columns q.x +- 7
+ * clipped to the image, the minimum depth is >= n.z or every pixel is empty. rast[j][t] = 1 when
+ * face_to_tet[face_off[job_mesh[j]] + id] == t for an id in the job's face_id buffer. tets device int32 [n_tets][4]
+ * (16-byte aligned); depth / face_id as mdb_raster_depth wrote them; visible, rast uint8 [n_jobs][n_tets], overwritten. */
+int mdb_visible_tets(const float* pos, long long pos_stride, const int* tets, int n_tets, const long long* face_to_tet,
+                     const long long* face_off, const int* job_mesh, const float* mvp, int n_jobs, int res, const float* depth,
+                     const int* face_id, unsigned char* visible, unsigned char* rast, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -115,6 +115,8 @@ SIGNATURES = {
     "mdb_chamfer_matrix": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp]),
     "mdb_emd_matrix": (_i, [_vp, _i, _vp, _i, _i, _f, _vp, _vp, _vp]),
     "mdb_pflow_drift_div": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _i, _i, _ll, _vp]),
+    "mdb_raster_depth": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "mdb_visible_tets": (_i, [_vp, _ll, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
 }
 
 

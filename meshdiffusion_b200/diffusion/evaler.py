@@ -1,4 +1,5 @@
-"""`--mode=uncond_gen` / `--mode=cond_gen` drivers (reference: lib/diffusion/evaler.py:14-60, 134-211).
+"""`--mode=uncond_gen` / `--mode=cond_gen` drivers (reference: lib/diffusion/evaler.py:14-60, 134-211), and
+`--mode=make_partial`, which makes `cond_gen`'s partial DMTets from dataset grids (nvdiffrec/fit_singleview.py:783-827).
 
 One process per GPU: under torchrun every rank loads the checkpoint, draws `eval.batch_size` samples with its own
 seed and writes `<eval_dir>/<rank>.npy` (rank 0 writes `0.npy`, the reference's single-process file name); no
@@ -90,3 +91,55 @@ def cond_gen(config, save_fname=None):
     out = os.path.join(eval_dir, f"{save_fname}.npy")
     np.save(out, samples.cpu().numpy())
     return out
+
+
+# second_stage_deform of nvdiffrec/configs/res{64,128}.json: the deformation scale the fitted grids were made with
+_DEFORM_SCALE = {64: 3.0, 128: 1.5}
+
+
+def make_partial(config):
+    """`--mode=make_partial`: the partial DMTets `cond_gen` takes (`eval.partial_dmtet_path`), made from the shapes
+    `config.data.meta_path` / `filter_meta_path` select (the reference set of `eval_metrics`) and the validation views
+    `eval.partial_views` (default (0,)) at `eval.partial_res` (default 1000) pixels square.
+
+    Writes `<eval_dir>/partial/<shape:06d>_view<v:02d>.pt` (the reference's `tets/dmtet.pt` layout; `shape` is the index
+    in the selected list) and an index of the files it wrote: `index.json` in a single process, `index_<rank>.json` per
+    rank under torchrun, where rank r takes the shapes i = r (mod world size). Returns the index entries."""
+    import json
+
+    from ..dataset.shapenet_dmtet_dataset import ShapeNetDMTetDataset
+    from ..geometry.singleview import PartialDMTets
+    from .trainer import _path_or_none
+    device = config.device
+    R = config.data.image_size
+    rank, world = _rank(), int(os.environ.get("WORLD_SIZE", "1"))
+    views = config.eval.get("partial_views", (0,))
+    views = (views,) if isinstance(views, int) else tuple(views)
+    res = int(config.eval.get("partial_res", 1000))
+    mesh_scale = float(config.eval.get("mesh_scale", 1.1))
+    deform_scale = float(config.eval.get("deform_scale", _DEFORM_SCALE.get(R, 3.0)))
+    mask = load_grid_mask(R, device).view(1, 1, R, R, R)
+    ds = ShapeNetDMTetDataset(config.data.meta_path, mask.cpu(), filter_meta_path=_path_or_none(config.data.get("filter_meta_path", None)),
+                              extension=config.data.get("extension", "pt"), aug=False, normalize_sdf=False)
+    if len(ds) == 0:
+        raise ValueError(f"the shape list {config.data.meta_path} selects no shapes")
+    out_dir = os.path.join(config.eval.eval_dir, "partial")
+    os.makedirs(out_dir, exist_ok=True)
+    make = PartialDMTets(R, views, res, mesh_scale, deform_scale, device)
+    mine = list(range(rank, len(ds), world))
+    index = []
+    for c0 in range(0, len(mine), make.max_batch):
+        ids = mine[c0:c0 + make.max_batch]
+        grids = torch.stack([ds[i] for i in ids]).to(device)
+        for i, row in zip(ids, make(grids)):
+            for k, (d, n_vis_tets) in enumerate(row):
+                name = f"{i:06d}_view{views[k]:02d}.pt"
+                torch.save(d, os.path.join(out_dir, name))
+                index.append({"file": name, "shape": i, "source": ds.fpath_list[i].rstrip(), "view": views[k],
+                              "mvp": make.mvps[k].tolist(), "res": res, "visible_tets": n_vis_tets,
+                              "visible_verts": int(d["vis"].sum()), "visible_and_rast_verts": int(d["vis_rast"].sum())})
+        logging.info("make_partial: rank %d, %d / %d shapes", rank, min(c0 + make.max_batch, len(mine)), len(mine))
+    with open(os.path.join(out_dir, "index.json" if world == 1 else f"index_{rank}.json"), "w") as fh:
+        json.dump({"resolution": R, "views": list(views), "res": res, "mesh_scale": mesh_scale,
+                   "deform_scale": deform_scale, "files": index}, fh, indent=1)
+    return index

@@ -2,8 +2,9 @@
 
 * `partial_dmtet_from_visibility` -- the `tets/dmtet.pt` dictionary that `--mode=cond_gen` consumes
   (`config.eval.partial_dmtet_path`), i.e. the tail of nvdiffrec/fit_singleview.py:783-827: per-vertex visibility from
-  the ids of the tetrahedra a view sees. The renderer that PRODUCES those ids (nvdiffrast rasterisation + the
-  renderutils plugin) is out of scope; everything after it is here.
+  the ids of the tetrahedra a view sees. Those ids come from geometry/singleview.py (the library's first-layer depth /
+  face-id rasterizer and the reference's visible-tet test in place of the nvdiffrast rasterisation of
+  nvdiffrec/lib/render/render.py:335-407); shading and the rest of the renderer are out of scope.
 * `tets_to_3dgrid` -- data/tets_to_3dgrid.py:7-15: a fitted DMTet (`sdf` [Nv], `deform` [Nv,3]) scattered onto the
   cubic grid the diffusion model trains on (`grid_*.pt`, [4,R,R,R]).
 * the grid mask (data/get_tet_mask.py) lives in geometry/dmtet.py::grid_mask_from_tets.
