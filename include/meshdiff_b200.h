@@ -384,6 +384,41 @@ int mdb_visible_tets(const float* pos, long long pos_stride, const int* tets, in
                      const long long* face_off, const int* job_mesh, const float* mvp, int n_jobs, int res, const float* depth,
                      const int* face_id, unsigned char* visible, unsigned char* rast, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Geometry-only fit of DMTet training grids to triangle meshes (`--mode=fit_grids`; the reference fits them by rendering,
+ * nvdiffrec/fit_dmtets.py). Every product, sum and quotient is rounded on its own (no FMA contraction), so a float32
+ * restatement reproduces the flags, distances, indices and closest points bit for bit.
+ */
+/* Space carving. pts fp32 [n_pts][3] (shared by the meshes); mvp device fp32 [n_views][16] (row-major); depth / face_id
+ * [n_meshes][n_views][res][res] as mdb_raster_depth wrote them. Per vertex and view: clip = mvp [p, 1] (rows as in
+ * mdb_raster_depth), skipped unless w > 0; X = (x / w * 0.5 + 0.5) * res, Y likewise, z = z / w; skipped unless X and Y
+ * are in [0, res); pixel (floor Y, floor X). The view sees the vertex when every pixel of rows floor Y +- window and
+ * columns floor X +- window, clipped to the image, is empty (face_id < 0) or has depth > z. outside uint8
+ * [n_meshes][n_pts]: set to 1 where a view sees the vertex, left as it is elsewhere (zero it before the first call, so
+ * that views can be carved in several calls). */
+int mdb_carve_vertices(const float* pts, int n_pts, const float* mvp, int n_views, int n_meshes, int res, int window,
+                       const float* depth, const int* face_id, unsigned char* outside, void* stream);
+/* Closest point of a triangle mesh for every query point. Queries fp32 [Q][3] packed by mesh: query_off device int64
+ * [n_meshes + 1] (exclusive sums), max_queries >= the largest per-mesh count. Meshes packed as in mdb_raster_depth
+ * (verts, faces int64 local to their mesh, vert_off [n_meshes], face_off [n_meshes + 1]). Brute force over the mesh's
+ * faces by Voronoi region (Ericson, Real-Time Collision Detection 5.1.5); a degenerate face whose regions give no finite
+ * point takes the nearest of its edges ab, bc, ca. dist2 fp32 [Q] = (dx dx + dy dy) + dz dz of query - closest; face int64
+ * [Q] = the nearest face's index within its mesh, ties to the lower index; closest fp32 [Q][3]. A mesh without faces gives
+ * dist2 = +inf, face = -1 and NaN points. */
+int mdb_closest_points(const float* queries, const long long* query_off, int n_meshes, long long max_queries, const float* verts,
+                       const long long* faces, const long long* vert_off, const long long* face_off, float* dist2,
+                       long long* face, float* closest, void* stream);
+/* Nearest point of a point set for every query: queries packed as in mdb_closest_points, points fp32 [P][3] packed by
+ * point_off device int64 [n_meshes + 1]. dist2 fp32 [Q] as in mdb_closest_points; index int64 [Q] within the mesh's
+ * points, ties to the lower index; -1 (and dist2 = +inf) when the set is empty. */
+int mdb_nearest_vertex(const float* queries, const long long* query_off, int n_meshes, long long max_queries, const float* points,
+                       const long long* point_off, float* dist2, long long* index, void* stream);
+/* out fp32 [n_rows][width] (overwritten): row r = sum of src[perm[k]] (fp32 [*][width]) over k in
+ * [row_off[r], row_off[r + 1]), added in k order. With perm a stable sort of the rows' keys this is a deterministic
+ * scatter-add (no float atomics). perm, row_off device int64. */
+int mdb_segment_sum(const float* src, int width, const long long* perm, const long long* row_off, long long n_rows, float* out,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif
