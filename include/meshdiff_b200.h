@@ -383,6 +383,22 @@ int mdb_raster_depth(const float* verts, const long long* faces, const long long
 int mdb_visible_tets(const float* pos, long long pos_stride, const int* tets, int n_tets, const long long* face_to_tet,
                      const long long* face_off, const int* job_mesh, const float* mvp, int n_jobs, int res, const float* depth,
                      const int* face_id, unsigned char* visible, unsigned char* rast, void* stream);
+/* The diffuse preview image of nvdiffrec/eval.py (kd material, environment light, white background) on the face ids of an
+ * mdb_raster_depth pass at res * ssaa (ssaa in 1..4, res * ssaa <= 16384). Meshes, job_mesh and mvp as in
+ * mdb_raster_depth; v_nrm fp32 [V][3] smooth vertex normals packed like verts; campos device fp32 [n_jobs][3] (world-space
+ * camera position, the translation of the inverse model-view); face_id [n_jobs][res * ssaa][res * ssaa]. Per sub-pixel
+ * centre (c + 0.5, r + 0.5): empty -> bg; else barycentrics e_k / area made perspective-correct (b_k / w_k renormalised),
+ * interpolated position p and smooth normal, and bsdf_prepare_shading_normal with two-sided shading (safe-normalised smooth
+ * normal and view campos - p, face normal (v1 - v0) x (v2 - v0) normalised, both flipped unless face . view > 0, lerp
+ * geom + t (smooth - geom) with t = clamp(view . smooth / 0.1, 0, 1)); colour kd * max(E(n), 0) with E the 9-term real SH
+ * sum_i sh_coef[i][c] Y_i(n) (order Y00, Y1-1, Y10, Y11, Y2-2, Y2-1, Y20, Y21, Y22; sh_coef device fp32 [9][3], the SH
+ * coefficients of irradiance / pi). Per output pixel: the ssaa^2 sub-pixel colours summed in row-major order, divided by
+ * ssaa^2, and each channel encoded as the number of srgb_thresholds (device fp32 [255], ascending) it reaches. kd, bg:
+ * device fp32 [3], linear. rgb uint8 [n_jobs][res][res][3], row 0 = buffer row 0. Every step rounded on its own. */
+int mdb_render_shade(const float* verts, const float* v_nrm, const long long* faces, const long long* vert_off,
+                     const long long* face_off, const int* job_mesh, const float* mvp, const float* campos, int n_jobs, int res,
+                     int ssaa, const int* face_id, const float* sh_coef, const float* kd, const float* bg,
+                     const float* srgb_thresholds, unsigned char* rgb, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Geometry-only fit of DMTet training grids to triangle meshes (`--mode=fit_grids`; the reference fits them by rendering,

@@ -117,6 +117,7 @@ SIGNATURES = {
     "mdb_pflow_drift_div": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _i, _i, _ll, _vp]),
     "mdb_raster_depth": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "mdb_visible_tets": (_i, [_vp, _ll, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "mdb_render_shade": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mdb_carve_vertices": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "mdb_closest_points": (_i, [_vp, _vp, _i, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mdb_nearest_vertex": (_i, [_vp, _vp, _i, _ll, _vp, _vp, _vp, _vp, _vp]),

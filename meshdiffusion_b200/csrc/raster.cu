@@ -7,6 +7,10 @@
 //   atomicMin on (depth key, face index): the result does not depend on scheduling.
 // * mdb_visible_tets: the reference's visible-tet test (a tet centre in front of the minimum depth, or over empty pixels,
 //   of the 15 x 15 window around its pixel) fused into one pass, plus the flags of the tets that own a rasterized face.
+// * mdb_render_shade: the diffuse, environment-lit preview of nvdiffrec/eval.py on the face ids of a supersampled
+//   mdb_raster_depth pass: perspective-correct interpolation, nvdiffrec's two-sided shading normal, 9-term SH irradiance,
+//   a box resolve in linear space and an sRGB encode by threshold table. Rounded step by step like the rasterizer
+//   (oracle/render_oracle.py).
 #include "../../include/meshdiff_b200.h"
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -193,6 +197,151 @@ __global__ void rast_tets_kernel(const int* __restrict__ face_id, long long pixe
   }
 }
 
+// ---- shading ---------------------------------------------------------------------------------------------------------
+
+constexpr int kShadeThreads = 256;
+constexpr int kShadeJobChunk = 4096;  // jobs per launch (blockIdx.y)
+constexpr int kSrgbLevels = 255;      // thresholds between the 256 output codes
+constexpr float kNormalThreshold = 0.1f;  // NORMAL_THRESHOLD of nvdiffrec's renderutils (bsdf.py, normal.cu)
+
+struct V3 { float x, y, z; };
+
+__device__ __forceinline__ V3 v3_load(const float* p) { return {p[0], p[1], p[2]}; }
+__device__ __forceinline__ V3 v3_sub(V3 a, V3 b) { return {__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z)}; }
+__device__ __forceinline__ V3 v3_neg(V3 a) { return {-a.x, -a.y, -a.z}; }
+__device__ __forceinline__ float v3_dot(V3 a, V3 b) {
+  return __fadd_rn(__fadd_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)), __fmul_rn(a.z, b.z));
+}
+__device__ __forceinline__ V3 v3_cross(V3 a, V3 b) {
+  return {__fsub_rn(__fmul_rn(a.y, b.z), __fmul_rn(a.z, b.y)), __fsub_rn(__fmul_rn(a.z, b.x), __fmul_rn(a.x, b.z)),
+          __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x))};
+}
+// x / sqrt(max(x . x, 1e-20)): nvdiffrec's safe_normalize
+__device__ __forceinline__ V3 v3_safe_normalize(V3 a) {
+  const float l = __fsqrt_rn(fmaxf(v3_dot(a, a), 1e-20f));
+  return {__fdiv_rn(a.x, l), __fdiv_rn(a.y, l), __fdiv_rn(a.z, l)};
+}
+// (b0 a0 + b1 a1) + b2 a2
+__device__ __forceinline__ V3 v3_interp(const float b[3], V3 a0, V3 a1, V3 a2) {
+  return {__fadd_rn(__fadd_rn(__fmul_rn(b[0], a0.x), __fmul_rn(b[1], a1.x)), __fmul_rn(b[2], a2.x)),
+          __fadd_rn(__fadd_rn(__fmul_rn(b[0], a0.y), __fmul_rn(b[1], a1.y)), __fmul_rn(b[2], a2.y)),
+          __fadd_rn(__fadd_rn(__fmul_rn(b[0], a0.z), __fmul_rn(b[1], a1.z)), __fmul_rn(b[2], a2.z))};
+}
+
+// Linear RGB of face f at supersampled pixel centre (px, py); false when the face is not drawn (then the pixel is
+// background, as it would be had the rasterizer not drawn it).
+__device__ __forceinline__ bool shade_fragment(const float* __restrict__ v, const float* __restrict__ vn,
+                                               const long long* __restrict__ f, const float* m, float fres, float px, float py,
+                                               V3 cam, const float* sh, const float* kd, float col[3]) {
+  Tri t;
+  bool behind;
+  if (!setup_tri(v, f, m, fres, t, behind)) return false;
+  // barycentrics from the edge functions, then perspective-correct with each vertex's clip w
+  const float e[3] = {edge_fn(t.x[1], t.y[1], t.x[2], t.y[2], px, py), edge_fn(t.x[2], t.y[2], t.x[0], t.y[0], px, py),
+                      edge_fn(t.x[0], t.y[0], t.x[1], t.y[1], px, py)};
+  V3 p[3], n[3];
+  float q[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    p[k] = v3_load(v + 3 * f[k]);
+    n[k] = v3_load(vn + 3 * f[k]);
+    q[k] = __fdiv_rn(__fdiv_rn(e[k], t.area), mvp_row(m + 12, p[k].x, p[k].y, p[k].z));
+  }
+  const float qs = __fadd_rn(__fadd_rn(q[0], q[1]), q[2]);
+  const float b[3] = {__fdiv_rn(q[0], qs), __fdiv_rn(q[1], qs), __fdiv_rn(q[2], qs)};
+  const V3 pos = v3_interp(b, p[0], p[1], p[2]);
+  // bsdf_prepare_shading_normal: two-sided, no normal map, no tangents
+  V3 smooth = v3_safe_normalize(v3_interp(b, n[0], n[1], n[2]));
+  const V3 view = v3_safe_normalize(v3_sub(cam, pos));
+  V3 geom = v3_safe_normalize(v3_cross(v3_sub(p[1], p[0]), v3_sub(p[2], p[0])));
+  if (!(v3_dot(geom, view) > 0.f)) {
+    smooth = v3_neg(smooth);
+    geom = v3_neg(geom);
+  }
+  const float tb = fminf(fmaxf(__fdiv_rn(v3_dot(view, smooth), kNormalThreshold), 0.f), 1.f);
+  const V3 s = v3_sub(smooth, geom);
+  const float x = __fadd_rn(geom.x, __fmul_rn(tb, s.x)), y = __fadd_rn(geom.y, __fmul_rn(tb, s.y));
+  const float z = __fadd_rn(geom.z, __fmul_rn(tb, s.z));
+  // real SH basis, l <= 2, in the order Y00, Y1-1, Y10, Y11, Y2-2, Y2-1, Y20, Y21, Y22
+  const float Y[9] = {0.28209479177387814f,
+                      __fmul_rn(0.4886025119029199f, y),
+                      __fmul_rn(0.4886025119029199f, z),
+                      __fmul_rn(0.4886025119029199f, x),
+                      __fmul_rn(__fmul_rn(1.0925484305920792f, x), y),
+                      __fmul_rn(__fmul_rn(1.0925484305920792f, y), z),
+                      __fmul_rn(0.31539156525252005f, __fsub_rn(__fmul_rn(3.f, __fmul_rn(z, z)), 1.f)),
+                      __fmul_rn(__fmul_rn(1.0925484305920792f, x), z),
+                      __fmul_rn(0.5462742152960396f, __fsub_rn(__fmul_rn(x, x), __fmul_rn(y, y)))};
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    float E = __fmul_rn(sh[c], Y[0]);
+#pragma unroll
+    for (int i = 1; i < 9; ++i) E = __fadd_rn(E, __fmul_rn(sh[3 * i + c], Y[i]));
+    col[c] = __fmul_rn(kd[c], fmaxf(E, 0.f));
+  }
+  return true;
+}
+
+// One thread per (output pixel, job): shade the ssaa x ssaa sub-pixels, average them in row-major order, encode to sRGB.
+__global__ void __launch_bounds__(kShadeThreads) shade_kernel(const float* __restrict__ verts, const float* __restrict__ v_nrm,
+                                                              const long long* __restrict__ faces, const long long* __restrict__ vert_off,
+                                                              const long long* __restrict__ face_off, const int* __restrict__ job_mesh,
+                                                              const float* __restrict__ mvps, const float* __restrict__ campos, int job0,
+                                                              int res, int ssaa, const int* __restrict__ face_id,
+                                                              const float* __restrict__ sh_coef, const float* __restrict__ kd,
+                                                              const float* __restrict__ bg, const float* __restrict__ thresholds,
+                                                              unsigned char* __restrict__ rgb) {
+  __shared__ float s_thr[kSrgbLevels], s_sh[27], s_kd[3], s_bg[3];
+  for (int i = threadIdx.x; i < kSrgbLevels; i += blockDim.x) s_thr[i] = thresholds[i];
+  if (threadIdx.x < 27) s_sh[threadIdx.x] = sh_coef[threadIdx.x];
+  if (threadIdx.x < 3) {
+    s_kd[threadIdx.x] = kd[threadIdx.x];
+    s_bg[threadIdx.x] = bg[threadIdx.x];
+  }
+  __syncthreads();
+  const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= (long long)res * res) return;
+  const int job = job0 + blockIdx.y;
+  const int r = (int)(pix / res), c = (int)(pix % res);
+  const int mesh = job_mesh[job];
+  const long long* f = faces + 3 * face_off[mesh];
+  const float* v = verts + 3 * vert_off[mesh];
+  const float* vn = v_nrm + 3 * vert_off[mesh];
+  float m[16];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) m[i] = mvps[16 * job + i];
+  const V3 cam = v3_load(campos + 3 * job);
+  const int sres = res * ssaa;
+  const float fres = (float)sres;
+  const int* id = face_id + (long long)job * sres * sres;
+  float acc[3] = {0.f, 0.f, 0.f};
+  for (int a = 0; a < ssaa; ++a)
+    for (int b = 0; b < ssaa; ++b) {
+      const int sr = r * ssaa + a, sc = c * ssaa + b;
+      const int fi = id[(long long)sr * sres + sc];
+      float col[3];
+      if (fi < 0 || !shade_fragment(v, vn, f + 3LL * fi, m, fres, (float)sc + 0.5f, (float)sr + 0.5f, cam, s_sh, s_kd, col)) {
+        col[0] = s_bg[0];
+        col[1] = s_bg[1];
+        col[2] = s_bg[2];
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) acc[k] = __fadd_rn(acc[k], col[k]);
+    }
+  const float n_sub = (float)(ssaa * ssaa);
+  unsigned char* out = rgb + ((long long)job * res * res + pix) * 3;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float x = __fdiv_rn(acc[k], n_sub);
+    // the number of thresholds x reaches (the table is ascending; a NaN reaches none)
+    int code = 0;
+#pragma unroll
+    for (int step = 128; step > 0; step >>= 1)
+      if (code + step <= kSrgbLevels && x >= s_thr[code + step - 1]) code += step;
+    out[k] = (unsigned char)code;
+  }
+}
+
 int sm_count(int* n) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
@@ -248,6 +397,25 @@ int mdb_visible_tets(const float* pos, long long pos_stride, const int* tets, in
   const int gx = (int)std::min<long long>((pixels + 255) / 256, std::max(1, (8 * sms + n_jobs - 1) / n_jobs));
   rast_tets_kernel<<<dim3((unsigned)gx, (unsigned)n_jobs), 256, 0, s>>>(face_id, pixels, job_mesh, face_to_tet, face_off, n_tets, rast);
   return check_launch("mdb_visible_tets (rasterized tets)");
+}
+
+int mdb_render_shade(const float* verts, const float* v_nrm, const long long* faces, const long long* vert_off,
+                     const long long* face_off, const int* job_mesh, const float* mvp, const float* campos, int n_jobs, int res,
+                     int ssaa, const int* face_id, const float* sh_coef, const float* kd, const float* bg,
+                     const float* srgb_thresholds, unsigned char* rgb, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  if (check_sizes("mdb_render_shade", n_jobs, res)) return 1;
+  if (ssaa < 1 || ssaa > 4) return fail("mdb_render_shade: ssaa must be in [1, 4]");
+  if ((long long)res * ssaa > 16384) return fail("mdb_render_shade: res * ssaa must be at most 16384");
+  if (n_jobs == 0) return 0;
+  const unsigned gx = (unsigned)(((long long)res * res + kShadeThreads - 1) / kShadeThreads);
+  for (int j0 = 0; j0 < n_jobs; j0 += kShadeJobChunk) {
+    const int nj = std::min(kShadeJobChunk, n_jobs - j0);
+    shade_kernel<<<dim3(gx, (unsigned)nj), kShadeThreads, 0, s>>>(verts, v_nrm, faces, vert_off, face_off, job_mesh, mvp, campos, j0,
+                                                                  res, ssaa, face_id, sh_coef, kd, bg, srgb_thresholds, rgb);
+    if (check_launch("mdb_render_shade")) return 1;
+  }
+  return 0;
 }
 
 }  // extern "C"
