@@ -435,6 +435,27 @@ int mdb_nearest_vertex(const float* queries, const long long* query_off, int n_m
 int mdb_segment_sum(const float* src, int width, const long long* perm, const long long* row_off, long long n_rows, float* out,
                     void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Shape interpolation (`--mode=uncond_gen_interp`). Replaces `slerp` of lib/diffusion/evaler.py:63-71 (which the
+ * reference's uncond_gen_interp, :73-130, applies to two prior noises): spherical interpolation over the whole tensor, no
+ * grid mask.
+ */
+/* Number of reduction chunks per pair (the second extent of `partial`). */
+int mdb_slerp_chunks(void);
+/* P = pairs endpoint pairs za, zb fp32 [P][n]; alphas: HOST fp64 [frames] (any finite values; frames >= 2).
+ * Phase 1: pair p is cut into mdb_slerp_chunks() contiguous ranges of ceil(n / chunks) elements whatever P; each range's
+ *   fp64 sums of a*b, a*a, b*b (per thread in element order, then a fixed block tree) -> partial [P][chunks][3] (device
+ *   scratch, overwritten).
+ * Phase 2: the chunk sums in a fixed tree -> sums fp64 [P][3] = (a.b, a.a, b.b); bitwise reproducible and independent of P.
+ *   In fp64: cos t = a.b / sqrt(a.a b.b) clamped to [-1, 1], t = acos, w_a = sin((1 - alpha) t) / sin t,
+ *   w_b = sin(alpha t) / sin t; when a.a or b.b is 0 or sin t < 1e-6 (parallel or antiparallel endpoints) the weights
+ *   are lerp's (1 - alpha, alpha). Rounded to fp32 -> coef [P][frames][2] (8-byte aligned). alpha = 0 and 1 give exactly
+ *   (1, 0) and (0, 1).
+ * Phase 3: out fp32 [P][frames][n], frame f of pair p = fl(fl(w_a a) + fl(w_b b)) per element, each operation rounded on
+ *   its own. The call only enqueues work. */
+int mdb_slerp_frames(const float* za, const float* zb, long long n, int pairs, const double* alphas, int frames,
+                     double* partial, double* sums, float* coef, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,7 +7,8 @@ path: one native U-Net evaluation and ONE fused update kernel per step (score sc
 both grid-mask multiplies), with the state resident in HBM and no host synchronisation inside the loop. Other
 registered predictors / correctors use the same native network through `get_score_fn` with a few torch
 elementwise ops around it. `method='dpm_solver'` (no working reference counterpart) is the few-step DPM-Solver++(2M)
-sampler at the end of this file.
+sampler at the end of this file; `get_dpm_solver_inverter` runs its ODE form backwards (a grid's latent, for
+`--mode=uncond_gen_interp`).
 """
 import abc
 import ctypes
@@ -486,6 +487,12 @@ def dpm_solver_schedule(sde, n_steps, stochastic=False, denoise=True):
         if not labels or n != labels[-1]:
             labels.append(n)
     assert labels[0] == N - 1 and labels[-1] == 0 and all(a > b for a, b in zip(labels, labels[1:]))
+    return labels, _solver_table(alpha, sigma, lam, labels, stochastic, denoise)
+
+
+def _solver_table(alpha, sigma, lam, labels, stochastic=False, denoise=True):
+    """float64 step table of DPM-Solver++(2M) along `labels` (any direction): row k moves x from labels[k] to
+    labels[k + 1] with h = lambda_t - lambda_s; row 0 is first order."""
     K_eff = len(labels) - 1
     table = np.zeros((K_eff, 9), dtype=np.float64)
     h_prev = None
@@ -505,7 +512,21 @@ def dpm_solver_schedule(sde, n_steps, stochastic=False, denoise=True):
             c_0, c_1 = b * (1.0 + 1.0 / (2.0 * r)), -b / (2.0 * r)
         table[k] = (s, sigma[s], 1.0 / alpha[s], c_x, c_0, c_1, c_z, alpha[t], sigma[t])
         h_prev = h
-    return labels, table
+    return table
+
+
+def dpm_solver_inversion_schedule(sde, n_steps):
+    """Labels and step table of the inverse map: the ODE form of DPM-Solver++(2M) run backwards over the labels of
+    `dpm_solver_schedule(sde, n_steps)`, from label 0 to N - 1. The rows use the same float64 formula with h < 0; row 0
+    is first order and c_z = 0 (the cond fields are not used). K_eff network evaluations map a grid at label 0 (what the
+    sampler returns) to the latent at label N - 1 that the sampler with the same K maps back to it, up to the
+    discretisation error of both directions. Returns (labels, table)."""
+    labels, _ = dpm_solver_schedule(sde, n_steps)
+    labels = labels[::-1]
+    abar = sde.alphas_cumprod.detach().to("cpu", torch.float64).numpy()
+    alpha, sigma = np.sqrt(abar), np.sqrt(1.0 - abar)
+    lam = np.log(alpha) - np.log(sigma)
+    return labels, _solver_table(alpha, sigma, lam, labels)
 
 
 def _solver_steps_c(table):
@@ -575,10 +596,11 @@ def _native_solver_loop(net, x, x0_hist, mask_flat, steps_c, seed, step0=0, n=No
 
 def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=False, denoise=True, device="cuda",
                            grid_mask=None, native_rng=False, seed=42):
-    """Returns `dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None)` ->
-    (samples, number of network evaluations), the signature of pc_sampler.
+    """Returns `dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None)`
+    -> (samples, number of network evaluations), the signature of pc_sampler.
 
-    The prior is pc_sampler's (sde.prior_sampling(shape) * grid_mask). With `partial`, channel c is replaced before step 0
+    The prior is pc_sampler's (sde.prior_sampling(shape) * grid_mask), or x0 * grid_mask when `x0` (shape `shape`) is
+    given: no prior is drawn then. With `partial`, channel c is replaced before step 0
     (alpha, sigma of label N-1) and after every step k but the last whose label n_k has N-1-n_k < freeze_iters (alpha,
     sigma of n_{k+1}), with fresh per-sample noise; the x0 history keeps the network's prediction. Paths: on CUDA with
     `native_rng` and a native ScoreNet the whole loop runs in the library (mdb_solver_run, Philox noise keyed by
@@ -592,13 +614,15 @@ def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=Fa
     abar_T = float(sde.alphas_cumprod[N - 1])
     a_T, s_T = (float(np.float32(v)) for v in (np.sqrt(abar_T), np.sqrt(1.0 - abar_T)))  # alpha, sigma of label N - 1
 
-    def dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None):
+    def dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None):
         with torch.no_grad():
             if freeze_iters is None:
                 freeze_iters = N + 10
             c = partial_channel
             B = shape[0]
-            x = sde.prior_sampling(shape).to(device)
+            if x0 is not None and tuple(x0.shape) != tuple(shape):
+                raise ValueError(f"dpm_solver: x0 has shape {tuple(x0.shape)}, the sampler {tuple(shape)}")
+            x = sde.prior_sampling(shape).to(device) if x0 is None else x0.to(device=device, dtype=torch.float32)
             assert x.dim() == 5
             x = (x * grid_mask).contiguous()
             V = x[0, 0].numel()
@@ -636,3 +660,48 @@ def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=Fa
             return inverse_scaler(x), K_eff
 
     return dpm_solver_sampler
+
+
+def get_dpm_solver_inverter(sde, shape, n_steps=25, grid_mask=None, device="cuda"):
+    """Returns `invert(model, x) -> (z, number of network evaluations)`: the latent at label N - 1 of grids x (shape
+    `shape`), taken as the state at label 0 after the grid mask is applied, by the ODE form of DPM-Solver++(2M) run
+    backwards (dpm_solver_inversion_schedule). The dpm_solver sampler with the same `n_steps`, started from z
+    (x0=z), maps it back to x up to discretisation error. No noise is drawn. Paths: a native ScoreNet on CUDA runs the
+    whole loop in the library (mdb_solver_run); other CUDA models run model + mdb_solver_update per step; CPU tensors run
+    the eager fp32 update."""
+    labels, table = dpm_solver_inversion_schedule(sde, n_steps)
+    rows32 = table.astype(np.float32)
+    steps_c = _solver_steps_c(table)
+    K_eff = len(labels) - 1
+
+    def invert(model, x):
+        with torch.no_grad():
+            if tuple(x.shape) != tuple(shape):
+                raise ValueError(f"dpm_solver inversion: x has shape {tuple(x.shape)}, expected {tuple(shape)}")
+            B = shape[0]
+            x = x.to(device=device, dtype=torch.float32)
+            V = x[0, 0].numel()
+            if grid_mask.numel() != V:
+                raise ValueError("dpm_solver inversion: grid_mask must hold one value per voxel")
+            mask_v = grid_mask.to(device=x.device, dtype=torch.float32).reshape(x.shape[2:]).contiguous()
+            x = (x * mask_v).contiguous()
+            x0_hist = torch.empty_like(x)
+            net = _native_net(model)
+            if x.is_cuda and net is not None:
+                net._ensure_engine(B, x.device)
+                net.sync_parameters()
+                net._frozen = True  # nobody edits the weights inside the loop: skip per-step change detection
+                try:
+                    _native_solver_loop(net, x, x0_hist, mask_v.reshape(-1), steps_c, 0)
+                finally:
+                    net._frozen = False
+                return x, K_eff
+            for k in range(K_eff):
+                eps_out = model(x, torch.full((B,), float(labels[k]), device=x.device))
+                if x.is_cuda:
+                    _solver_update(eps_out.float().contiguous(), x, x0_hist, mask_v.reshape(-1), steps_c[k])
+                else:
+                    _solver_update_eager(eps_out.float(), x, x0_hist, mask_v, rows32[k])
+            return x, K_eff
+
+    return invert

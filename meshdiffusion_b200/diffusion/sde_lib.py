@@ -32,8 +32,8 @@ class VPSDE:
         log_mean_coeff = -0.25 * t ** 2 * (self.beta_1 - self.beta_0) - 0.5 * t * self.beta_0
         return torch.exp(log_mean_coeff[:, None, None, None, None]) * x, torch.sqrt(1.0 - torch.exp(2.0 * log_mean_coeff))
 
-    def prior_sampling(self, shape):
-        return torch.randn(*shape)
+    def prior_sampling(self, shape, generator=None):
+        return torch.randn(*shape, generator=generator)
 
     def prior_logp(self, z):
         n = np.prod(z.shape[1:])
