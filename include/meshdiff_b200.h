@@ -333,6 +333,16 @@ int mdb_mesh_sample_points(const float* verts, const long long* faces, const lon
  * CD(X, Y) and CD(Y, X) are bitwise equal. B == NULL: self matrix of A (nB, M ignored), only i < j computed and mirrored,
  * diagonal exactly 0. The N + M per-point minima of a pair live in shared memory: N + M up to about 50 000 points. */
 int mdb_chamfer_matrix(const float* A, int nA, int N, const float* B, int nB, int M, double* out, void* stream);
+/* Paired Chamfer distances for shape completion. clouds fp32 [n_clouds][N][3] (one size N); pairs: DEVICE int32 [P][2] of
+ * cloud indices (a, b). Per pair p, one CTA computes, with mdb_chamfer_matrix's distance, minima and fixed-order sums:
+ *   cd[p]      = CD(clouds[a], clouds[b]), bitwise mdb_chamfer_matrix's entry for the same two clouds;
+ *   mean_ab[p] = mean over x in a of min over y in b of d (the a->b half of cd[p]);
+ *   max_ab[p]  = max over x in a of min over y in b of d (fp32; sqrt of it is the one-sided Hausdorff distance a->b).
+ * Bitwise reproducible; an entry does not depend on the other pairs of the launch. Callers check the list on the host:
+ * a pair with a == b or an index outside [0, n_clouds) is not an error here but gets NaN in all three outputs. 2N
+ * per-point minima live in shared memory, as in mdb_chamfer_matrix. The call only enqueues work. */
+int mdb_chamfer_pairs(const float* clouds, int n_clouds, int N, const int* pairs, int P, double* cd, double* mean_ab,
+                      float* max_ab, void* stream);
 /* out[i][j] = EMD(A_i, B_j) fp64 [nA][nB] for A fp32 [nA][N][3], B fp32 [nB][N][3] (equal sizes):
  * EMD(X, Y) = min over bijections pi of (1/N) sum_i |x_i - y_pi(i)| (Euclidean, not squared), with
  * |d| = sqrt((dx*dx + dy*dy) + dz*dz) in fp32, each operation rounded. Forward auction with epsilon-scaling, one CTA per

@@ -113,6 +113,7 @@ SIGNATURES = {
     "mdb_marching_tets_backward": (_i, [_vp, _vp, _ll, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mdb_mesh_sample_points": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _u64, _ll, _vp, _vp, _vp, _vp]),
     "mdb_chamfer_matrix": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp]),
+    "mdb_chamfer_pairs": (_i, [_vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp]),
     "mdb_emd_matrix": (_i, [_vp, _i, _vp, _i, _i, _f, _vp, _vp, _vp]),
     "mdb_pflow_drift_div": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _i, _i, _ll, _vp]),
     "mdb_raster_depth": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),

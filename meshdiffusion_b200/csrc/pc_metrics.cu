@@ -7,6 +7,10 @@
 // * mdb_chamfer_matrix: all-pairs Chamfer distance CD(X,Y) = mean_x min_y d + mean_y min_x d, d the squared Euclidean
 //   distance in fp32 on the CUDA cores. One CTA per cloud pair computes both directions in one pass; the minima are exact,
 //   so the result is bitwise reproducible, batch-invariant and symmetric in (X, Y).
+// * mdb_chamfer_pairs: the same distance over a list of (a, b) pairs of one cloud set (shape completion's block-diagonal
+//   pairs), with the a->b half and the largest a->b minimum (the squared one-sided Hausdorff distance). Both kernels run
+//   the same device function for the minima and the same fixed-order sums, so a listed pair's CD is bitwise its matrix
+//   entry.
 #include "../../include/meshdiff_b200.h"
 #include <cuda_runtime.h>
 #include <curand_kernel.h>
@@ -144,23 +148,12 @@ __device__ double fixed_order_sum(const float* v, int n, double* red) {
   return r;
 }
 
-__global__ void __launch_bounds__(kCdThreads, 2) chamfer_pair_kernel(const float* __restrict__ A, int N, const float* __restrict__ B,
-                                                                    int M, int nB, int self, double* __restrict__ out) {
-  const int i = blockIdx.y, j = blockIdx.x;
-  if (self && j < i) return;  // the mirror of (j, i)
-  if (self && j == i) {
-    if (threadIdx.x == 0) out[(long long)i * nB + j] = 0.0;
-    return;
-  }
-  extern __shared__ __align__(16) unsigned char smem[];
-  float4* ytile = reinterpret_cast<float4*>(smem);
-  double* red = reinterpret_cast<double*>(ytile + kYTile);
-  float* rowmin = reinterpret_cast<float*>(red + kCdThreads);
-  float* colmin = rowmin + round_up(N, kXChunk);
+// Row minima of X (min over y of d) -> rowmin[0..N), column minima (min over x of d) -> colmin[0..M), both in shared
+// memory (laid out by chamfer_smem_bytes), then a barrier. Every CTA of both kernels runs exactly this code, so a pair's
+// minima do not depend on which kernel or launch computed them.
+__device__ __forceinline__ void chamfer_minima(const float* __restrict__ X, int N, const float* __restrict__ Y, int M,
+                                               float4* ytile, float* rowmin, float* colmin) {
   unsigned* colbits = reinterpret_cast<unsigned*>(colmin);
-
-  const float* X = A + (long long)i * N * 3;
-  const float* Y = B + (long long)j * M * 3;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, xl = lane % kXL, yl = lane / kXL;
   const float kNaN = __int_as_float(0x7fc00000), kInf = __int_as_float(0x7f800000);
   const int Mt = (int)round_up(M, kYTile);
@@ -220,12 +213,81 @@ __global__ void __launch_bounds__(kCdThreads, 2) chamfer_pair_kernel(const float
     }
   }
   __syncthreads();
-  const double sx = fixed_order_sum(rowmin, N, red);
-  const double sy = fixed_order_sum(colmin, M, red);
+}
+
+// The shared-memory regions of chamfer_smem_bytes.
+struct ChamferSmem {
+  float4* ytile;
+  double* red;
+  float* rowmin;
+  float* colmin;
+  __device__ ChamferSmem(unsigned char* smem, int N) {
+    ytile = reinterpret_cast<float4*>(smem);
+    red = reinterpret_cast<double*>(ytile + kYTile);
+    rowmin = reinterpret_cast<float*>(red + kCdThreads);
+    colmin = rowmin + round_up(N, kXChunk);
+  }
+};
+
+__global__ void __launch_bounds__(kCdThreads, 2) chamfer_pair_kernel(const float* __restrict__ A, int N, const float* __restrict__ B,
+                                                                    int M, int nB, int self, double* __restrict__ out) {
+  const int i = blockIdx.y, j = blockIdx.x;
+  if (self && j < i) return;  // the mirror of (j, i)
+  if (self && j == i) {
+    if (threadIdx.x == 0) out[(long long)i * nB + j] = 0.0;
+    return;
+  }
+  extern __shared__ __align__(16) unsigned char smem[];
+  const ChamferSmem sm(smem, N);
+  chamfer_minima(A + (long long)i * N * 3, N, B + (long long)j * M * 3, M, sm.ytile, sm.rowmin, sm.colmin);
+  const double sx = fixed_order_sum(sm.rowmin, N, sm.red);
+  const double sy = fixed_order_sum(sm.colmin, M, sm.red);
   if (threadIdx.x == 0) {
     const double cd = sx / (double)N + sy / (double)M;
     out[(long long)i * nB + j] = cd;
     if (self) out[(long long)j * nB + i] = cd;
+  }
+}
+
+// Max of v[0..n) (non-negative floats; exact in any order). Thread-strided, then the same halving tree as fixed_order_sum.
+__device__ float block_max(const float* v, int n, double* red) {
+  float m = 0.f;
+  for (int i = threadIdx.x; i < n; i += kCdThreads) m = fmaxf(m, v[i]);
+  red[threadIdx.x] = (double)m;
+  __syncthreads();
+  for (int h = kCdThreads / 2; h > 0; h >>= 1) {
+    if (threadIdx.x < h) red[threadIdx.x] = fmax(red[threadIdx.x], red[threadIdx.x + h]);
+    __syncthreads();
+  }
+  const float r = (float)red[0];
+  __syncthreads();
+  return r;
+}
+
+// One CTA per listed pair (a, b) of clouds of one size N: the matrix kernel's minima and sums, plus the largest row minimum.
+// A pair the host would refuse (a == b, an index out of range) gets NaN in all three outputs rather than a stray read.
+__global__ void __launch_bounds__(kCdThreads, 2) chamfer_list_kernel(const float* __restrict__ clouds, int n_clouds, int N,
+                                                                    const int* __restrict__ pairs, double* __restrict__ cd,
+                                                                    double* __restrict__ mean_ab, float* __restrict__ max_ab) {
+  const int p = blockIdx.x;
+  const int a = pairs[2 * p], b = pairs[2 * p + 1];
+  if (a == b || a < 0 || b < 0 || a >= n_clouds || b >= n_clouds) {
+    if (threadIdx.x == 0) {
+      cd[p] = mean_ab[p] = __longlong_as_double(0x7ff8000000000000LL);
+      max_ab[p] = __int_as_float(0x7fc00000);
+    }
+    return;
+  }
+  extern __shared__ __align__(16) unsigned char smem[];
+  const ChamferSmem sm(smem, N);
+  chamfer_minima(clouds + (long long)a * N * 3, N, clouds + (long long)b * N * 3, N, sm.ytile, sm.rowmin, sm.colmin);
+  const double sx = fixed_order_sum(sm.rowmin, N, sm.red);
+  const double sy = fixed_order_sum(sm.colmin, N, sm.red);
+  const float mx = block_max(sm.rowmin, N, sm.red);
+  if (threadIdx.x == 0) {
+    cd[p] = sx / (double)N + sy / (double)N;
+    mean_ab[p] = sx / (double)N;
+    max_ab[p] = mx;
   }
 }
 
@@ -266,6 +328,28 @@ int mdb_chamfer_matrix(const float* A, int nA, int N, const float* B, int nB, in
     return fail("mdb_chamfer_matrix: cudaFuncSetAttribute failed");
   chamfer_pair_kernel<<<dim3((unsigned)nB, (unsigned)nA), kCdThreads, smem, s>>>(A, N, B, M, nB, self, out);
   return check_launch("mdb_chamfer_matrix");
+}
+
+int mdb_chamfer_pairs(const float* clouds, int n_clouds, int N, const int* pairs, int P, double* cd, double* mean_ab,
+                      float* max_ab, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  if (n_clouds < 2) return fail("mdb_chamfer_pairs: a pair needs two distinct clouds, got n_clouds = " + std::to_string(n_clouds));
+  if (N < 1) return fail("mdb_chamfer_pairs: every cloud needs at least one point");
+  if (P < 0) return fail("mdb_chamfer_pairs: negative pair count");
+  if (P == 0) return 0;
+  if (!clouds || !pairs || !cd || !mean_ab || !max_ab) return fail("mdb_chamfer_pairs: null pointer");
+  int dev = 0, optin = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess)
+    return fail("mdb_chamfer_pairs: cannot query the device");
+  const size_t smem = chamfer_smem_bytes(N, N);
+  if (smem > (size_t)optin)
+    return fail("mdb_chamfer_pairs: the per-point minima of 2N = " + std::to_string(2LL * N) +
+                " points do not fit in shared memory");
+  if (cudaFuncSetAttribute(chamfer_list_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+    return fail("mdb_chamfer_pairs: cudaFuncSetAttribute failed");
+  chamfer_list_kernel<<<(unsigned)P, kCdThreads, smem, s>>>(clouds, n_clouds, N, pairs, cd, mean_ab, max_ab);
+  return check_launch("mdb_chamfer_pairs");
 }
 
 }  // extern "C"

@@ -63,6 +63,25 @@ def uncond_gen(config, idx=None):
     return out
 
 
+def tet_grid_coords(tet_path, device):
+    """Integer grid coordinates int64 [Nv, 3] of the vertices of the tet grid stored at `tet_path` (`eval.tet_path`)."""
+    from ..geometry.dmtet import grid_coords_of_tet_vertices
+    tet = np.load(tet_path)
+    return grid_coords_of_tet_vertices(torch.tensor(tet["vertices"])).to(device)
+
+
+def partial_grids(partials, coords, R, device):
+    """Partial DMTets ({'sdf', 'vis'} per tet vertex) -> the sampler's conditioning: sdf and visibility grids float32
+    [n, 1, R, R, R] holding each vertex's value at its voxel `coords` and 0 elsewhere (evaler.py:198-201 of the
+    reference)."""
+    sdf_grid = torch.zeros(len(partials), 1, R, R, R, device=device)
+    vis_grid = torch.zeros(len(partials), 1, R, R, R, device=device)
+    for i, d in enumerate(partials):
+        sdf_grid[i, 0, coords[:, 0], coords[:, 1], coords[:, 2]] = d["sdf"].to(device).float()
+        vis_grid[i, 0, coords[:, 0], coords[:, 1], coords[:, 2]] = d["vis"].to(device).float()
+    return sdf_grid, vis_grid
+
+
 def cond_gen(config, save_fname=None):
     save_fname = str(_rank()) if save_fname is None else save_fname
     eval_dir = config.eval.eval_dir
@@ -78,14 +97,7 @@ def cond_gen(config, save_fname=None):
     ema.copy_to(score_model.parameters())
 
     partial = torch.load(config.eval.partial_dmtet_path, map_location=device)
-    partial_sdf, partial_vis = partial["sdf"], partial["vis"]
-    tet = np.load(config.eval.tet_path)
-    from ..geometry.dmtet import grid_coords_of_tet_vertices
-    c = grid_coords_of_tet_vertices(torch.tensor(tet["vertices"])).to(device)
-    sdf_grid = torch.zeros(1, 1, R, R, R, device=device)
-    sdf_grid[0, 0, c[:, 0], c[:, 1], c[:, 2]] = partial_sdf.to(device).float()
-    vis_grid = torch.zeros(1, 1, R, R, R, device=device)
-    vis_grid[0, 0, c[:, 0], c[:, 1], c[:, 2]] = partial_vis.to(device).float()
+    sdf_grid, vis_grid = partial_grids([partial], tet_grid_coords(config.eval.tet_path, device), R, device)
     samples, _ = sampling_fn(score_model, partial=sdf_grid, partial_mask=vis_grid,
                              freeze_iters=config.eval.freeze_iters)
     out = os.path.join(eval_dir, f"{save_fname}.npy")

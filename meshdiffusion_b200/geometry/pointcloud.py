@@ -83,6 +83,34 @@ def chamfer_matrix(A, B=None):
     return out
 
 
+def chamfer_pairs(clouds, pairs):
+    """clouds fp32 [n, N, 3] (CUDA), pairs: P index pairs (a, b) with a != b -> (cd float64 [P], mean_ab float64 [P],
+    max_ab float32 [P]) from one `mdb_chamfer_pairs` launch. cd[p] = CD(clouds[a], clouds[b]), bitwise the
+    `chamfer_matrix` entry of the same two clouds; mean_ab[p] and max_ab[p] are the mean and the max over x in a of
+    min over y in b of |x - y|^2 (sqrt(max_ab) is the one-sided Hausdorff distance a -> b). An entry does not depend on
+    the other pairs. The list is checked on the host: a == b or an index out of range raises ValueError."""
+    L = _native.lib()
+    clouds = clouds.float().contiguous()
+    if clouds.dim() != 3 or clouds.shape[2] != 3 or not clouds.is_cuda:
+        raise ValueError("clouds must be a CUDA tensor [n, N, 3]")
+    n, N = clouds.shape[0], clouds.shape[1]
+    p = np.asarray(pairs.cpu() if torch.is_tensor(pairs) else pairs, dtype=np.int64).reshape(-1, 2)
+    if p.size and (p.min() < 0 or p.max() >= n):
+        raise ValueError(f"chamfer_pairs: a cloud index is outside [0, {n})")
+    if np.any(p[:, 0] == p[:, 1]):
+        raise ValueError("chamfer_pairs: a pair (a, a) compares a cloud with itself")
+    P = p.shape[0]
+    cd = torch.empty(P, device=clouds.device, dtype=torch.float64)
+    mean_ab = torch.empty_like(cd)
+    max_ab = torch.empty(P, device=clouds.device, dtype=torch.float32)
+    if P == 0:
+        return cd, mean_ab, max_ab
+    pd = torch.from_numpy(p.astype(np.int32)).to(clouds.device)
+    _native.check(L.mdb_chamfer_pairs(_native.ptr(clouds), n, N, _native.ptr(pd), P, _native.ptr(cd), _native.ptr(mean_ab),
+                                      _native.ptr(max_ab), _native.current_stream()))
+    return cd, mean_ab, max_ab
+
+
 # the auction's fp32 limit (csrc/emd.cu kFloor): eps must be at least this share of the pair's bounding-box diagonal
 EMD_EPS_FLOOR = 2.0 ** -18
 
