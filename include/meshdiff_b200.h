@@ -354,6 +354,28 @@ int mdb_chamfer_pairs(const float* clouds, int n_clouds, int N, const int* pairs
  * Bitwise reproducible and batch-invariant. B == NULL: self matrix of A (nB ignored), only i < j computed and mirrored,
  * diagonal exactly 0 with gap 0. About 35 N bytes of shared memory per pair: N up to about 6000 points. */
 int mdb_emd_matrix(const float* A, int nA, const float* B, int nB, int N, float eps, double* out, double* gap, void* stream);
+/* Light field descriptors (Chen et al. 2003 structure; geometry/lfd.py). face_id int32 [n_images][res][res] (res in
+ * [1, 256]); the silhouette is face_id >= 0. One CTA of 256 threads per image; pixel p (row-major, centre (c + 0.5, r + 0.5))
+ * belongs to thread p mod 256, visited in increasing order. n = inside pixels, cx = fp32(fp64(sum 2c + 1) / 2n), cy
+ * likewise; dx = x - cx, dy = y - cy, radius r = sqrt(max (dx dx + dy dy)) + 0.5. Zernike n = 1..10, m = n mod 2..n step 2
+ * (35 terms): per inside pixel u = dx / r, w = dy / r, s = u u + w w, V* = P_nm(s) (u - i w)^m (P_nm = R_n^m / rho^m by
+ * Horner in s, powers by repeated complex products), fp32 products added into fp64 per-thread sums, combined by the tree
+ * part[t] += part[t + s], s = 128..1; |A| = ((n + 1) |sum|) / ((pi r) r), byte min(255, floor(256 |A| + 0.5)). Fourier:
+ * ray k of 64 (ray_cs device fp32 [64][2], cos and sin), sample j at (cx + (0.5 j) cos, cy + (0.5 j) sin) while inside
+ * [0, res)^2; r_k = 0.5 x the last j whose pixel (floor y, floor x) is inside (else 0); F_m = sum_k r_k e^(-2 pi i m k / 64)
+ * in k order with dft device fp64 [11][64][2] (cos, sin); byte min(255, floor(512 |F_m| / |F_0| + 0.5)), m = 1..10 (0 when
+ * F_0 = 0). desc uint8 [n_images][48]: 35 Zernike, 10 Fourier, 3 zero bytes (all zero for an empty image); n_inside int32
+ * [n_images]. Every operation rounded on its own: oracle/lfd_oracle.py reproduces the bytes. */
+int mdb_lfd_descriptors(const int* face_id, int n_images, int res, const float* ray_cs, const double* dft,
+                        unsigned char* desc, int* n_inside, void* stream);
+/* Light field distance matrix. A uint8 [nA][10][10][48], B uint8 [nB][10][10][48] (light field, view, descriptor; 16-byte
+ * aligned); perms device int8 [60][10], the view permutation pi_g of each rotation of the dodecahedron (values outside
+ * 0..9 are clamped to 9). out int32 [nA][nB] = min over light fields s of A, t of B and g of
+ * sum_i sum_c |A[s][i][c] - B[t][pi_g(i)][c]|: one CTA per pair builds the 100 x 100 view-distance table in shared memory
+ * (__vsadu4) and takes the 6000 alignment sums as lookups. Exact integers: batch-invariant, and symmetric when perms is
+ * a group. B == NULL: self matrix of A (nB ignored), only i < j computed and mirrored, diagonal 0. nA, nB <= 65535. */
+int mdb_lfd_matrix(const unsigned char* A, int nA, const unsigned char* B, int nB, const signed char* perms, int* out,
+                   void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Probability-flow ODE likelihood (lib/diffusion/likelihood.py:26-113 with the continuous VP score -e / std(t)).

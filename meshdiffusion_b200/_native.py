@@ -123,6 +123,8 @@ SIGNATURES = {
     "mdb_closest_points": (_i, [_vp, _vp, _i, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mdb_nearest_vertex": (_i, [_vp, _vp, _i, _ll, _vp, _vp, _vp, _vp, _vp]),
     "mdb_segment_sum": (_i, [_vp, _i, _vp, _vp, _ll, _vp, _vp]),
+    "mdb_lfd_descriptors": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "mdb_lfd_matrix": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp]),
     "mdb_slerp_chunks": (_i, []),
     "mdb_slerp_frames": (_i, [_vp, _vp, _ll, _i, ctypes.POINTER(_d), _i, _vp, _vp, _vp, _vp, _vp]),
 }

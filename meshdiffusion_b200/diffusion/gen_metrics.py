@@ -15,7 +15,10 @@ distance (geometry/pointcloud.py) between those clouds:
 Ties go to the lowest index: in R for the argmin, in the concatenated order [G..., R...] for 1-NNA. With
 `eval.metric_emd` set, the same three metrics are also computed over the Earth Mover's distance (`mmd_emd`, `cov_emd`,
 `1nna_emd`, ...), each EMD solved to within EMD_EPS of the optimum; `emd_max_gap` is the largest certified gap over the
-three EMD matrices.
+three EMD matrices. With `eval.metric_lfd` set, the same non-empty shapes also get light-field descriptors
+(geometry/lfd.py) and the three metrics are computed over the light field distance (`mmd_lfd`, `cov_lfd`, `1nna_lfd`,
+...; integer distances, ties as above); `lfd_empty_views` counts silhouettes with no pixel, `lfd_saturated` is the share
+of descriptor coefficient bytes at 255.
 """
 import glob
 import json
@@ -26,7 +29,7 @@ import time
 import numpy as np
 import torch
 
-from ..geometry import pointcloud
+from ..geometry import lfd, pointcloud
 
 # grids per marching-tets launch while the sets are streamed through; only the point clouds stay on the device
 _CHUNK = 8
@@ -75,18 +78,45 @@ def generation_metrics(gen_points, ref_points, emd=False):
     return out
 
 
-def _clouds(grid_batches, resolution, n_points, seed, device):
-    """Streams [b,4,R,R,R] host batches through marching tets + sampling -> (non-empty clouds [n,N,3], n_empty)."""
-    kept, n_empty, next_id = [], 0, 0
+def _clouds(grid_batches, resolution, n_points, seed, device, light_fields=False):
+    """Streams [b,4,R,R,R] host batches through marching tets + sampling -> (non-empty clouds [n,N,3], n_empty, lfd) where
+    lfd is None, or with light_fields (descriptors uint8 [n,10,10,48] of the same shapes, their empty views, seconds)."""
+    kept, descs, n_empty, next_id, empty_views, lfd_seconds = [], [], 0, 0, 0, 0.0
     for batch in grid_batches:
         for c0 in range(0, batch.shape[0], _CHUNK):
             g = torch.as_tensor(batch[c0:c0 + _CHUNK], dtype=torch.float32).to(device)
-            pts, empty = pointcloud.grids_to_point_clouds(g, resolution, n_points, seed, first_id=next_id)
+            verts, faces, vert_off, face_off = pointcloud.grids_to_meshes(g, resolution)
+            pts, empty = pointcloud.sample_surface_points(verts, faces, vert_off, face_off, n_points, seed, first_id=next_id)
             next_id += g.shape[0]
             n_empty += int(empty.sum())
             kept.append(pts[~empty])
+            if light_fields:
+                torch.cuda.synchronize(device)
+                t0 = time.perf_counter()
+                d, ev = lfd.lfd_descriptors(verts, faces, vert_off, face_off)
+                keep = ~empty
+                descs.append(d[keep])
+                empty_views += int(ev[keep.cpu().numpy()].sum())
+                torch.cuda.synchronize(device)
+                lfd_seconds += time.perf_counter() - t0
     pts = torch.cat(kept) if kept else torch.empty(0, n_points, 3, device=device)
-    return pts, n_empty
+    if not light_fields:
+        return pts, n_empty, None
+    shape = (lfd.N_FIELDS, lfd.N_VIEWS, lfd.DESC_BYTES)
+    d = torch.cat(descs) if descs else torch.empty((0,) + shape, device=device, dtype=torch.uint8)
+    return pts, n_empty, (d, empty_views, lfd_seconds)
+
+
+def lfd_metrics(gen_desc, ref_desc):
+    """gen_desc [nG,10,10,48], ref_desc [nR,10,10,48] (CUDA, uint8) -> the metrics over the light field distance
+    (+ `lfd_matrix_seconds`)."""
+    torch.cuda.synchronize(gen_desc.device)
+    t0 = time.perf_counter()
+    d_gr, d_gg, d_rr = lfd.lfd_matrix(gen_desc, ref_desc), lfd.lfd_matrix(gen_desc), lfd.lfd_matrix(ref_desc)
+    torch.cuda.synchronize(gen_desc.device)
+    out = metrics_from_matrices(d_gr.cpu().numpy(), d_gg.cpu().numpy(), d_rr.cpu().numpy(), suffix="lfd")
+    out["lfd_matrix_seconds"] = time.perf_counter() - t0
+    return out
 
 
 def _generated_batches(eval_dir):
@@ -120,10 +150,13 @@ def eval_metrics(config):
     eval_dir = config.eval.eval_dir
     torch.cuda.synchronize(device)
     t0 = time.perf_counter()
-    gen, n_empty_gen = _clouds(_generated_batches(eval_dir), R, n_points, seed, device)
-    ref, n_empty_ref = _clouds(_reference_batches(config, R, device), R, n_points, seed, device)
+    light_fields = bool(config.eval.get("metric_lfd", False))
+    gen, n_empty_gen, gen_lf = _clouds(_generated_batches(eval_dir), R, n_points, seed, device, light_fields)
+    ref, n_empty_ref, ref_lf = _clouds(_reference_batches(config, R, device), R, n_points, seed, device, light_fields)
     torch.cuda.synchronize(device)
     sample_seconds = time.perf_counter() - t0
+    if light_fields:
+        sample_seconds -= gen_lf[2] + ref_lf[2]
     logging.info("eval_metrics: %d generated (%d empty), %d reference (%d empty) shapes, %d points each",
                  gen.shape[0], n_empty_gen, ref.shape[0], n_empty_ref, n_points)
     emd = bool(config.eval.get("metric_emd", False))
@@ -136,6 +169,13 @@ def eval_metrics(config):
         out.update({k: m[k] for k in ("mmd_emd", "cov_emd", "1nna_emd", "1nna_emd_gen", "1nna_emd_ref")})
         out.update(emd_convention=pointcloud.EMD_CONVENTION, emd_eps=EMD_EPS, emd_max_gap=m["emd_max_gap"],
                    emd_seconds=m["emd_seconds"])
+    if light_fields:
+        ml = lfd_metrics(gen_lf[0], ref_lf[0])
+        out.update({k: ml[k] for k in ("mmd_lfd", "cov_lfd", "1nna_lfd", "1nna_lfd_gen", "1nna_lfd_ref")})
+        coefs = torch.cat([gen_lf[0], ref_lf[0]])[..., :lfd.COEFS]
+        out.update(lfd_convention=lfd.LFD_CONVENTION, lfd_seconds=gen_lf[2] + ref_lf[2] + ml["lfd_matrix_seconds"],
+                   lfd_empty_views=gen_lf[1] + ref_lf[1],
+                   lfd_saturated=float((coefs == 255).sum()) / max(1, coefs.numel()))
     path = os.path.join(eval_dir, "metrics.json")
     with open(path, "w") as fh:
         json.dump(out, fh, indent=2)

@@ -176,14 +176,21 @@ def _tet_grid(resolution, device):
     return _TETS[key]
 
 
-def grids_to_point_clouds(grids, resolution, n_points, seed, first_id=0, mesh_scale=1.1, deform_scale=3.0):
-    """grids [B,4,R,R,R] (CUDA) -> (points fp32 [B, n_points, 3], empty bool [B]): tet-vertex gather, marching tets and
-    surface sampling, mesh b keyed by id first_id + b. The scale defaults are tools/npy_to_obj.py's
-    (nvdiffrec configs/res64.json), so every set sampled through here shares one frame."""
+def grids_to_meshes(grids, resolution, mesh_scale=1.1, deform_scale=3.0):
+    """grids [B,4,R,R,R] (CUDA) -> (verts fp32 [V,3], faces int64 [F,3], vert_off, face_off host int64 [B + 1]): tet-vertex
+    gather and marching tets, meshes packed in batch order. The scale defaults are tools/npy_to_obj.py's (nvdiffrec
+    configs/res64.json), so every set meshed through here shares one frame."""
     v, coords, idx, engines = _tet_grid(resolution, grids.device)
     B = grids.shape[0]
     if B not in engines:
         engines[B] = dmtet.MarchingTets(idx, v.shape[0], max_batch=B)
     sdf, pos = dmtet.grid_to_tet_inputs(grids.float(), coords, v, resolution, mesh_scale, deform_scale)
     mverts, mfaces, _, _, _, off = engines[B]._extract_raw(pos, sdf)
-    return sample_surface_points(mverts, mfaces, off[:, 0], off[:, 1], n_points, seed, first_id=first_id)
+    return mverts, mfaces, off[:, 0], off[:, 1]
+
+
+def grids_to_point_clouds(grids, resolution, n_points, seed, first_id=0, mesh_scale=1.1, deform_scale=3.0):
+    """grids [B,4,R,R,R] (CUDA) -> (points fp32 [B, n_points, 3], empty bool [B]): `grids_to_meshes` and surface sampling,
+    mesh b keyed by id first_id + b."""
+    mverts, mfaces, vert_off, face_off = grids_to_meshes(grids, resolution, mesh_scale, deform_scale)
+    return sample_surface_points(mverts, mfaces, vert_off, face_off, n_points, seed, first_id=first_id)
