@@ -171,7 +171,33 @@ void GemmOp::enable_splits(int S, float* scratch) {
   p.split_stride = (long long)p.Bn * p.X * p.Y * p.Z * p.N;
 }
 
+#ifdef MDB_EPI_TRACE
+std::vector<const GemmOp*>& trace_registry() {
+  static std::vector<const GemmOp*> ops;
+  return ops;
+}
+// Instrumented build only (not part of the C ABI): the epilogue stamps of the last launch of uploaded op i, as
+// [kTraceCtas][kTraceTiles][kTraceStamps] nanoseconds (0 = not reached), and its name. Returns -1 past the last op.
+extern "C" int mdb_epi_trace_read(int i, char* name, int name_cap, unsigned long long* out) {
+  auto& ops = trace_registry();
+  if (i < 0 || i >= (int)ops.size()) return -1;
+  snprintf(name, name_cap, "%s", ops[i]->name.c_str());
+  if (cudaMemcpy(out, ops[i]->d_trace, sizeof(unsigned long long) * kTraceCtas * kTraceTiles * kTraceStamps,
+                 cudaMemcpyDeviceToHost) != cudaSuccess) return -2;
+  return kTraceCtas * kTraceTiles * kTraceStamps;
+}
+extern "C" int mdb_epi_trace_dims(int* ctas, int* tiles, int* stamps) {
+  *ctas = kTraceCtas; *tiles = kTraceTiles; *stamps = kTraceStamps;
+  return 0;
+}
+#endif
+
 GemmOp::~GemmOp() {
+#ifdef MDB_EPI_TRACE
+  auto& ops = trace_registry();
+  for (size_t i = 0; i < ops.size(); ++i) if (ops[i] == this) { ops.erase(ops.begin() + i); break; }
+  if (d_trace) cudaFree(d_trace);
+#endif
   if (d_loads) cudaFree(d_loads);
   if (d_ks0) cudaFree(d_ks0);
   if (d_wpacked && owns_w) cudaFree(d_wpacked);
@@ -524,8 +550,62 @@ void GemmOp::finalize() {
   if (p.splits > p.total_groups) { p.splits = p.total_groups; splits = p.splits; }
 }
 
+// The TMA epilogue needs 128-column tiles of bf16 / split-bf16 rows stored whole (no split-K partials, no scalar column
+// stride, no fp32 output), a residual in the same format with its own rows per sample, and tensor-map-compatible
+// addresses: 16-byte aligned bases and strides. Every other launch keeps the per-thread stores.
+bool GemmOp::epi_tma_ok(const GemmParams& p) const {
+  if (gnb || block_n != 128 || prec == kTF32 || p.splits > 1 || p.ocs != 1 || p.out_fp32) return false;
+  if (p.res && (p.res_fp32 || p.batch_fastest)) return false;
+  const long long es = esize(prec);
+  auto aligned = [&](const void* base, long long lo_off, long long sx, long long sy, long long sz, long long sb) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(base);
+    return a % 16 == 0 && (lo_off * es) % 16 == 0 && (sx * es) % 16 == 0 && (sy * es) % 16 == 0 && (sz * es) % 16 == 0 &&
+           (sb * es) % 16 == 0;
+  };
+  if (!aligned(p.out, prec == kBF16X3 ? p.out_lo_off : 0, p.osx, p.osy, p.osz, p.osb)) return false;
+  if (p.res && !aligned(p.res, prec == kBF16X3 ? p.res_lo_off : 0, p.rsx, p.rsy, p.rsz, p.rsb)) return false;
+  return true;
+}
+
+// Output and residual maps of the TMA epilogue at batch B: (N channels, X, Y, Z, B) over the (physical) element strides
+// of the epilogue, boxes of one staging round (64 channels) by the M-tile; part 1 = the split-bf16 lo parts.
+static MapDesc epi_map(const void* base, Precision prec, int part, long long lo_off, const GemmParams& q, int B, long long sx,
+                       long long sy, long long sz, long long sb) {
+  const long long es = esize(prec);
+  MapDesc m;
+  m.rank = 5;
+  m.base = const_cast<char*>(static_cast<const char*>(base)) + (long long)part * lo_off * es;
+  m.dims[0] = q.N; m.dims[1] = q.X; m.dims[2] = q.Y; m.dims[3] = q.Z; m.dims[4] = B;
+  const long long st[4] = {sx * es, sy * es, sz * es, sb * es};
+  // an axis of extent 1 is only ever addressed at 0: its stride (0 in some callers' views) is replaced by a valid one
+  long long prev = es * q.N;
+  for (int i = 0; i < 4; ++i) {
+    m.strides[i] = (uint64_t)(m.dims[i + 1] == 1 ? prev : st[i]);
+    prev = (long long)m.strides[i] * (long long)m.dims[i + 1];
+  }
+  m.box[0] = kRowBytes / es; m.box[1] = q.bx; m.box[2] = q.by; m.box[3] = q.bz; m.box[4] = q.bb;
+  return m;
+}
+
+void GemmOp::encode_epi_maps(GemmParams& q, int B) const {
+  for (int part = 0; part < parts(prec); ++part) {
+    encode_map(&q.omap[part], prec, epi_map(q.out, prec, part, q.out_lo_off, q, B, q.osx, q.osy, q.osz, q.osb));
+    if (q.res) encode_map(&q.rmap[part], prec, epi_map(q.res, prec, part, q.res_lo_off, q, B, q.rsx, q.rsy, q.rsz, q.rsb));
+  }
+}
+
 void GemmOp::upload(cudaStream_t stream) {
   for (size_t i = 0; i < amaps_.size(); ++i) encode_map(&p.amap[i], prec, amaps_[i]);
+  p.epi_tma = epi_tma_ok(p) ? 1 : 0;
+  if (p.epi_tma && p.out) encode_epi_maps(p, p.Bn);
+#ifdef MDB_EPI_TRACE
+  // (instrumented build only: time the per-thread stores on the same launches)
+  if (getenv("MDB_EPI_TRACE_PER_THREAD")) p.epi_tma = 0;
+  MDB_CUDA_CHECK(cudaMalloc(&d_trace, sizeof(unsigned long long) * kTraceCtas * kTraceTiles * kTraceStamps));
+  MDB_CUDA_CHECK(cudaMemset(d_trace, 0, sizeof(unsigned long long) * kTraceCtas * kTraceTiles * kTraceStamps));
+  p.trace = d_trace;
+  trace_registry().push_back(this);
+#endif
   MDB_CUDA_CHECK(cudaMalloc(&d_loads, loads.size() * sizeof(LoadEntry)));
   MDB_CUDA_CHECK(cudaMemcpyAsync(d_loads, loads.data(), loads.size() * sizeof(LoadEntry), cudaMemcpyHostToDevice, stream));
   p.loads = d_loads;
@@ -549,6 +629,11 @@ void GemmOp::launch(cudaStream_t stream, int B, void* out_override) const {
     p.tb = (B + p.bb - 1) / p.bb;
   }
   if (out_override) p.out = out_override;
+  // the epilogue's maps clip at the launch's batch and address the launch's output
+  if (p.epi_tma && (out_override || p.Bn != this->p.Bn)) {
+    p.epi_tma = epi_tma_ok(p) ? 1 : 0;
+    if (p.epi_tma) encode_epi_maps(p, p.Bn);
+  }
   const int tiles_m = p.tx * p.ty * p.tz * p.tb;
   const int total = tiles_m * p.n_tiles_n * (p.splits > 1 ? p.splits : 1);
   const int grid = total < sm_count() ? total : sm_count();

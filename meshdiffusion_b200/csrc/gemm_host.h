@@ -77,6 +77,9 @@ class GemmOp {
   int* d_ks0 = nullptr;      // (weight packer) first k-step of every load entry
   void* d_wpacked = nullptr;  // [N][ksteps * parts * KB] in activation dtype
   bool owns_w = false;
+#ifdef MDB_EPI_TRACE
+  unsigned long long* d_trace = nullptr;  // the kernel's epilogue stamps of the last launch (instrumented build)
+#endif
   double flops = 0;  // algorithmic FLOPs of one launch (2*M*N*K over valid taps, counted densely)
   std::string name;
 
@@ -160,6 +163,8 @@ class GemmOp {
   int a_slot_need = 0;  // bytes of the largest A box (X3: both parts): the A slot size
   int nk_max = 0;       // most k-steps of one entry
   int pick_slots(GemmParams& q) const;  // sets the ring depths of q; returns the dynamic shared memory bytes
+  bool epi_tma_ok(const GemmParams& q) const;        // whether launch q can take the TMA epilogue (gemm_tc.cuh)
+  void encode_epi_maps(GemmParams& q, int B) const;  // q.omap / q.rmap for q's output and residual at batch B
   long long b_lo_off = 0;  // X3 activation-B: K coordinate of the lo parts
   std::vector<MapDesc> amaps_;  // p.amap[i] once uploaded
   MapDesc bmap_;                // p.bmap once uploaded (packed weights: described by upload itself)
@@ -167,6 +172,9 @@ class GemmOp {
 };
 
 int sm_count();
+#ifdef MDB_EPI_TRACE
+std::vector<const GemmOp*>& trace_registry();  // every uploaded op, for mdb_epi_trace_read
+#endif
 // SMs the split-K plans and grid caps are sized for (the H100 SXM's 132). A constant (not the device query) so that the
 // GPU-less sizing pass and the real pass agree on every scratch size.
 constexpr int kPlanSMs = 132;

@@ -15,7 +15,9 @@
 //   m64nNk8). After the last k-step they are staged through shared memory (64 columns at a time), and the same 256
 //   threads read them back one row per thread to add bias / time-embedding bias / residual, store NDHWC output and
 //   reduce per-(sample, channel) sum and sum-of-squares for the GroupNorm that follows (warp-shuffle butterfly + shared
-//   + one atomic per channel).
+//   + one atomic per channel). In the bf16 / split-bf16 inference kernels with 128-column tiles (GemmParams::epi_tma)
+//   each 64-column round borrows the next B slot: the producer TMA-loads the residual box into it, the threads
+//   overwrite it with the output box and one thread stores that with TMA. Other launches store row by row.
 //
 // Warp roles (384 threads): warpgroup 0 = TMA producer (warp 0), warpgroups 1-2 = MMA + epilogue.
 #pragma once
@@ -67,6 +69,15 @@ constexpr int kMaxSegs = 8;
 struct GemmParams {
   CUtensorMap amap[kMaxAMaps];
   CUtensorMap bmap;
+  // TMA epilogue (epi_tma != 0): each 64-column staging round takes the next B slot; the producer loads the residual box
+  // into it, the epilogue threads overwrite it with the output box and one thread stores that with TMA. Boxes are
+  // (kStageCols channels, bx, by, bz, bb), 128B-swizzled; [0] = the tensor / the hi parts, [1] = the split-bf16 lo parts.
+  CUtensorMap omap[2];
+  CUtensorMap rmap[2];
+  int epi_tma;
+#ifdef MDB_EPI_TRACE
+  unsigned long long* trace;  // [kTraceCtas][kTraceTiles][kTraceStamps] globaltimer stamps (instrumented build only)
+#endif
   const LoadEntry* loads;
   int n_loads;
   int n_segs;
@@ -140,6 +151,24 @@ struct GemmCfg {
   static constexpr int kFixedBytes = 1024 + kAccFloats * 4 + kStatsFloats * 4 + 4 * kMaxSlots * 8;
 };
 constexpr int kRegsProducer = 40, kRegsConsumer = 232;  // 128 x 40 + 256 x 232 <= 65 536
+
+// The TMA epilogue exists in the inference instantiations with 128-column tiles of bf16 rows: there one round's output box
+// (64 channels x 128 rows x 2 B) is exactly one weight tile, and a split-bf16 B slot holds its hi and lo boxes.
+template <int BLOCK_N, Precision P, bool GNB>
+constexpr bool kHasTmaEpi = !GNB && BLOCK_N == 128 && P != kTF32;
+constexpr int kEpiBoxBytes = 64 * 2 * kBlockM;  // one part of one round's output / residual box
+static_assert(kEpiBoxBytes == GemmCfg<128>::kBTileBytes, "an epilogue box is one weight tile");
+
+#ifdef MDB_EPI_TRACE
+// Instrumented build (-DMDB_EPI_TRACE): the first kTraceTiles tiles of the first kTraceCtas CTAs record globaltimer
+// stamps, taken by epilogue thread 0: 0 = last wgmma_wait<0>, 1 = round 0 staged, 2 = round 0's chunks done (TMA
+// epilogue: its store issued), 3 = the same for round 1, 4 = statistics atomics done, 5 = the tile's first k-step has its
+// operands (the previous tile's epilogue ends at the next tile's stamp 5).
+constexpr int kTraceCtas = 16, kTraceTiles = 64, kTraceStamps = 6;
+#define MDB_STAMP(k) do { if (trace_row && et == 0) trace_row[k] = globaltimer(); } while (0)
+#else
+#define MDB_STAMP(k) do { } while (0)
+#endif
 
 // K-major 128B-swizzled operand at `saddr` (SBO = 1024 B)
 __device__ __forceinline__ uint64_t kdesc(uint32_t saddr) { return make_wgmma_desc(saddr, 16, 1024); }
@@ -295,6 +324,28 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
             ++l;
           }
         }
+        if constexpr (kHasTmaEpi<BLOCK_N, P, GNB>) {
+          // the tile's epilogue slots, one per staging round: the residual box(es) of the round's columns, loaded while
+          // the last k-steps run, or (no residual / no valid column) a plain arrival
+          if (p.epi_tma) {
+            for (int rnd = 0; rnd < Cfg::kStageRounds; ++rnd) {
+              mbar_wait(b_empty + 8 * bs, bph ^ 1);
+              if (elect_one()) {
+                const uint32_t bbase = b_ring + bs * b_slot, bar = b_full + 8 * bs;
+                const int c = n0 + rnd * Cfg::kStageCols;
+                if (p.res && c < p.N) {
+                  mbar_expect_tx(bar, kParts * kEpiBoxBytes);
+                  tma_load_5d(&p.rmap[0], bar, bbase, c, x0, y0, z0, b0);
+                  if constexpr (P == kBF16X3) tma_load_5d(&p.rmap[1], bar, bbase + kEpiBoxBytes, c, x0, y0, z0, b0);
+                } else {
+                  mbar_arrive(bar);
+                }
+              }
+              __syncwarp();
+              if (++bs == (uint32_t)NB) { bs = 0; bph ^= 1; }
+            }
+          }
+        }
       }
     }
   } else {
@@ -321,8 +372,23 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
       asm volatile("" : "+r"(want_cols));
     }
     uint32_t as = 0, aph = 0, bs = 0, bph = 0;
+    // TMA epilogue: the slot of the tile's last round, handed back once its store has read it (epilogue thread 0 only)
+    int epi_pend = -1;
     for (int tile = first_tile; tile < total_tiles; tile += tile_step, ++it) {
       const int vit = it;
+#ifdef MDB_EPI_TRACE
+      unsigned long long* trace_row = (p.trace && (int)blockIdx.x < kTraceCtas && it < kTraceTiles)
+                                          ? p.trace + ((long long)blockIdx.x * kTraceTiles + it) * kTraceStamps : nullptr;
+      bool first_k = true;
+#endif
+      if constexpr (kHasTmaEpi<BLOCK_N, P, GNB>) {
+        if (et == 0 && epi_pend >= 0) {
+          bulk_wait_read<0>();
+          mbar_arrive(b_empty + 8 * epi_pend);
+          mbar_arrive(b_empty + 8 * epi_pend);
+          epi_pend = -1;
+        }
+      }
       // ---------------------------------------------------------------- main loop: wgmma over the k-step groups
       constexpr int kAccRegs = kParts * BLOCK_N / 2;  // split bf16: [W_hi columns | W_lo columns] until the fold
       float acc[kAccRegs];
@@ -344,6 +410,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
             const uint32_t abase = a_ring + as * a_slot + a_row0;
             for (int j = 0; j < sgm.nk; ++j) {
               mbar_wait(b_full + 8 * bs, bph);
+#ifdef MDB_EPI_TRACE
+              if (first_k) { MDB_STAMP(5); first_k = false; }
+#endif
               const uint64_t ad = kdesc(abase + j * sgm.jbytes);
               const uint64_t bd = kdesc(b_ring + bs * b_slot);
               wgmma_fence();  // directly in front of the straight-line wgmmas: no branch between the fence and them
@@ -373,6 +442,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
         }
         wgmma_wait<0>();
         fence_operands(acc);
+        MDB_STAMP(0);
         if (wt == 0) {
           if (prev_b >= 0) mbar_arrive(b_empty + 8 * prev_b);
           if (prev_a >= 0) mbar_arrive(a_empty + 8 * prev_a);
@@ -469,9 +539,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
           }
         }
       };
+      // TMA epilogue (residual, when there is one, from the round's slot; output into it): decided by the launch's
+      // parameters, the same for every thread and for the producer
+      const bool tma_epi = kHasTmaEpi<BLOCK_N, P, GNB> && p.epi_tma != 0;
       const int ch0 = kChunkStep == 2 ? half : 0;
       const bool active = kChunkStep == 2 || half == 0;  // BLOCK_N == 32: one chunk, the second warp of a quarter idles
-      if (active) prefetch_res(ch0);
+      if (active && !tma_epi) prefetch_res(ch0);
 
       // the chunks of round r are [kRoundChunks * r, kRoundChunks * (r + 1)); each warp takes its own in the same order
       // (half, half + 2, ...) as from a single round
@@ -483,6 +556,19 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
           stage();
         }
         named_bar_sync(2, kEpiThreads);  // staged accumulators (and bias) visible to every epilogue thread
+        if (rnd == 0) MDB_STAMP(1);
+        // TMA epilogue: the round's slot, in the producer's ring order; 128B-swizzled rows of 128 B (64 bf16 channels),
+        // the 16-byte vector c of row r at r * 128 + 16 (c ^ r % 8), so the row-per-lane accesses are conflict-free
+        int eslot_i = 0;
+        uint8_t* eslot = nullptr;
+        if constexpr (kHasTmaEpi<BLOCK_N, P, GNB>) {
+          if (tma_epi) {
+            eslot_i = (int)bs;
+            eslot = smem + NA * p.a_slot_bytes + bs * p.b_slot_bytes;
+            mbar_wait(b_full + 8 * bs, bph);
+            if (++bs == (uint32_t)NB) { bs = 0; bph ^= 1; }
+          }
+        }
 
 #pragma unroll 1
         for (int ch = ch0 + rnd * kRoundChunks; ch < (rnd + 1) * kRoundChunks && active; ch += kChunkStep) {
@@ -555,7 +641,19 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
               for (int i = 0; i < 32; ++i) q2[i] = 0.f;
             }
           }
-          if (!GNB && p.res && valid) {
+          // byte offset of this chunk's 16-byte vector i in the round's slot (TMA epilogue)
+          const int chr = ch - rnd * kRoundChunks;
+          auto eoff = [&](int i) { return row * 128 + (((4 * chr + i) ^ (row & 7)) << 4); };
+          if (!GNB && p.res && valid && tma_epi) {
+            // (columns past N were zero-filled by TMA and are not stored)
+            uint4 buf[8];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              buf[i] = *reinterpret_cast<const uint4*>(eslot + eoff(i));
+              buf[4 + i] = P == kBF16X3 ? *reinterpret_cast<const uint4*>(eslot + kEpiBoxBytes + eoff(i)) : buf[i];
+            }
+            add_res_chunk<P>(buf, v);
+          } else if (!GNB && p.res && valid) {
             if (P == kTF32 || p.res_fp32) {  // plain fp32 (also the tf32 activation format, whose loads need no rounding)
               if (full) {
                 add_res_chunk<kTF32>(rbuf, v);
@@ -572,8 +670,16 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
               }
             }
           }
-          if (ch + kChunkStep < kChunks) prefetch_res(ch + kChunkStep);  // lands while this chunk is stored / reduced
-          if (valid) {
+          if (!tma_epi && ch + kChunkStep < kChunks) prefetch_res(ch + kChunkStep);  // lands while this chunk is stored / reduced
+          if (tma_epi) {
+            // over the residual bytes this thread has read; rows outside the grid are clipped by the store
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const uint4 h = bf16x8_encode(v + 8 * i);
+              *reinterpret_cast<uint4*>(eslot + eoff(i)) = h;
+              if constexpr (P == kBF16X3) *reinterpret_cast<uint4*>(eslot + kEpiBoxBytes + eoff(i)) = bf16x8_encode_lo(h, v + 8 * i);
+            }
+          } else if (valid) {
             if (p.out_fp32) {
               float* op = reinterpret_cast<float*>(p.out) + ooff + nb;
               if (full) {
@@ -606,6 +712,31 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
             s_part[(q * 2 + 1) * BLOCK_N + ch * 32 + lane] = ss[0];
           }
         }
+        if constexpr (kHasTmaEpi<BLOCK_N, P, GNB>) {
+          if (tma_epi) {
+            fence_proxy_async();  // this thread's output bytes, visible to the TMA store
+            named_bar_sync(2, kEpiThreads);
+            if (et == 0) {
+              // TMA clips the box at the grid and at N (a round wholly past N stores nothing)
+              const int c = n0 + rnd * Cfg::kStageCols;
+              const uint32_t src = b_ring + eslot_i * b_slot;
+              if (c < p.N) {
+                tma_store_5d(&p.omap[0], src, c, x0, y0, z0, b0);
+                if constexpr (P == kBF16X3) tma_store_5d(&p.omap[1], src + kEpiBoxBytes, c, x0, y0, z0, b0);
+              }
+              bulk_commit();
+              // the previous round's slot goes back to the producer once its store has read it; nothing waits for the
+              // global writes
+              if (epi_pend >= 0) {
+                bulk_wait_read<1>();
+                mbar_arrive(b_empty + 8 * epi_pend);
+                mbar_arrive(b_empty + 8 * epi_pend);
+              }
+              epi_pend = eslot_i;
+            }
+          }
+        }
+        MDB_STAMP(2 + rnd);
       }
       if constexpr (GNB) {
         if (p.gnb_part && splits == 1) {
@@ -651,6 +782,10 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tc_kernel(const __grid_c
           }
         }
       }
+      MDB_STAMP(4);
+    }
+    if constexpr (kHasTmaEpi<BLOCK_N, P, GNB>) {
+      if (et == 0 && epi_pend >= 0) bulk_wait<0>();  // the shared memory outlives the last store
     }
   }
 }

@@ -66,6 +66,27 @@ __device__ __forceinline__ void tma_load_3d(const void* desc, uint32_t bar, uint
       : "r"(dst), "l"(reinterpret_cast<uint64_t>(desc)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// shared -> global box store; elements outside the tensor map's extents are not written. Completion is tracked per
+// thread by bulk async-groups (bulk_commit / bulk_wait_read), so the thread that stores is the one that waits.
+__device__ __forceinline__ void tma_store_5d(const void* desc, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+      :
+      : "l"(reinterpret_cast<uint64_t>(desc)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups are still in flight (their global writes included)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
 
 // ---------------------------------------------------------------- wgmma (warpgroup MMA, accumulators in registers)
 // Shared-memory matrix descriptor, 128B swizzle: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout [62,64) (1 = SWIZZLE_128B).
