@@ -187,6 +187,53 @@ int mdb_solver_run(mdb_unet* net, float* x, float* x0_hist, const float* mask, c
                    int batch, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
                    const mdb_sampler_cond* cond /* nullable */, int cond_until, void* stream);
 
+/* Shape editing (`--mode=edit`): RePaint resampling (Lugmayr et al. 2022) on the DPM-Solver++(2M) label grid
+ * (diffusion/sampling.py: repaint_schedule, get_repaint_sampler, which compute the entry table in float64 on the host).
+ * An entry is one of two kinds, on x fp32 [B][C][V] with the grid mask g [V]:
+ *   denoise (kind 0): the network runs at `label`, then mdb_solver_update's step without its replacement:
+ *            x0 = (x - sigma eps) inv_alpha;  x' = (c_x x + c_0 x0 + c_1 x0_prev + c_z z) g;  x0_prev <- x0
+ *   renoise (kind 1): a jump up the label grid by forward diffusion, no network: x' = (c_x x + c_z z) g with
+ *            c_x = alpha_hi / alpha_lo and c_z = sqrt(1 - c_x^2); x0_prev is not touched (sigma, inv_alpha, c_0, c_1 unused)
+ * Both kinds then replace the kept region on every channel c in `known->channels`:
+ *   x_c <- (x_c (1 - m) + (known_coef known_c + known_std z'_c) m) g
+ * with (known_coef, known_std) = alpha, sigma of the label the entry lands on, and (1, 0) on the last entry, which makes
+ * the kept region of the output equal `known`. One channel in `channels` and a denoise-only table give mdb_solver_update's
+ * arithmetic, rounding and Philox keys. */
+typedef struct mdb_repaint_entry {
+  int kind;                      /* 0 = denoise, 1 = renoise */
+  float label;                   /* denoise: network label; renoise: the label it jumps to */
+  float sigma, inv_alpha;
+  float c_x, c_0, c_1, c_z;
+  float known_coef, known_std;
+} mdb_repaint_entry;
+
+/* The kept region. known: channel 0 of sample 0 of a [B][C][V] fp32 tensor; known_bstride is the element distance to the
+ * next sample (0 = one grid for the whole batch). mask: m [V] of sample 0, mask_bstride likewise. channels: bit c set =
+ * channel c is replaced (channels < 2^C). noise: z' [B][C][V], or NULL for Philox(seed, element, offset + 2). */
+typedef struct mdb_repaint_known {
+  const float* known;
+  long long known_bstride;
+  const float* mask;
+  long long mask_bstride;
+  unsigned channels;
+  const float* noise;
+} mdb_repaint_known;
+
+/* One entry, in place on x and x0_hist ([batch][channels][voxels] fp32; mask [voxels]). eps: the network output (denoise;
+ * ignored by renoise). noise: z [batch][channels][voxels], or NULL for Philox(seed, element, offset) with element the
+ * index in x (a loop passes offset = 4 * e for global entry e). known: nullable (no replacement). */
+int mdb_repaint_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry* entry,
+                       long long voxels, int channels, int batch, const float* noise /* nullable */,
+                       unsigned long long seed, unsigned long long offset, const mdb_repaint_known* known /* nullable */,
+                       void* stream);
+/* The whole schedule without host round trips: for i < n_entries: denoise entries run entries[i].label -> network
+ * (eps_buf) -> update, renoise entries the update alone, with in-kernel Philox at offset 4 * (step0 + i). `entries` is a
+ * HOST array of n_entries entries for the global entries step0 .. step0 + n_entries - 1. eps_buf: device scratch [B][C][V];
+ * labels_buf: device scratch [B]. known->noise must be NULL. The call only enqueues work. */
+int mdb_repaint_run(mdb_unet* net, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry* entries,
+                    int n_entries, int batch, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
+                    const mdb_repaint_known* known /* nullable */, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Training-step kernels (optimiser side). Replace get_ddpm_loss_fn's elementwise tail (lib/diffusion/losses.py:69-78),
  * torch.nn.utils.clip_grad_norm_ + torch.optim.Adam.step (losses.py:45-50, 26-35) and

@@ -17,7 +17,7 @@ from meshdiffusion_b200.compat.config_dict import parse_override_value
 from meshdiffusion_b200.compat.install import ensure_ml_collections
 
 MODES = ("train", "uncond_gen", "cond_gen", "eval_metrics", "eval_likelihood", "make_partial", "fit_grids", "export",
-         "uncond_gen_interp", "eval_completion")
+         "uncond_gen_interp", "eval_completion", "edit")
 
 
 def load_config_file(path):
@@ -94,6 +94,9 @@ def main(argv=None):
     elif mode == "eval_completion":
         from meshdiffusion_b200.diffusion import completion
         completion.eval_completion(config)
+    elif mode == "edit":
+        from meshdiffusion_b200.diffusion import edit
+        edit.edit(config)
 
 
 if __name__ == "__main__":

@@ -50,6 +50,22 @@ class SolverStepC(ctypes.Structure):
                 ("label", "sigma", "inv_alpha", "c_x", "c_0", "c_1", "c_z", "cond_coef", "cond_std")]
 
 
+class RepaintEntryC(ctypes.Structure):
+    """mdb_repaint_entry (include/meshdiff_b200.h)."""
+    _fields_ = [("kind", ctypes.c_int)] + [(name, ctypes.c_float) for name in
+                                           ("label", "sigma", "inv_alpha", "c_x", "c_0", "c_1", "c_z", "known_coef",
+                                            "known_std")]
+
+
+class RepaintKnownC(ctypes.Structure):
+    """mdb_repaint_known (include/meshdiff_b200.h)."""
+    _fields_ = [
+        ("known", ctypes.c_void_p), ("known_bstride", ctypes.c_longlong),
+        ("mask", ctypes.c_void_p), ("mask_bstride", ctypes.c_longlong),
+        ("channels", ctypes.c_uint), ("noise", ctypes.c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); the symbol list is checked against the header by tests/test_abi.py
 _vp, _i, _ll, _f, _u64, _d = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float, ctypes.c_ulonglong, ctypes.c_double
 SIGNATURES = {
@@ -88,6 +104,10 @@ SIGNATURES = {
                                ctypes.POINTER(SamplerCondC), _vp]),
     "mdb_solver_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverStepC), _i, _i, _u64, _vp, _vp, _i,
                             ctypes.POINTER(SamplerCondC), _i, _vp]),
+    "mdb_repaint_update": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(RepaintEntryC), _ll, _i, _i, _vp, _u64, _u64,
+                                ctypes.POINTER(RepaintKnownC), _vp]),
+    "mdb_repaint_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(RepaintEntryC), _i, _i, _u64, _vp, _vp, _i,
+                             ctypes.POINTER(RepaintKnownC), _vp]),
     "mdb_ddpm_loss": (_i, [_vp, _vp, _vp, _d, _vp, _vp, _vp, _i, _i, _ll, _vp]),
     "mdb_ddpm_perturb": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _ll, _vp]),
     "mdb_chunk_elems": (_i, []),

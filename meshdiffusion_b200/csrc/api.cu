@@ -362,6 +362,57 @@ int mdb_solver_run(mdb_unet* n, float* x, float* x0_hist, const float* mask, con
   MDB_API_END
 }
 
+static RepaintArgs repaint_args(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry& e,
+                                long long V, int C, const mdb_repaint_known* k) {
+  if (e.kind != 0 && e.kind != 1) throw std::runtime_error("mdb: repaint entry kind must be 0 (denoise) or 1 (renoise)");
+  RepaintArgs a{};
+  a.renoise = e.kind; a.eps = eps; a.x = x; a.x0_hist = x0_hist; a.mask = mask;
+  a.sigma = e.sigma; a.inv_alpha = e.inv_alpha; a.c_x = e.c_x; a.c_0 = e.c_0; a.c_1 = e.c_1; a.c_z = e.c_z;
+  a.V = V; a.C = C;
+  if (k && k->known && k->channels) {
+    if (!k->mask) throw std::runtime_error("mdb: the kept region needs its mask");
+    if (C > 32 || (C < 32 && (k->channels >> C) != 0u)) throw std::runtime_error("mdb: repaint channel set outside the channels");
+    a.known = k->known; a.known_bs = k->known_bstride; a.kmask = k->mask; a.kmask_bs = k->mask_bstride;
+    a.channels = k->channels; a.coef = e.known_coef; a.std = e.known_std; a.known_noise = k->noise;
+  }
+  return a;
+}
+
+int mdb_repaint_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry* entry,
+                       long long V, int C, int B, const float* noise, unsigned long long seed, unsigned long long offset,
+                       const mdb_repaint_known* known, void* stream) {
+  MDB_API_BEGIN
+  if (!entry) throw std::runtime_error("mdb: mdb_repaint_update needs an entry");
+  if (V <= 0 || C <= 0 || B <= 0) throw std::runtime_error("mdb: mdb_repaint_update needs positive voxels, channels, batch");
+  RepaintArgs a = repaint_args(eps, x, x0_hist, mask, *entry, V, C, known);
+  if (!a.renoise && !eps) throw std::runtime_error("mdb: a denoise entry needs the network output");
+  a.noise = noise; a.seed = seed; a.offset = offset;
+  launch_repaint_update(a, B, (cudaStream_t)stream);
+  MDB_API_END
+}
+
+int mdb_repaint_run(mdb_unet* n, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry* entries,
+                    int n_entries, int B, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
+                    const mdb_repaint_known* known, void* stream) {
+  MDB_API_BEGIN
+  cudaStream_t s = (cudaStream_t)stream;
+  const UNetConfig& c = n->net->cfg();
+  const long long V = (long long)c.image_size * c.image_size * c.image_size;
+  if (n_entries > 0 && !entries) throw std::runtime_error("mdb: mdb_repaint_run needs the entry table");
+  if (known && known->noise) throw std::runtime_error("mdb: mdb_repaint_run draws its noise in-kernel (known->noise must be NULL)");
+  for (int i = 0; i < n_entries; ++i) {
+    RepaintArgs a = repaint_args(eps_buf, x, x0_hist, mask, entries[i], V, c.num_channels, known);
+    if (!a.renoise) {
+      fill_kernel<<<(B + 127) / 128, 128, 0, s>>>(labels_buf, entries[i].label, B);
+      n->net->forward(x, labels_buf, eps_buf, B, s, /*allow_graph=*/true);
+    }
+    // mdb_solver_run's Philox counter blocks, keyed by the global entry: 4 outputs per entry, the replacement draw at +2
+    a.noise = nullptr; a.seed = seed; a.offset = 4ull * (unsigned long long)(step0 + i);
+    launch_repaint_update(a, B, s);
+  }
+  MDB_API_END
+}
+
 int mdb_conv3d(const void* x, int B, int cin, int z, int y_, int x_, const float* w, const float* bias, int cout,
                int ksize, int stride, void* out, const float* rowbias, const void* residual, long long* stats,
                int precision, void* stream) {

@@ -105,4 +105,27 @@ struct SolverUpdateArgs {
 };
 void launch_solver_update(const SolverUpdateArgs& a, int B, cudaStream_t s);
 
+// One entry of a RePaint resampling schedule (csrc/repaint.cu), in place, fp32 NCDHW [B][C][V]; mask [V]:
+//   denoise: solver_update_kernel's step without its replacement (x0_hist <- x0)
+//   renoise: x' = (c_x x + c_z z) g   (c_x = alpha_hi / alpha_lo, c_z = sqrt(1 - c_x^2); x0_hist untouched)
+// then, when known != nullptr, on every channel c with bit c of `channels` set:
+//   x_c <- (x_c (1 - m) + (coef known_c + std z'_c) m) g
+struct RepaintArgs {
+  int renoise;
+  const float* eps;    // network output (denoise)
+  float* x;            // in/out state
+  float* x0_hist;      // denoise: in x0 of the previous step, out x0 of this step
+  const float* mask;   // g [V]
+  float sigma, inv_alpha, c_x, c_0, c_1, c_z;
+  long long V; int C;
+  const float* noise;               // z [B][C][V] or null (then Philox(seed, element, offset))
+  unsigned long long seed, offset;
+  const float* known; long long known_bs;  // [C][V] of sample 0, sample stride (0 = shared)
+  const float* kmask; long long kmask_bs;  // m [V] of sample 0, sample stride (0 = shared)
+  unsigned channels;
+  float coef, std;                  // alpha, sigma of the label the entry lands on; (1, 0) on the last entry
+  const float* known_noise;         // z' [B][C][V] or null (then Philox(seed, element, offset + 2))
+};
+void launch_repaint_update(const RepaintArgs& a, int B, cudaStream_t s);
+
 }  // namespace mdb

@@ -705,3 +705,198 @@ def get_dpm_solver_inverter(sde, shape, n_steps=25, grid_mask=None, device="cuda
             return x, K_eff
 
     return invert
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# RePaint resampling (Lugmayr et al., "RePaint: Inpainting using Denoising Diffusion Probabilistic Models", CVPR 2022) on
+# the DPM-Solver++(2M) label grid, for shape editing: the kept region is replaced on every step, and every block of
+# `jump` solver steps is redone `resample` times, jumping back to the block's first label by forward diffusion in
+# between, so the network sees the kept and the regenerated region together at every noise level of the block.
+REPAINT_COLUMNS = ("kind", "label", "sigma", "inv_alpha", "c_x", "c_0", "c_1", "c_z", "known_coef", "known_std")
+
+
+def repaint_schedule(sde, n_steps, jump, resample, stochastic=False, denoise=True):
+    """Entry table of RePaint resampling over the labels of `dpm_solver_schedule(sde, n_steps, stochastic, denoise)`.
+
+    The K_eff solver steps are cut into blocks of `jump` steps. Every block but the last runs `resample` times, with a
+    renoise entry from the block's last label lo back to its first label hi between two runs; the last block runs once.
+    Rows (float64, mdb_repaint_entry field order, REPAINT_COLUMNS):
+      denoise (kind 0): the solver step's row (label, sigma, inv_alpha, c_x, c_0, c_1, c_z, alpha, sigma of the label it
+        lands on); the first step of a repeated run is first order (c_1 = 0), since the x0 history belongs to the
+        abandoned run;
+      renoise (kind 1): (1, hi, 0, 0, a, 0, 0, s, alpha_hi, sigma_hi) with a = alpha_hi / alpha_lo, s = sqrt(1 - a^2).
+    The last row's replacement pair is (1, 0), so the kept region of the output equals the known grid. With resample = 1
+    the rows are dpm_solver_schedule's. Returns (table, number of network evaluations = denoise rows)."""
+    for name, v in (("jump", jump), ("resample", resample)):
+        if isinstance(v, bool) or int(v) != v or v < 1:
+            raise ValueError(f"repaint: {name} must be an integer >= 1, got {v!r}")
+    jump, resample = int(jump), int(resample)
+    labels, table = dpm_solver_schedule(sde, n_steps, stochastic, denoise)
+    abar = sde.alphas_cumprod.detach().to("cpu", torch.float64).numpy()
+    alpha, sigma = np.sqrt(abar), np.sqrt(1.0 - abar)
+    lam = np.log(alpha) - np.log(sigma)
+    K = len(labels) - 1
+    rows = []
+    for b0 in range(0, K, jump):
+        b1 = min(b0 + jump, K)
+        runs = 1 if b1 == K else resample
+        for r in range(runs):
+            for k in range(b0, b1):
+                row = table[k]
+                if r > 0 and k == b0:  # first order; never the last step, so the sub-table's noise term is the table's
+                    row = _solver_table(alpha, sigma, lam, labels[b0:b0 + 2], stochastic, denoise=False)[0]
+                rows.append(np.concatenate([[0.0], row]))
+            if r < runs - 1:
+                lo, hi = labels[b1], labels[b0]
+                a = alpha[hi] / alpha[lo]
+                rows.append(np.array([1.0, hi, 0.0, 0.0, a, 0.0, 0.0, np.sqrt(1.0 - a * a), alpha[hi], sigma[hi]]))
+    out = np.stack(rows)
+    out[-1, 8:10] = (1.0, 0.0)
+    return out, int((out[:, 0] == 0).sum())
+
+
+def _repaint_entries_c(table):
+    """The entry table as the float32 mdb_repaint_entry array the library takes."""
+    rows = table.astype(np.float32)
+    arr = (_native.RepaintEntryC * len(rows))()
+    for i, r in enumerate(rows):
+        arr[i] = _native.RepaintEntryC(int(r[0]), *(float(v) for v in r[1:]))
+    return arr
+
+
+class _Known:
+    """The kept region in the form the update kernel takes it: `known` fp32 [1 or B, C, R, R, R] (what the output must
+    hold there), `mask` fp32 [1 or B, R, R, R] (1 = kept voxel; 1 / B samples = shared / per sample) and the replaced
+    channels."""
+
+    def __init__(self, known, mask, channels, B):
+        self.known = known.to(torch.float32).contiguous()
+        C = self.known.shape[1]
+        self.mask = mask.to(torch.float32).reshape(mask.shape[0], *self.known.shape[2:]).contiguous()
+        for t in (self.known, self.mask):
+            if t.shape[0] not in (1, B):
+                raise ValueError("repaint: known / known_mask must have batch 1 or the sampling batch")
+        self.channels = sorted({int(c) for c in channels})
+        if not self.channels or self.channels[0] < 0 or self.channels[-1] >= C:
+            raise ValueError(f"repaint: channels must be a non-empty subset of 0 .. {C - 1}, got {channels!r}")
+        self.kb = self.known[0].numel() if self.known.shape[0] == B and B > 1 else 0
+        self.mb = self.mask[0].numel() if self.mask.shape[0] == B and B > 1 else 0
+
+    def struct(self, noise=None):
+        s = _native.RepaintKnownC()
+        s.known, s.known_bstride = self.known.data_ptr(), self.kb
+        s.mask, s.mask_bstride = self.mask.data_ptr(), self.mb
+        s.channels = sum(1 << c for c in self.channels)
+        s.noise = noise.data_ptr() if noise is not None else None
+        return s
+
+
+def _repaint_update_eager(eps, x, x0_hist, mask, row, noise=None, known=None, known_noise=None):
+    """One entry in torch fp32 ops, in place on x and x0_hist, with the operation order of repaint_update_kernel (each
+    product and sum rounded on its own), so it is the kernel's bit-exact oracle. `row`: a float32 table row; `mask`
+    broadcasts over x; `known`: a _Known; known_noise: z' shaped like x."""
+    kind, _, sg, inv_a, c_x, c_0, c_1, c_z, coef, std = (float(v) for v in row)
+    if kind:
+        xn = (x * c_x + noise * c_z) * mask
+    else:
+        x0 = (x - eps * sg) * inv_a
+        xn = x * c_x + x0 * c_0
+        if c_1 != 0.0:
+            xn = xn + x0_hist * c_1
+        if c_z != 0.0:
+            xn = xn + noise * c_z
+        xn = xn * mask
+        x0_hist.copy_(x0)
+    if known is not None:
+        for c in known.channels:
+            xn[:, c] = _replace_channel(xn[:, c], known.known[:, c], known.mask, mask, coef, std, known_noise[:, c])
+    x.copy_(xn)
+    return x
+
+
+def _repaint_update(eps, x, x0_hist, mask_flat, entry_c, noise=None, known=None, known_noise=None, seed=0, offset=0):
+    """One entry through mdb_repaint_update, in place on x and x0_hist; noise=None draws it in-kernel."""
+    L = _native.lib()
+    B, C = x.shape[0], x.shape[1]
+    ks = known.struct(noise=known_noise) if known is not None else None
+    _native.check(L.mdb_repaint_update(_native.ptr(eps), _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat),
+                                       ctypes.byref(entry_c), x[0, 0].numel(), C, B, _native.ptr(noise), int(seed),
+                                       int(offset), ctypes.byref(ks) if ks is not None else None,
+                                       _native.current_stream()))
+    return x
+
+
+def _native_repaint_loop(net, x, x0_hist, mask_flat, entries_c, seed, step0=0, n=None, known=None):
+    """Entries step0 .. step0+n-1 of the schedule inside the library (mdb_repaint_run), in place on x and x0_hist.
+    `entries_c` is the whole table (_repaint_entries_c), indexed by the GLOBAL entry."""
+    L = _native.lib()
+    B = x.shape[0]
+    n = len(entries_c) - step0 if n is None else n
+    net._ensure_engine(B, x.device)
+    net.sync_parameters()
+    eps_buf = torch.empty_like(x)
+    labels_buf = torch.empty(B, device=x.device, dtype=torch.float32)
+    part = (_native.RepaintEntryC * n).from_buffer(entries_c, step0 * ctypes.sizeof(_native.RepaintEntryC))
+    ks = known.struct() if known is not None else None
+    _native.check(L.mdb_repaint_run(net._handle, _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat), part, n,
+                                    B, int(seed), _native.ptr(eps_buf), _native.ptr(labels_buf), int(step0),
+                                    ctypes.byref(ks) if ks is not None else None, _native.current_stream()))
+    return x
+
+
+def get_repaint_sampler(sde, shape, inverse_scaler, n_steps=25, jump=5, resample=5, stochastic=False, denoise=True,
+                        device="cuda", grid_mask=None, native_rng=False, seed=42):
+    """Returns `repaint_sampler(model, known, known_mask, channels, x0=None)` -> (samples, number of network
+    evaluations): samples of shape `shape` whose kept region (known_mask = 1, batch 1 or shape[0]) holds `known` (batch 1
+    or shape[0]) exactly on `channels`, the rest regenerated by repaint_schedule's entries.
+
+    The prior is sde.prior_sampling(shape) * grid_mask, or x0 * grid_mask; its kept region is replaced at label N - 1
+    (alpha, sigma of N - 1, fresh noise), as the conditional dpm_solver sampler does. Paths: on CUDA with `native_rng`
+    and a native ScoreNet the whole schedule runs in the library (mdb_repaint_run, Philox noise keyed by seed + rank and
+    entry); other CUDA states run model + mdb_repaint_update per entry with torch.randn_like noise; CPU tensors run the
+    eager fp32 update (_repaint_update_eager), which is the kernel's oracle."""
+    table, nfe = repaint_schedule(sde, n_steps, jump, resample, stochastic, denoise)
+    rows32 = table.astype(np.float32)
+    entries_c = _repaint_entries_c(table)
+    N = sde.N
+    abar_T = float(sde.alphas_cumprod[N - 1])
+    a_T, s_T = (float(np.float32(v)) for v in (np.sqrt(abar_T), np.sqrt(1.0 - abar_T)))  # alpha, sigma of label N - 1
+
+    def repaint_sampler(model, known, known_mask, channels, x0=None):
+        with torch.no_grad():
+            B = shape[0]
+            if x0 is not None and tuple(x0.shape) != tuple(shape):
+                raise ValueError(f"repaint: x0 has shape {tuple(x0.shape)}, the sampler {tuple(shape)}")
+            x = sde.prior_sampling(shape).to(device) if x0 is None else x0.to(device=device, dtype=torch.float32)
+            x = (x * grid_mask).contiguous()
+            if tuple(known.shape[1:]) != tuple(shape[1:]):
+                raise ValueError(f"repaint: known has shape {tuple(known.shape)}, the sampler {tuple(shape)}")
+            mask_v = grid_mask.to(device=x.device, dtype=torch.float32).reshape(x.shape[2:]).contiguous()
+            kn = _Known(known.to(x.device), known_mask.to(x.device), channels, B)
+            z = torch.randn_like(x)
+            for c in kn.channels:
+                x[:, c] = _replace_channel(x[:, c], kn.known[:, c], kn.mask, mask_v, a_T, s_T, z[:, c])
+            x0_hist = torch.empty_like(x)
+            net = _native_net(model)
+            if x.is_cuda and native_rng and net is not None:
+                net._ensure_engine(B, x.device)
+                net.sync_parameters()
+                net._frozen = True  # nobody edits the weights inside the loop: skip per-step change detection
+                try:
+                    _native_repaint_loop(net, x, x0_hist, mask_v.reshape(-1), entries_c, seed + _rank(), known=kn)
+                finally:
+                    net._frozen = False
+                return inverse_scaler(x), nfe
+            for e in range(len(rows32)):
+                renoise = rows32[e, 0] != 0
+                eps_out = None if renoise else model(x, torch.full((B,), float(rows32[e, 1]), device=x.device)).float()
+                noise = torch.randn_like(x) if (renoise or rows32[e, 7] != 0) else None
+                z2 = torch.randn_like(x)
+                if x.is_cuda:
+                    _repaint_update(None if renoise else eps_out.contiguous(), x, x0_hist, mask_v.reshape(-1),
+                                    entries_c[e], noise, kn, z2)
+                else:
+                    _repaint_update_eager(eps_out, x, x0_hist, mask_v, rows32[e], noise, kn, z2)
+            return inverse_scaler(x), nfe
+
+    return repaint_sampler
