@@ -515,6 +515,31 @@ int mdb_segment_sum(const float* src, int width, const long long* perm, const lo
                     void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Partial DMTets from observed depth maps (`--mode=partial_from_depth`). Every product, sum and quotient is rounded on its
+ * own (no FMA contraction), so a float32 restatement reproduces the buffers, flags, distances and points bit for bit.
+ */
+/* depth fp32 [n_obs][res][res]: camera depth along -z_cam, row 0 = clip y = -1; 0 or non-finite = no surface. proj,
+ * inv_mv device fp32 [n_obs][16] (row-major): the perspective matrix (rows [p00 0 p02 0], [0 p11 p12 0], [0 0 A B],
+ * [0 0 -1 0]) and the inverse of the model-view. Per observed pixel (r, c): x_ndc = (c + 0.5) / res * 2 - 1 (y_ndc from
+ * r), camera point (d (x_ndc + p02) / p00, d (y_ndc + p12) / p11, -d), world point = rows 0-2 of inv_mv times it (rows as
+ * in mdb_raster_depth), z / w = (B - A d) / d. Outputs [n_obs][res][res]: zbuf fp32 (100 where empty), valid int32 (0
+ * surface, -1 empty; with zbuf the buffers mdb_carve_vertices reads), points fp32 [..][3] (0 where empty), edge uint8 (1
+ * where an observed 4-neighbour's depth differs by more than max_jump). res in [2, 4096]. */
+int mdb_depth_unproject(const float* depth, int n_obs, int res, const float* proj, const float* inv_mv, float max_jump,
+                        float* zbuf, int* valid, float* points, unsigned char* edge, void* stream);
+/* Closest point on the observed surface for every query: queries fp32 [Q][3] packed by observation (query_off device
+ * int64 [n_obs + 1], max_queries >= the largest count); mvp, proj device fp32 [n_obs][16]; points, valid, edge as
+ * mdb_depth_unproject wrote them. The query is projected like mdb_carve_vertices (skipped unless w > 0 and X, Y lie within
+ * 64 px of the image); the window half-width is min(31, ceil(radius max(|p00|, |p11|) 0.5 res / w)) blocks around block
+ * (floor(Y - 0.5), floor(X - 0.5)), clipped to the image. Block (r, c) with all four corner pixels valid and not edges
+ * gives triangles (r c, r c+1, r+1 c+1) and (r c, r+1 c+1, r+1 c), tested as in mdb_closest_points; blocks in row-major
+ * order, the nearest wins, ties to the first. dist2 fp32 [Q] (+inf if none), closest fp32 [Q][3] (NaN if none), found
+ * uint8 [Q]. */
+int mdb_depth_closest_points(const float* queries, const long long* query_off, int n_obs, long long max_queries, int res,
+                             const float* mvp, const float* proj, float radius, const float* points, const int* valid,
+                             const unsigned char* edge, float* dist2, float* closest, unsigned char* found, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Shape interpolation (`--mode=uncond_gen_interp`). Replaces `slerp` of lib/diffusion/evaler.py:63-71 (which the
  * reference's uncond_gen_interp, :73-130, applies to two prior noises): spherical interpolation over the whole tensor, no
  * grid mask.

@@ -1,6 +1,6 @@
 """Entry point with the reference's command line (main_diffusion.py:13-28):
 
-    python main_diffusion.py --config=configs/res64.py --mode={train,uncond_gen,cond_gen,eval_metrics,eval_likelihood,make_partial,fit_grids,export,uncond_gen_interp,eval_completion} [--config.a.b=value ...]
+    python main_diffusion.py --config=configs/res64.py --mode={train,uncond_gen,cond_gen,eval_metrics,eval_likelihood,make_partial,partial_from_depth,fit_grids,export,uncond_gen_interp,eval_completion,edit} [--config.a.b=value ...]
 
 The reference parses this with absl + ml_collections.config_flags (lock_config=False: overrides may create keys);
 neither ml_collections nor network access is available here, so the same syntax is parsed directly.
@@ -17,7 +17,7 @@ from meshdiffusion_b200.compat.config_dict import parse_override_value
 from meshdiffusion_b200.compat.install import ensure_ml_collections
 
 MODES = ("train", "uncond_gen", "cond_gen", "eval_metrics", "eval_likelihood", "make_partial", "fit_grids", "export",
-         "uncond_gen_interp", "eval_completion", "edit")
+         "uncond_gen_interp", "eval_completion", "edit", "partial_from_depth")
 
 
 def load_config_file(path):
@@ -82,6 +82,8 @@ def main(argv=None):
         eval_likelihood.eval_likelihood(config)
     elif mode == "make_partial":
         evaler.make_partial(config)
+    elif mode == "partial_from_depth":
+        evaler.partial_from_depth(config)
     elif mode == "fit_grids":
         from meshdiffusion_b200.diffusion import fit_grids
         fit_grids.fit_grids(config)

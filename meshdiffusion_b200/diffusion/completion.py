@@ -111,6 +111,7 @@ def read_index(partial_dir):
         entries += idx["files"]
     if not entries:
         raise ValueError(f"eval_completion: the partial index in {partial_dir} lists no files")
+    _require_fields(entries)
     entries.sort(key=lambda e: (int(e["shape"]), int(e["view"])))
     seen = set()
     for e in entries:
@@ -131,7 +132,18 @@ def plan_calls(positions, per_call):
     return calls
 
 
+def _require_fields(entries):
+    """Completion needs each partial's ground truth: refuses an index without it (`--mode=partial_from_depth` writes
+    partials of observations that have none)."""
+    for e in entries:
+        for key in ("shape", "view", "source"):
+            if key not in e:
+                raise ValueError(f"eval_completion: the index entry of {e.get('file', '?')} has no {key!r} field; "
+                                 "completion is scored against the source shape, so it takes make_partial's index")
+
+
 def check_sources(entries, fpath_list):
+    _require_fields(entries)
     for e in entries:
         i = int(e["shape"])
         if not 0 <= i < len(fpath_list):

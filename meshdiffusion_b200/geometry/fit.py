@@ -171,6 +171,48 @@ def _point_to_mesh(points, verts, faces, vo, fo):
     return d2.view(B, n).double().mean(1)
 
 
+def sample_grad(q, off, samples, s_off, s_mesh, n_points):
+    """mesh -> samples: d/dm mean_s |s - nn(s)|^2 over the n_points samples of each mesh (packed [B * n_points, 3], s_mesh
+    their mesh), nn the nearest marching-tet vertex of q (packed by off[:, 0]), gathered onto the vertices in a fixed
+    order."""
+    _, nn = nearest_vertex(samples, s_off, q, off[:, 0])
+    hit = nn >= 0
+    rows = nn + torch.from_numpy(off[:-1, 0]).to(q.device)[s_mesh]
+    contrib = 2.0 * (q[rows.clamp(min=0)] - samples) / n_points
+    return segment_sum(contrib[hit], rows[hit], q.shape[0])
+
+
+def fit_deformation(mt, pos, sdf, n_verts, iters, lr, reg, data_grad):
+    """The deformation fit of GridFitter and of the depth partials: `iters` Adam steps on deform [B, n_verts, 3] (from
+    zero) through the differentiable marching tets `mt` with the topology the sign `sdf` [B, n_verts] fixes, pos(deform)
+    placing the tet vertices. data_grad(q, off) -> fp32 [Q, 3], the gradient of the data terms with respect to the
+    marching-tet vertices q (packed by off[:, 0], detached); reg * mean |deform|^2 per mesh is added. The deformation is
+    clamped to [-0.99, 0.99] after every step (the reference's `clamp_deform`)."""
+    deform = torch.zeros(sdf.shape[0], n_verts, 3, device=sdf.device, requires_grad=True)
+    opt = torch.optim.Adam([deform], lr=lr)
+    for _ in range(iters):
+        mverts, _, _, _, _ = dmtet._ExtractFn.apply(mt, pos(deform), sdf)
+        grad = data_grad(mverts.detach(), mt._last_off)
+        r = reg * deform.square().mean(dim=(1, 2)).sum()
+        opt.zero_grad()
+        torch.autograd.backward([mverts, r], [grad, torch.ones_like(r)])
+        opt.step()
+        with torch.no_grad():
+            deform.clamp_(-0.99, 0.99)
+    return deform
+
+
+def zero_off_surface(mt, pos, sdf, deform):
+    """deform * vert_mask (fit_dmtets.py:784-789): the deformation with zeros off the vertices of the surface tets."""
+    B, Nv, dev = deform.shape[0], deform.shape[1], deform.device
+    _, _, _, _, vvi, off = mt._extract_raw(pos(deform), sdf)
+    mask = torch.zeros(B * Nv, device=dev)
+    packed_ids = vvi + torch.arange(B, device=dev).repeat_interleave(
+        torch.from_numpy(np.diff(off[:, 2])).to(dev), output_size=vvi.shape[0]) * Nv
+    mask[packed_ids] = 1.0
+    return deform.detach() * mask.view(B, Nv, 1)
+
+
 class GridFitter:
     """Meshes -> DMTet training grids for a fixed tet grid; holds the device state between batches."""
 
@@ -224,39 +266,20 @@ class GridFitter:
         s_off = np.arange(B + 1) * self.points
         s_mesh = torch.arange(B, device=dev).repeat_interleave(self.points)
 
-        deform = torch.zeros(B, Nv, 3, device=dev, requires_grad=True)
-        opt = torch.optim.Adam([deform], lr=self.lr)
-        for _ in range(self.iters):
-            mverts, _, _, _, _ = dmtet._ExtractFn.apply(self.mt, self._pos(deform), sdf)
-            off = self.mt._last_off
-            q = mverts.detach()
+
+        def data_grad(q, off):
             counts = torch.from_numpy(np.diff(off[:, 0])).to(dev)
             v_mesh = torch.arange(B, device=dev).repeat_interleave(counts, output_size=q.shape[0])
             # surface -> mesh: d/dm mean_m |m - cp|^2, cp held fixed
             _, _, cp = closest_points(q, off[:, 0], src_v, src_f, vo, fo)
             grad = 2.0 * (q - cp) / counts[v_mesh].float()[:, None]
-            # mesh -> surface: d/dm mean_s |s - nn(s)|^2, gathered onto the vertices in a fixed order
-            _, nn = nearest_vertex(samples, s_off, q, off[:, 0])
-            hit = nn >= 0
-            rows = nn + torch.from_numpy(off[:-1, 0]).to(dev)[s_mesh]
-            contrib = 2.0 * (q[rows.clamp(min=0)] - samples) / self.points
-            grad = grad + segment_sum(contrib[hit], rows[hit], q.shape[0])
-            reg = self.reg * deform.square().mean(dim=(1, 2)).sum()
-            opt.zero_grad()
-            torch.autograd.backward([mverts, reg], [grad, torch.ones_like(reg)])
-            opt.step()
-            with torch.no_grad():
-                deform.clamp_(-0.99, 0.99)
+            return grad + sample_grad(q, off, samples, s_off, s_mesh, self.points)
+
+        deform = fit_deformation(self.mt, self._pos, sdf, Nv, self.iters, self.lr, self.reg, data_grad)
         t2 = self._sync()
 
-        # deform * vert_mask (fit_dmtets.py:784-789): zero off the vertices of the surface tets
         with torch.no_grad():
-            _, _, _, _, vvi, off = self.mt._extract_raw(self._pos(deform), sdf)
-            mask = torch.zeros(B * Nv, device=dev)
-            packed_ids = vvi + torch.arange(B, device=dev).repeat_interleave(
-                torch.from_numpy(np.diff(off[:, 2])).to(dev), output_size=vvi.shape[0]) * Nv
-            mask[packed_ids] = 1.0
-            final = deform.detach() * mask.view(B, Nv, 1)
+            final = zero_off_surface(self.mt, self._pos, sdf, deform)
             grids = torch.stack([tets_to_3dgrid(self.coords, sdf[b], final[b], self.R) for b in range(B)])
             sdf_g, pos_g = dmtet.grid_to_tet_inputs(grids, self.coords, self.verts, self.R, self.mesh_scale, self.deform_scale)
             fv, ff, _, _, _, foff = self.mt._extract_raw(pos_g, sdf_g)
