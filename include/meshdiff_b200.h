@@ -187,6 +187,38 @@ int mdb_solver_run(mdb_unet* net, float* x, float* x0_hist, const float* mask, c
                    int batch, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
                    const mdb_sampler_cond* cond /* nullable */, int cond_until, void* stream);
 
+/* Progressive distillation (Salimans & Ho 2022; `--mode=distill`, diffusion/distill.py, with the rows computed in float64
+ * on the host by diffusion/sampling.py: distill_rows). A student step i moves z from label s = l_{2i} to e = l_{2i+2} of
+ * the teacher's DDIM grid l (ddim_grid); the teacher takes two first-order ODE (DDIM) steps s -> m = l_{2i+1} -> e, each
+ * in mdb_solver_update's form with c_1 = c_z = 0:  x0 = (z - sigma eps) inv_alpha;  z' = (c_x z + c_0 x0) g.
+ * The student's target is the noise prediction whose single DDIM step from z_s lands on the teacher's z_e:
+ *   eps~ = (z_e - r z_s) inv_d   with r = alpha_e / alpha_s and inv_d = 1 / (sigma_e - alpha_e sigma_s / alpha_s). */
+typedef struct mdb_distill_row {
+  float label_s, label_m, label_e;                    /* network labels of the three grid points */
+  float sigma_s, inv_alpha_s, c_x_s, c_0_s;           /* teacher step s -> m */
+  float sigma_m, inv_alpha_m, c_x_m, c_0_m;           /* teacher step m -> e */
+  float r, inv_d;                                     /* target coefficients */
+} mdb_distill_row;
+
+/* One phase on fp32 [batch][channels][voxels] tensors (mask g [voxels]). step_idx: DEVICE int [batch], sample b uses
+ * rows[step_idx[b]]; rows: DEVICE array of n_rows entries. An index outside [0, n_rows) reads no row: that sample's
+ * outputs and label are NaN.
+ *   phase 0 (teacher step s -> m, eps = teacher(z_s, s)): z_mid = (c_x_s z_s + c_0_s x0) g, bitwise mdb_solver_update's
+ *           first-order step; labels[b] = m (the next forward's labels). out is not touched (may be NULL).
+ *   phase 1 (teacher step m -> e, eps = teacher(z_mid, m)): z_e as above from z_mid, then out = ((z_e - r z_s) inv_d) g;
+ *           labels[b] = s (the student's labels). z_mid is read only.
+ * Every product and sum is rounded on its own. The call only enqueues work. */
+int mdb_distill_step(const float* eps, const float* z_s, float* z_mid, float* out, const float* mask, const int* step_idx,
+                     const mdb_distill_row* rows, int n_rows, int phase, float* labels, long long voxels, int channels,
+                     int batch, void* stream);
+/* The student's targets on the teacher's inference engine, without host round trips: teacher(z_s, labels) -> phase 0 ->
+ * teacher(z_mid, labels) -> phase 1 -> eps_target. labels: device fp32 [batch] holding s = rows[step_idx[b]].label_s on
+ * entry (the perturbation and the student's forward use them too); it holds them again on return. z_mid, eps_buf: device
+ * scratch [batch][C][V]. Rows and indices as in mdb_distill_step. The call only enqueues work. */
+int mdb_distill_targets(mdb_unet* teacher, const float* z_s, const int* step_idx, const mdb_distill_row* rows, int n_rows,
+                        const float* mask, float* eps_target, float* labels, float* z_mid, float* eps_buf, int batch,
+                        void* stream);
+
 /* Shape editing (`--mode=edit`): RePaint resampling (Lugmayr et al. 2022) on the DPM-Solver++(2M) label grid
  * (diffusion/sampling.py: repaint_schedule, get_repaint_sampler, which compute the entry table in float64 on the host).
  * An entry is one of two kinds, on x fp32 [B][C][V] with the grid mask g [V]:

@@ -1,6 +1,6 @@
 """Entry point with the reference's command line (main_diffusion.py:13-28):
 
-    python main_diffusion.py --config=configs/res64.py --mode={train,uncond_gen,cond_gen,eval_metrics,eval_likelihood,make_partial,partial_from_depth,fit_grids,export,uncond_gen_interp,eval_completion,edit} [--config.a.b=value ...]
+    python main_diffusion.py --config=configs/res64.py --mode={train,uncond_gen,cond_gen,eval_metrics,eval_likelihood,make_partial,partial_from_depth,fit_grids,export,uncond_gen_interp,eval_completion,edit,distill} [--config.a.b=value ...]
 
 The reference parses this with absl + ml_collections.config_flags (lock_config=False: overrides may create keys);
 neither ml_collections nor network access is available here, so the same syntax is parsed directly.
@@ -17,7 +17,7 @@ from meshdiffusion_b200.compat.config_dict import parse_override_value
 from meshdiffusion_b200.compat.install import ensure_ml_collections
 
 MODES = ("train", "uncond_gen", "cond_gen", "eval_metrics", "eval_likelihood", "make_partial", "fit_grids", "export",
-         "uncond_gen_interp", "eval_completion", "edit", "partial_from_depth")
+         "uncond_gen_interp", "eval_completion", "edit", "partial_from_depth", "distill")
 
 
 def load_config_file(path):
@@ -99,6 +99,9 @@ def main(argv=None):
     elif mode == "edit":
         from meshdiffusion_b200.diffusion import edit
         edit.edit(config)
+    elif mode == "distill":
+        from meshdiffusion_b200.diffusion import distill
+        distill.distill(config)
 
 
 if __name__ == "__main__":

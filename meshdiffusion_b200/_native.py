@@ -50,6 +50,13 @@ class SolverStepC(ctypes.Structure):
                 ("label", "sigma", "inv_alpha", "c_x", "c_0", "c_1", "c_z", "cond_coef", "cond_std")]
 
 
+class DistillRowC(ctypes.Structure):
+    """mdb_distill_row (include/meshdiff_b200.h)."""
+    _fields_ = [(name, ctypes.c_float) for name in
+                ("label_s", "label_m", "label_e", "sigma_s", "inv_alpha_s", "c_x_s", "c_0_s",
+                 "sigma_m", "inv_alpha_m", "c_x_m", "c_0_m", "r", "inv_d")]
+
+
 class RepaintEntryC(ctypes.Structure):
     """mdb_repaint_entry (include/meshdiff_b200.h)."""
     _fields_ = [("kind", ctypes.c_int)] + [(name, ctypes.c_float) for name in
@@ -104,6 +111,8 @@ SIGNATURES = {
                                ctypes.POINTER(SamplerCondC), _vp]),
     "mdb_solver_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverStepC), _i, _i, _u64, _vp, _vp, _i,
                             ctypes.POINTER(SamplerCondC), _i, _vp]),
+    "mdb_distill_step": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _ll, _i, _i, _vp]),
+    "mdb_distill_targets": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "mdb_repaint_update": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(RepaintEntryC), _ll, _i, _i, _vp, _u64, _u64,
                                 ctypes.POINTER(RepaintKnownC), _vp]),
     "mdb_repaint_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(RepaintEntryC), _i, _i, _u64, _vp, _vp, _i,

@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libmeshdiff_b200.so")
-SOURCES = ["gemm_host.cu", "wgrad_host.cu", "elementwise.cu", "backward.cu", "unet.cu", "unet_train.cu", "marching_tets.cu", "mesh_ops.cu", "train_ops.cu", "pc_metrics.cu", "emd.cu", "likelihood.cu", "raster.cu", "fit.cu", "depth_partial.cu", "interp.cu", "lfd.cu", "repaint.cu", "api.cu"]
+SOURCES = ["gemm_host.cu", "wgrad_host.cu", "elementwise.cu", "backward.cu", "unet.cu", "unet_train.cu", "marching_tets.cu", "mesh_ops.cu", "train_ops.cu", "pc_metrics.cu", "emd.cu", "likelihood.cu", "raster.cu", "fit.cu", "depth_partial.cu", "interp.cu", "lfd.cu", "repaint.cu", "distill.cu", "api.cu"]
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH_FLAGS + [
     "-O3", "-lineinfo", "-std=c++17",

@@ -24,6 +24,12 @@ namespace mdb { void set_last_error(const std::string& msg) { g_err = msg; } }
 
 struct mdb_unet { UNet* net; };
 
+namespace mdb {
+void launch_distill_step(const float* eps, const float* z_s, float* z_mid, float* out, const float* mask,
+                         const int* step_idx, const mdb_distill_row* rows, int n_rows, int phase, float* labels,
+                         long long V, int C, int B, cudaStream_t s);
+}  // csrc/distill.cu
+
 extern "C" {
 
 const char* mdb_last_error(void) { return g_err.c_str(); }
@@ -359,6 +365,27 @@ int mdb_solver_run(mdb_unet* n, float* x, float* x0_hist, const float* mask, con
     a.noise = nullptr; a.seed = seed; a.offset = 4ull * (unsigned long long)(step0 + i);
     launch_solver_update(a, B, s);
   }
+  MDB_API_END
+}
+
+int mdb_distill_targets(mdb_unet* n, const float* z_s, const int* step_idx, const mdb_distill_row* rows, int n_rows,
+                        const float* mask, float* eps_target, float* labels, float* z_mid, float* eps_buf, int B,
+                        void* stream) {
+  MDB_API_BEGIN
+  if (!n || !n->net) throw std::runtime_error("mdb: mdb_distill_targets needs the teacher network");
+  if (n_rows < 1) throw std::runtime_error("mdb: mdb_distill_targets needs at least one row");
+  if (!z_s || !step_idx || !rows || !mask || !eps_target || !labels || !z_mid || !eps_buf)
+    throw std::runtime_error("mdb: mdb_distill_targets: null argument");
+  if (B <= 0 || B > 65535) throw std::runtime_error("mdb: mdb_distill_targets needs a batch in [1, 65535]");
+  cudaStream_t s = (cudaStream_t)stream;
+  const UNetConfig& c = n->net->cfg();
+  const long long V = (long long)c.image_size * c.image_size * c.image_size;
+  // no CUDA graph: z_s, z_mid, eps_buf and labels are new buffers on every training micro-step, and graphs are keyed by
+  // the buffer addresses
+  n->net->forward(z_s, labels, eps_buf, B, s, /*allow_graph=*/false);
+  launch_distill_step(eps_buf, z_s, z_mid, nullptr, mask, step_idx, rows, n_rows, 0, labels, V, c.num_channels, B, s);
+  n->net->forward(z_mid, labels, eps_buf, B, s, /*allow_graph=*/false);
+  launch_distill_step(eps_buf, z_s, z_mid, eps_target, mask, step_idx, rows, n_rows, 1, labels, V, c.num_channels, B, s);
   MDB_API_END
 }
 

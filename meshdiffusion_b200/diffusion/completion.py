@@ -11,7 +11,7 @@ Inputs: the partial index `eval.partial_dir` (default `<eval_dir>/partial`: `ind
 
 Sampling: every call has batch `eval.batch_size`, a multiple of k, and holds batch_size / k partials in k consecutive
 slots each (per-sample conditioning). The last call is padded with copies of its last partial, whose outputs are dropped,
-so one engine size serves the run. `dpm_solver` (ODE or SDE) takes any multiple of k; `pc` only batch_size == k (one
+so one engine size serves the run. `dpm_solver` (ODE or SDE) and `distilled` take any multiple of k; `pc` only batch_size == k (one
 partial per call, `cond_gen`'s exact path: its step-0 initialisation broadcasts the first partial over the batch, the
 reference's behaviour); `ddim` is refused. Under torchrun rank r takes the partials p = r (mod world size), with the
 global torch RNG seeded `seed + rank` as in `cond_gen`. A completion therefore depends on the seed, its slot in the
@@ -79,6 +79,8 @@ def sampler(config, batch_size, k):
     if method == "dpm_solver":
         return method, {"dpm_steps": int(config.sampling.get("dpm_steps", 25)),
                         "dpm_sde": bool(config.sampling.get("dpm_sde", False))}
+    if method == "distilled":
+        return method, {"distill_steps": int(config.sampling.get("distill_steps", 8))}
     if method == "pc":
         if batch_size != k:
             raise ValueError(f"eval_completion: sampling.method='pc' needs eval.batch_size == eval.completion_k ({k}), "
@@ -87,7 +89,7 @@ def sampler(config, batch_size, k):
                              "only; use 'dpm_solver' to pack several partials per call")
         return method, {"max_iters": config.sampling.get("max_iters", None)}
     if method == "ddim":
-        raise ValueError("eval_completion: sampling.method='ddim' is not supported; use 'dpm_solver' or 'pc'")
+        raise ValueError("eval_completion: sampling.method='ddim' is not supported; use 'dpm_solver', 'distilled' or 'pc'")
     raise ValueError(f"eval_completion: unknown sampling.method {method!r}")
 
 

@@ -127,6 +127,10 @@ def load_sources(path, R, C):
 
 def sampler_settings(config):
     method = str(config.sampling.method).lower()
+    if method == "distilled":
+        raise ValueError("edit: sampling.method='distilled' is not supported: RePaint resampling runs on the dpm_solver "
+                         "grid and jumps back up it, which a distilled student was not trained for; edit with the "
+                         "teacher's checkpoint and sampling.method='dpm_solver'")
     if method != "dpm_solver":
         logging.info("edit: sampling.method=%r is not used; editing samples with RePaint on the dpm_solver grid", method)
     return {"dpm_steps": int(config.sampling.get("dpm_steps", 25)), "dpm_sde": bool(config.sampling.get("dpm_sde", False)),

@@ -77,6 +77,9 @@ def _method(config, shape_endpoints):
         if isinstance(K, bool) or int(K) != K or K < 2:
             raise ValueError(f"sampling.dpm_steps must be an integer >= 2, got {K!r}")
         return method, int(K)
+    if method == "distilled":
+        raise ValueError("uncond_gen_interp: sampling.method='distilled' is not supported: interpolation and inversion "
+                         "run the dpm_solver ODE; use the teacher's checkpoint with sampling.method='dpm_solver'")
     if method == "ddim":
         if shape_endpoints:
             raise ValueError("uncond_gen_interp: shape endpoints need sampling.method='dpm_solver' (the inversion runs "

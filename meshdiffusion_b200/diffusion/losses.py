@@ -86,19 +86,18 @@ def get_ddpm_loss_fn(vpsde, train, mask=None, loss_type="l2"):
     return loss_fn
 
 
-def get_step_fn(sde, train, optimize_fn=None, mask=None, loss_type="l2"):
-    loss_fn = get_ddpm_loss_fn(sde, train, mask=mask, loss_type=loss_type)
+def get_update_fn(optimize_fn=None):
+    """`update(state, loss, update_param)`: the optimiser and EMA sequencing of a training micro-step, shared by
+    `--mode=train` and `--mode=distill`: backward, then (last micro-batch only) optimize_fn, then the micro-step counter
+    and the EMA, which advance on every micro-step (losses.py:104-139 of the reference)."""
     takes_ema = False
     if optimize_fn is not None:
         import inspect
         ps = inspect.signature(optimize_fn).parameters
         takes_ema = "ema" in ps or any(p.kind is inspect.Parameter.VAR_KEYWORD for p in ps.values())
 
-    def train_step(state, batch, clear_grad, update_param):
+    def update(state, loss, update_param):
         model, optimizer = state["model"], state["optimizer"]
-        if clear_grad:
-            optimizer.zero_grad()
-        loss = loss_fn(model, batch)
         loss.backward()
         ema_done = False
         if update_param:
@@ -107,6 +106,20 @@ def get_step_fn(sde, train, optimize_fn=None, mask=None, loss_type="l2"):
         state["step"] += 1
         if not ema_done:
             state["ema"].update(model.parameters())
+
+    return update
+
+
+def get_step_fn(sde, train, optimize_fn=None, mask=None, loss_type="l2"):
+    loss_fn = get_ddpm_loss_fn(sde, train, mask=mask, loss_type=loss_type)
+    update = get_update_fn(optimize_fn)
+
+    def train_step(state, batch, clear_grad, update_param):
+        model, optimizer = state["model"], state["optimizer"]
+        if clear_grad:
+            optimizer.zero_grad()
+        loss = loss_fn(model, batch)
+        update(state, loss, update_param)
         return loss
 
     def eval_step(state, batch):

@@ -8,7 +8,8 @@ both grid-mask multiplies), with the state resident in HBM and no host synchroni
 registered predictors / correctors use the same native network through `get_score_fn` with a few torch
 elementwise ops around it. `method='dpm_solver'` (no working reference counterpart) is the few-step DPM-Solver++(2M)
 sampler at the end of this file; `get_dpm_solver_inverter` runs its ODE form backwards (a grid's latent, for
-`--mode=uncond_gen_interp`).
+`--mode=uncond_gen_interp`). `method='distilled'` is the DDIM ODE on the halving grid of a progressively distilled
+student (`--mode=distill`), through the same solver code.
 """
 import abc
 import ctypes
@@ -75,6 +76,11 @@ def get_sampling_fn(config, sde, shape, inverse_scaler, eps, grid_mask=None, ret
                                       stochastic=config.sampling.get("dpm_sde", False),
                                       denoise=config.sampling.noise_removal, device=config.device, grid_mask=grid_mask,
                                       native_rng=config.sampling.get("native_rng", False), seed=config.get("seed", 42))
+    if method == "distilled":
+        return get_distilled_sampler(sde=sde, shape=shape, inverse_scaler=inverse_scaler,
+                                     n_steps=config.sampling.get("distill_steps", 8), device=config.device,
+                                     grid_mask=grid_mask, native_rng=config.sampling.get("native_rng", False),
+                                     seed=config.get("seed", 42))
     raise ValueError(f"Sampler name {method} unknown.")
 
 
@@ -463,6 +469,13 @@ def get_ddim_sampler(sde, shape, predictor, inverse_scaler, n_steps=1, denoise=F
 # in its ODE form and in the SDE form of k-diffusion's sample_dpmpp_2m_sde: a second-order multistep exponential
 # integrator in log-SNR time on the same noise prediction as the samplers above, one network evaluation per step, so a
 # sample costs ~25 evaluations instead of 999.
+def _vp_arrays(sde):
+    """float64 alpha_n = sqrt(alphas_cumprod[n]), sigma_n = sqrt(1 - alphas_cumprod[n]) and lambda_n = log(alpha_n / sigma_n)."""
+    abar = sde.alphas_cumprod.detach().to("cpu", torch.float64).numpy()
+    alpha, sigma = np.sqrt(abar), np.sqrt(1.0 - abar)
+    return alpha, sigma, np.log(alpha) - np.log(sigma)
+
+
 def dpm_solver_schedule(sde, n_steps, stochastic=False, denoise=True):
     """Label grid and step table of DPM-Solver++(2M) with `n_steps` (K) log-SNR intervals.
 
@@ -476,10 +489,8 @@ def dpm_solver_schedule(sde, n_steps, stochastic=False, denoise=True):
     if isinstance(n_steps, bool) or int(n_steps) != n_steps or n_steps < 2:
         raise ValueError(f"sampling.dpm_steps must be an integer >= 2, got {n_steps!r}")
     K = int(n_steps)
-    abar = sde.alphas_cumprod.detach().to("cpu", torch.float64).numpy()
-    N = abar.shape[0]
-    alpha, sigma = np.sqrt(abar), np.sqrt(1.0 - abar)
-    lam = np.log(alpha) - np.log(sigma)
+    alpha, sigma, lam = _vp_arrays(sde)
+    N = alpha.shape[0]
     targets = lam[N - 1] + np.arange(K + 1) * ((lam[0] - lam[N - 1]) / K)
     labels = []
     for t in targets:
@@ -523,10 +534,54 @@ def dpm_solver_inversion_schedule(sde, n_steps):
     discretisation error of both directions. Returns (labels, table)."""
     labels, _ = dpm_solver_schedule(sde, n_steps)
     labels = labels[::-1]
-    abar = sde.alphas_cumprod.detach().to("cpu", torch.float64).numpy()
-    alpha, sigma = np.sqrt(abar), np.sqrt(1.0 - abar)
-    lam = np.log(alpha) - np.log(sigma)
+    alpha, sigma, lam = _vp_arrays(sde)
     return labels, _solver_table(alpha, sigma, lam, labels)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Progressive distillation (Salimans & Ho, "Progressive Distillation for Fast Sampling of Diffusion Models", ICLR 2022) on
+# the halving DDIM grid: a student with K steps learns two DDIM steps of its 2K-step teacher per step of its own.
+DISTILL_COLUMNS = ("label_s", "label_m", "label_e", "sigma_s", "inv_alpha_s", "c_x_s", "c_0_s",
+                   "sigma_m", "inv_alpha_m", "c_x_m", "c_0_m", "r", "inv_d")
+
+
+def ddim_grid(sde, K):
+    """The K-step DDIM label grid l_i = round((N - 1)(1 - i / K)), i = 0 .. K, rounded half up in integer arithmetic:
+    l_0 = N - 1, l_K = 0, and the grid halves exactly (l^(K)_i = l^(2K)_{2i}). K must lie in [2, N - 1]; a finer grid
+    would repeat labels."""
+    N = sde.N
+    if isinstance(K, bool) or not isinstance(K, (int, np.integer)) or not 2 <= K <= N - 1:
+        raise ValueError(f"the DDIM grid needs an integer number of steps in [2, N - 1 = {N - 1}], got {K!r}")
+    K = int(K)
+    return [((N - 1) * (K - i) * 2 + K) // (2 * K) for i in range(K + 1)]
+
+
+def ddim_table(sde, labels):
+    """float64 first-order ODE rows (mdb_solver_step field order) along `labels`: row k is _solver_table's first-order
+    step labels[k] -> labels[k + 1], i.e. DDIM (c_1 = 0, c_z = 0, cond_coef / cond_std = alpha, sigma of labels[k + 1])."""
+    if len(labels) < 2:
+        raise ValueError("ddim_table needs at least two labels")
+    alpha, sigma, lam = _vp_arrays(sde)
+    return np.stack([_solver_table(alpha, sigma, lam, labels[k:k + 2])[0] for k in range(len(labels) - 1)])
+
+
+def distill_rows(sde, K_T):
+    """float64 rows [K_T / 2, 13] (DISTILL_COLUMNS, mdb_distill_row field order) of a round whose teacher takes K_T steps
+    on ddim_grid(sde, K_T). Row i: labels s = l_{2i}, m = l_{2i+1}, e = l_{2i+2}; the (sigma, inv_alpha, c_x, c_0) of the
+    teacher's DDIM steps s -> m and m -> e (ddim_table's rows 2i and 2i + 1); r = alpha_e / alpha_s and
+    inv_d = 1 / (sigma_e - alpha_e sigma_s / alpha_s), so that eps~ = (z_e - r z_s) inv_d is the noise prediction whose
+    single DDIM step from z_s lands on z_e."""
+    if isinstance(K_T, bool) or not isinstance(K_T, (int, np.integer)) or K_T % 2:
+        raise ValueError(f"a distillation round needs an even number of teacher steps, got {K_T!r}")
+    labels = ddim_grid(sde, K_T)
+    table = ddim_table(sde, labels)
+    alpha, sigma, _ = _vp_arrays(sde)
+    rows = np.zeros((K_T // 2, len(DISTILL_COLUMNS)), dtype=np.float64)
+    for i in range(K_T // 2):
+        s, m, e = labels[2 * i:2 * i + 3]
+        a, b = table[2 * i], table[2 * i + 1]
+        rows[i] = (s, m, e, *a[1:5], *b[1:5], alpha[e] / alpha[s], 1.0 / (sigma[e] - alpha[e] * sigma[s] / alpha[s]))
+    return rows
 
 
 def _solver_steps_c(table):
@@ -597,7 +652,7 @@ def _native_solver_loop(net, x, x0_hist, mask_flat, steps_c, seed, step0=0, n=No
 def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=False, denoise=True, device="cuda",
                            grid_mask=None, native_rng=False, seed=42):
     """Returns `dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None)`
-    -> (samples, number of network evaluations), the signature of pc_sampler.
+    -> (samples, number of network evaluations), the signature of pc_sampler, on dpm_solver_schedule's labels and table.
 
     The prior is pc_sampler's (sde.prior_sampling(shape) * grid_mask), or x0 * grid_mask when `x0` (shape `shape`) is
     given: no prior is drawn then. With `partial`, channel c is replaced before step 0
@@ -607,6 +662,20 @@ def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=Fa
     seed + rank and step); other CUDA states run model + mdb_solver_update per step with torch.randn_like noise; CPU
     tensors run the eager fp32 update (_solver_update_eager), which is the kernel's oracle."""
     labels, table = dpm_solver_schedule(sde, n_steps, stochastic, denoise)
+    return _table_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, "dpm_solver")
+
+
+def get_distilled_sampler(sde, shape, inverse_scaler, n_steps=8, device="cuda", grid_mask=None, native_rng=False, seed=42):
+    """The sampler of a progressively distilled student (`sampling.method='distilled'`, `sampling.distill_steps`): the
+    DDIM ODE on `ddim_grid(sde, n_steps)`, through get_dpm_solver_sampler's paths and conditioning with the first-order
+    rows of `ddim_table`. Same signature and return as get_dpm_solver_sampler."""
+    labels = ddim_grid(sde, n_steps)
+    return _table_sampler(sde, shape, inverse_scaler, labels, ddim_table(sde, labels), device, grid_mask, native_rng, seed,
+                          "distilled")
+
+
+def _table_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, name):
+    """The sampler behind get_dpm_solver_sampler and get_distilled_sampler on any solver table along `labels`."""
     rows32 = table.astype(np.float32)
     steps_c = _solver_steps_c(table)
     K_eff = len(labels) - 1
@@ -621,13 +690,13 @@ def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=Fa
             c = partial_channel
             B = shape[0]
             if x0 is not None and tuple(x0.shape) != tuple(shape):
-                raise ValueError(f"dpm_solver: x0 has shape {tuple(x0.shape)}, the sampler {tuple(shape)}")
+                raise ValueError(f"{name}: x0 has shape {tuple(x0.shape)}, the sampler {tuple(shape)}")
             x = sde.prior_sampling(shape).to(device) if x0 is None else x0.to(device=device, dtype=torch.float32)
             assert x.dim() == 5
             x = (x * grid_mask).contiguous()
             V = x[0, 0].numel()
             if grid_mask.numel() != V:
-                raise ValueError("dpm_solver: grid_mask must hold one value per voxel")
+                raise ValueError(f"{name}: grid_mask must hold one value per voxel")
             mask_v = grid_mask.to(device=x.device, dtype=torch.float32).reshape(x.shape[2:]).contiguous()
             cond, cond_until = None, 0
             if partial is not None:
@@ -732,9 +801,7 @@ def repaint_schedule(sde, n_steps, jump, resample, stochastic=False, denoise=Tru
             raise ValueError(f"repaint: {name} must be an integer >= 1, got {v!r}")
     jump, resample = int(jump), int(resample)
     labels, table = dpm_solver_schedule(sde, n_steps, stochastic, denoise)
-    abar = sde.alphas_cumprod.detach().to("cpu", torch.float64).numpy()
-    alpha, sigma = np.sqrt(abar), np.sqrt(1.0 - abar)
-    lam = np.log(alpha) - np.log(sigma)
+    alpha, sigma, lam = _vp_arrays(sde)
     K = len(labels) - 1
     rows = []
     for b0 in range(0, K, jump):

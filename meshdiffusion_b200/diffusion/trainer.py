@@ -82,24 +82,72 @@ def sync_replicas(state):
             dist.broadcast(t.data, src=0)
 
 
+def data_parallel_optimize_fn(config, net, **overrides):
+    """optimization_manager's optimize_fn after the data-parallel gradient mean (a wait when the backward pass already
+    overlapped the bucketed all-reduce, see ScoreNet.reduce_in_backward). `overrides` (lr, warmup, grad_clip) replace
+    the config's values."""
+    base_optimize_fn = losses.optimization_manager(config)
+
+    def optimize_fn(optimizer, params, step, **kw):
+        net.allreduce_grads()  # no-op on one GPU
+        return base_optimize_fn(optimizer, params, step=step, **{**kw, **overrides})
+
+    return optimize_fn
+
+
 def make_train_step(config, state, sde, mask):
     """`train_step_fn(state, batch, clear_grad, update_param)` exactly as train() uses it: losses.get_step_fn around an
     optimize_fn that first completes the data-parallel gradient mean (a wait when the backward pass already overlapped the
     bucketed all-reduce, see ScoreNet.reduce_in_backward) and then runs warm-up + clip + FusedAdam (+ EMA)."""
     net = state["model"].module
-    base_optimize_fn = losses.optimization_manager(config)
-
-    def optimize_fn(optimizer, params, step, **kw):
-        net.allreduce_grads()  # no-op on one GPU
-        return base_optimize_fn(optimizer, params, step=step, **kw)
-
-    step_fn = losses.get_step_fn(sde, train=True, optimize_fn=optimize_fn, mask=mask, loss_type=config.training.loss_type)
+    step_fn = losses.get_step_fn(sde, train=True, optimize_fn=data_parallel_optimize_fn(config, net), mask=mask,
+                                 loss_type=config.training.loss_type)
 
     def train_step_fn(state, batch, clear_grad=True, update_param=True):
         net.reduce_in_backward = bool(update_param)  # gradients are exchanged once per optimiser step
         return step_fn(state, batch, clear_grad=clear_grad, update_param=update_param)
 
     return train_step_fn
+
+
+def batch_source(config, mask, local_batch, rank=0, world=1):
+    """`next_batch(generator)` -> this rank's next training batch [local_batch, C, R, R, R] on config.device: on-device
+    synthetic grids (`data.synthetic`) or the dataset (trainer.py:64-75 of the reference)."""
+    device = config.device
+    R = config.data.image_size
+    synthetic = bool(config.data.get("synthetic", False))
+    data_iter = train_loader = sampler = None
+    epoch = 0
+    if not synthetic:
+        # trainer.py:64-75 of the reference: JSON list of per-shape grids, shuffled DataLoader; under torchrun every rank
+        # reads its own shard (DistributedSampler) instead of nn.DataParallel scattering one batch
+        from ..dataset.shapenet_dmtet_dataset import ShapeNetDMTetDataset
+        dataset = ShapeNetDMTetDataset(config.data.meta_path, deform_scale=config.model.get("deform_scale", 1.0), aug=True,
+                                       grid_mask=mask.cpu(), filter_meta_path=_path_or_none(config.data.get("filter_meta_path", None)),
+                                       normalize_sdf=config.data.get("normalize_sdf", True),
+                                       extension=config.data.get("extension", "pt"))
+        if world > 1:
+            sampler = torch.utils.data.distributed.DistributedSampler(dataset, num_replicas=world, rank=rank, shuffle=True,
+                                                                      seed=int(config.get("seed", 42)))
+        train_loader = torch.utils.data.DataLoader(dataset, batch_size=local_batch, shuffle=sampler is None,
+                                                   sampler=sampler, num_workers=config.data.get("num_workers", 0), pin_memory=True)
+        data_iter = iter(train_loader)
+
+    def next_batch(gen):
+        nonlocal data_iter, epoch
+        if synthetic:
+            return synthetic_grids(local_batch, R, device, gen) * mask
+        try:
+            batch = next(data_iter)
+        except StopIteration:
+            epoch += 1
+            if sampler is not None:
+                sampler.set_epoch(epoch)  # a new shuffle every epoch
+            data_iter = iter(train_loader)
+            batch = next(data_iter)
+        return batch.to(device, non_blocking=True)
+
+    return next_batch
 
 
 def train(config):
@@ -134,37 +182,7 @@ def train(config):
         raise ValueError(f"training.batch_size {config.training.batch_size} is not divisible by the {world} ranks")
     local_batch = config.training.batch_size // world
 
-    synthetic = bool(config.data.get("synthetic", False))
-    data_iter = train_loader = sampler = None
-    epoch = 0
-    if not synthetic:
-        # trainer.py:64-75 of the reference: JSON list of per-shape grids, shuffled DataLoader; under torchrun every rank
-        # reads its own shard (DistributedSampler) instead of nn.DataParallel scattering one batch
-        from ..dataset.shapenet_dmtet_dataset import ShapeNetDMTetDataset
-        dataset = ShapeNetDMTetDataset(config.data.meta_path, deform_scale=config.model.get("deform_scale", 1.0), aug=True,
-                                       grid_mask=mask.cpu(), filter_meta_path=_path_or_none(config.data.get("filter_meta_path", None)),
-                                       normalize_sdf=config.data.get("normalize_sdf", True),
-                                       extension=config.data.get("extension", "pt"))
-        if world > 1:
-            sampler = torch.utils.data.distributed.DistributedSampler(dataset, num_replicas=world, rank=rank, shuffle=True,
-                                                                      seed=int(config.get("seed", 42)))
-        train_loader = torch.utils.data.DataLoader(dataset, batch_size=local_batch, shuffle=sampler is None,
-                                                   sampler=sampler, num_workers=config.data.get("num_workers", 0), pin_memory=True)
-        data_iter = iter(train_loader)
-
-    def next_batch(gen):
-        nonlocal data_iter, epoch
-        if synthetic:
-            return synthetic_grids(local_batch, R, device, gen) * mask
-        try:
-            batch = next(data_iter)
-        except StopIteration:
-            epoch += 1
-            if sampler is not None:
-                sampler.set_epoch(epoch)  # a new shuffle every epoch
-            data_iter = iter(train_loader)
-            batch = next(data_iter)
-        return batch.to(device, non_blocking=True)
+    next_batch = batch_source(config, mask, local_batch, rank, world)
 
     iter_size = config.training.iter_size
     num_train_steps = config.training.n_iters
