@@ -158,39 +158,63 @@ int mdb_sampler_run(mdb_unet* net, float* x, float* x_mean, const float* mask, c
                     float* eps_buf, float* labels_buf, int step0, const mdb_sampler_cond* cond /* nullable */,
                     const float* cond_mean_coefs, const float* cond_stds, int cond_until, void* stream);
 
-/* Few-step sampling: DPM-Solver++(2M) (Lu et al. 2022), ODE or SDE form, on the same noise prediction as the sampler
- * above (diffusion/sampling.py: get_dpm_solver_sampler, which computes the step table in float64 on the host).
- * Step k runs the network at label n_k and moves x from n_k to n_{k+1}:
- *   x0 = (x - sigma eps) inv_alpha;   x' = (c_x x + c_0 x0 + c_1 x0_prev + c_z z) g;   x0_prev <- x0
- * with g the grid mask. c_1 = 0 marks a first-order step (x0_hist is not read); c_z = 0 one without noise. With `cond`,
- * channel `channel` is then replaced: x_c <- (x_c (1 - pm) + (cond_coef partial + cond_std z') pm) g (the mean_coef / std
- * fields of mdb_sampler_cond are ignored). */
-typedef struct mdb_solver_step {
-  float label;               /* network label n_k */
-  float sigma, inv_alpha;    /* x0 = (x - sigma*eps) * inv_alpha */
-  float c_x, c_0, c_1, c_z;  /* x' = c_x*x + c_0*x0 + c_1*x0_prev + c_z*z */
-  float cond_coef, cond_std; /* replacement after the step: alpha, sigma of n_{k+1} */
-} mdb_solver_step;
+/* Solver tables: few-step sampling with DPM-Solver++(2M) (Lu et al. 2022), ODE or SDE form, on the same noise prediction
+ * as the sampler above, its inverse (a grid's latent), the distilled student's DDIM grid, and RePaint resampling
+ * (Lugmayr et al. 2022) for shape editing (`--mode=edit`). diffusion/sampling.py computes every table in float64 on the
+ * host (dpm_solver_schedule, dpm_solver_inversion_schedule, ddim_table, repaint_schedule). An entry is one of two kinds,
+ * on x fp32 [B][C][V] with the grid mask g [V]:
+ *   denoise (kind 0): the network runs at `label`, then one DPM-Solver++(2M) step from that label to the next:
+ *            x0 = (x - sigma eps) inv_alpha;  x' = (c_x x + c_0 x0 + c_1 x0_prev + c_z z) g;  x0_prev <- x0
+ *            c_1 = 0 marks a first-order step (x0_prev is not read); c_z = 0 one without noise.
+ *   renoise (kind 1): a jump up the label grid by forward diffusion, no network: x' = (c_x x + c_z z) g with
+ *            c_x = alpha_hi / alpha_lo and c_z = sqrt(1 - c_x^2); x0_prev is not touched (sigma, inv_alpha, c_0, c_1 unused)
+ * With a kept region, both kinds then replace it on every channel c in `known->channels`:
+ *   x_c <- (x_c (1 - m) + (known_coef known_c + known_std z'_c) m) g
+ * with (known_coef, known_std) = alpha, sigma of the label the entry lands on. The conditional sampler (`cond_gen`) keeps
+ * one channel of a partial grid and stops replacing before its last step; a RePaint table ends with (1, 0), which makes
+ * the kept region of the output equal `known`. */
+typedef struct mdb_solver_entry {
+  int kind;                      /* 0 = denoise, 1 = renoise */
+  float label;                   /* denoise: network label; renoise: the label it jumps to */
+  float sigma, inv_alpha;        /* x0 = (x - sigma*eps) * inv_alpha */
+  float c_x, c_0, c_1, c_z;      /* x' = c_x*x + c_0*x0 + c_1*x0_prev + c_z*z */
+  float known_coef, known_std;   /* replacement after the entry */
+} mdb_solver_entry;
 
-/* One step, in place on x and x0_hist ([batch][channels][voxels] fp32; mask [voxels]). noise: z [batch][channels][voxels],
- * or NULL for Philox(seed, element, offset) as in mdb_sampler_update (a loop passes offset = 4 * k); cond->noise likewise
- * NULL for Philox(seed, element, offset + 2). */
-int mdb_solver_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_solver_step* step,
+/* The kept region. known: channel 0 of sample 0 of a [B][C][V] fp32 tensor; known_bstride is the element distance to the
+ * next sample (0 = one grid for the whole batch). mask: m [V] of sample 0, mask_bstride likewise. channels: bit c set =
+ * channel c is replaced (channels < 2^C). noise: z' [B][C][V], or NULL for Philox(seed, element, offset + 2). */
+typedef struct mdb_solver_known {
+  const float* known;
+  long long known_bstride;
+  const float* mask;
+  long long mask_bstride;
+  unsigned channels;
+  const float* noise;
+} mdb_solver_known;
+
+/* One entry, in place on x and x0_hist ([batch][channels][voxels] fp32; mask [voxels]). eps: the network output (denoise;
+ * ignored by renoise). noise: z [batch][channels][voxels], or NULL for Philox(seed, element, offset) with element the
+ * index in x, as in mdb_sampler_update (a loop passes offset = 4 * e for global entry e). known: nullable (no
+ * replacement). */
+int mdb_solver_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_solver_entry* entry,
                       long long voxels, int channels, int batch, const float* noise /* nullable */,
-                      unsigned long long seed, unsigned long long offset, const mdb_sampler_cond* cond /* nullable */,
+                      unsigned long long seed, unsigned long long offset, const mdb_solver_known* known /* nullable */,
                       void* stream);
-/* The whole solver loop without host round trips: for i < n_steps: steps[i].label -> network -> mdb_solver_update with
- * in-kernel Philox at offset 4 * (step0 + i), and the replacement while step0 + i < cond_until. `steps` is a HOST array of
- * n_steps entries for the global steps step0 .. step0 + n_steps - 1. eps_buf: device scratch [B][C][V]; labels_buf: device
- * scratch [B]. cond->noise must be NULL. The call only enqueues work. */
-int mdb_solver_run(mdb_unet* net, float* x, float* x0_hist, const float* mask, const mdb_solver_step* steps, int n_steps,
-                   int batch, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
-                   const mdb_sampler_cond* cond /* nullable */, int cond_until, void* stream);
+/* The whole table without host round trips: for i < n_entries: denoise entries run entries[i].label -> network
+ * (eps_buf) -> update, renoise entries the update alone, with in-kernel Philox at offset 4 * (step0 + i), and the
+ * replacement while step0 + i < replace_until. `entries` is a HOST array of n_entries entries for the global entries
+ * step0 .. step0 + n_entries - 1. eps_buf: device scratch [B][C][V]; labels_buf: device scratch [B]. known->noise must be
+ * NULL. The call only enqueues work. */
+int mdb_solver_run(mdb_unet* net, float* x, float* x0_hist, const float* mask, const mdb_solver_entry* entries,
+                   int n_entries, int batch, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
+                   const mdb_solver_known* known /* nullable */, int replace_until, void* stream);
 
 /* Progressive distillation (Salimans & Ho 2022; `--mode=distill`, diffusion/distill.py, with the rows computed in float64
  * on the host by diffusion/sampling.py: distill_rows). A student step i moves z from label s = l_{2i} to e = l_{2i+2} of
  * the teacher's DDIM grid l (ddim_grid); the teacher takes two first-order ODE (DDIM) steps s -> m = l_{2i+1} -> e, each
- * in mdb_solver_update's form with c_1 = c_z = 0:  x0 = (z - sigma eps) inv_alpha;  z' = (c_x z + c_0 x0) g.
+ * in the form of mdb_solver_update's denoise entry with c_1 = c_z = 0:  x0 = (z - sigma eps) inv_alpha;
+ *   z' = (c_x z + c_0 x0) g.
  * The student's target is the noise prediction whose single DDIM step from z_s lands on the teacher's z_e:
  *   eps~ = (z_e - r z_s) inv_d   with r = alpha_e / alpha_s and inv_d = 1 / (sigma_e - alpha_e sigma_s / alpha_s). */
 typedef struct mdb_distill_row {
@@ -204,7 +228,7 @@ typedef struct mdb_distill_row {
  * rows[step_idx[b]]; rows: DEVICE array of n_rows entries. An index outside [0, n_rows) reads no row: that sample's
  * outputs and label are NaN.
  *   phase 0 (teacher step s -> m, eps = teacher(z_s, s)): z_mid = (c_x_s z_s + c_0_s x0) g, bitwise mdb_solver_update's
- *           first-order step; labels[b] = m (the next forward's labels). out is not touched (may be NULL).
+ *           first-order denoise entry; labels[b] = m (the next forward's labels). out is not touched (may be NULL).
  *   phase 1 (teacher step m -> e, eps = teacher(z_mid, m)): z_e as above from z_mid, then out = ((z_e - r z_s) inv_d) g;
  *           labels[b] = s (the student's labels). z_mid is read only.
  * Every product and sum is rounded on its own. The call only enqueues work. */
@@ -218,53 +242,6 @@ int mdb_distill_step(const float* eps, const float* z_s, float* z_mid, float* ou
 int mdb_distill_targets(mdb_unet* teacher, const float* z_s, const int* step_idx, const mdb_distill_row* rows, int n_rows,
                         const float* mask, float* eps_target, float* labels, float* z_mid, float* eps_buf, int batch,
                         void* stream);
-
-/* Shape editing (`--mode=edit`): RePaint resampling (Lugmayr et al. 2022) on the DPM-Solver++(2M) label grid
- * (diffusion/sampling.py: repaint_schedule, get_repaint_sampler, which compute the entry table in float64 on the host).
- * An entry is one of two kinds, on x fp32 [B][C][V] with the grid mask g [V]:
- *   denoise (kind 0): the network runs at `label`, then mdb_solver_update's step without its replacement:
- *            x0 = (x - sigma eps) inv_alpha;  x' = (c_x x + c_0 x0 + c_1 x0_prev + c_z z) g;  x0_prev <- x0
- *   renoise (kind 1): a jump up the label grid by forward diffusion, no network: x' = (c_x x + c_z z) g with
- *            c_x = alpha_hi / alpha_lo and c_z = sqrt(1 - c_x^2); x0_prev is not touched (sigma, inv_alpha, c_0, c_1 unused)
- * Both kinds then replace the kept region on every channel c in `known->channels`:
- *   x_c <- (x_c (1 - m) + (known_coef known_c + known_std z'_c) m) g
- * with (known_coef, known_std) = alpha, sigma of the label the entry lands on, and (1, 0) on the last entry, which makes
- * the kept region of the output equal `known`. One channel in `channels` and a denoise-only table give mdb_solver_update's
- * arithmetic, rounding and Philox keys. */
-typedef struct mdb_repaint_entry {
-  int kind;                      /* 0 = denoise, 1 = renoise */
-  float label;                   /* denoise: network label; renoise: the label it jumps to */
-  float sigma, inv_alpha;
-  float c_x, c_0, c_1, c_z;
-  float known_coef, known_std;
-} mdb_repaint_entry;
-
-/* The kept region. known: channel 0 of sample 0 of a [B][C][V] fp32 tensor; known_bstride is the element distance to the
- * next sample (0 = one grid for the whole batch). mask: m [V] of sample 0, mask_bstride likewise. channels: bit c set =
- * channel c is replaced (channels < 2^C). noise: z' [B][C][V], or NULL for Philox(seed, element, offset + 2). */
-typedef struct mdb_repaint_known {
-  const float* known;
-  long long known_bstride;
-  const float* mask;
-  long long mask_bstride;
-  unsigned channels;
-  const float* noise;
-} mdb_repaint_known;
-
-/* One entry, in place on x and x0_hist ([batch][channels][voxels] fp32; mask [voxels]). eps: the network output (denoise;
- * ignored by renoise). noise: z [batch][channels][voxels], or NULL for Philox(seed, element, offset) with element the
- * index in x (a loop passes offset = 4 * e for global entry e). known: nullable (no replacement). */
-int mdb_repaint_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry* entry,
-                       long long voxels, int channels, int batch, const float* noise /* nullable */,
-                       unsigned long long seed, unsigned long long offset, const mdb_repaint_known* known /* nullable */,
-                       void* stream);
-/* The whole schedule without host round trips: for i < n_entries: denoise entries run entries[i].label -> network
- * (eps_buf) -> update, renoise entries the update alone, with in-kernel Philox at offset 4 * (step0 + i). `entries` is a
- * HOST array of n_entries entries for the global entries step0 .. step0 + n_entries - 1. eps_buf: device scratch [B][C][V];
- * labels_buf: device scratch [B]. known->noise must be NULL. The call only enqueues work. */
-int mdb_repaint_run(mdb_unet* net, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry* entries,
-                    int n_entries, int batch, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
-                    const mdb_repaint_known* known /* nullable */, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Training-step kernels (optimiser side). Replace get_ddpm_loss_fn's elementwise tail (lib/diffusion/losses.py:69-78),

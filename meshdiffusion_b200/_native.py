@@ -44,12 +44,6 @@ class SamplerCondC(ctypes.Structure):
     ]
 
 
-class SolverStepC(ctypes.Structure):
-    """mdb_solver_step (include/meshdiff_b200.h)."""
-    _fields_ = [(name, ctypes.c_float) for name in
-                ("label", "sigma", "inv_alpha", "c_x", "c_0", "c_1", "c_z", "cond_coef", "cond_std")]
-
-
 class DistillRowC(ctypes.Structure):
     """mdb_distill_row (include/meshdiff_b200.h)."""
     _fields_ = [(name, ctypes.c_float) for name in
@@ -57,15 +51,15 @@ class DistillRowC(ctypes.Structure):
                  "sigma_m", "inv_alpha_m", "c_x_m", "c_0_m", "r", "inv_d")]
 
 
-class RepaintEntryC(ctypes.Structure):
-    """mdb_repaint_entry (include/meshdiff_b200.h)."""
+class SolverEntryC(ctypes.Structure):
+    """mdb_solver_entry (include/meshdiff_b200.h)."""
     _fields_ = [("kind", ctypes.c_int)] + [(name, ctypes.c_float) for name in
                                            ("label", "sigma", "inv_alpha", "c_x", "c_0", "c_1", "c_z", "known_coef",
                                             "known_std")]
 
 
-class RepaintKnownC(ctypes.Structure):
-    """mdb_repaint_known (include/meshdiff_b200.h)."""
+class SolverKnownC(ctypes.Structure):
+    """mdb_solver_known (include/meshdiff_b200.h)."""
     _fields_ = [
         ("known", ctypes.c_void_p), ("known_bstride", ctypes.c_longlong),
         ("mask", ctypes.c_void_p), ("mask_bstride", ctypes.c_longlong),
@@ -107,16 +101,12 @@ SIGNATURES = {
     "mdb_sampler_update": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _f, _ll, _i, _i, _u64, _u64, ctypes.POINTER(SamplerCondC), _vp]),
     "mdb_sampler_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(_f), ctypes.POINTER(_f), ctypes.POINTER(_f), _i, _i, _u64, _vp, _vp,
                              _i, ctypes.POINTER(SamplerCondC), ctypes.POINTER(_f), ctypes.POINTER(_f), _i, _vp]),
-    "mdb_solver_update": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverStepC), _ll, _i, _i, _vp, _u64, _u64,
-                               ctypes.POINTER(SamplerCondC), _vp]),
-    "mdb_solver_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverStepC), _i, _i, _u64, _vp, _vp, _i,
-                            ctypes.POINTER(SamplerCondC), _i, _vp]),
+    "mdb_solver_update": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverEntryC), _ll, _i, _i, _vp, _u64, _u64,
+                               ctypes.POINTER(SolverKnownC), _vp]),
+    "mdb_solver_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverEntryC), _i, _i, _u64, _vp, _vp, _i,
+                            ctypes.POINTER(SolverKnownC), _i, _vp]),
     "mdb_distill_step": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _ll, _i, _i, _vp]),
     "mdb_distill_targets": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
-    "mdb_repaint_update": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(RepaintEntryC), _ll, _i, _i, _vp, _u64, _u64,
-                                ctypes.POINTER(RepaintKnownC), _vp]),
-    "mdb_repaint_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(RepaintEntryC), _i, _i, _u64, _vp, _vp, _i,
-                             ctypes.POINTER(RepaintKnownC), _vp]),
     "mdb_ddpm_loss": (_i, [_vp, _vp, _vp, _d, _vp, _vp, _vp, _i, _i, _ll, _vp]),
     "mdb_ddpm_perturb": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _ll, _vp]),
     "mdb_chunk_elems": (_i, []),

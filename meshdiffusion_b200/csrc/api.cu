@@ -295,6 +295,12 @@ __global__ void fill_kernel(float* p, float v, int n) {
   if (i < n) p[i] = v;
 }
 
+// eps_buf <- network(x) at `label` for every sample of the batch (labels_buf: device scratch [B])
+static void forward_at(mdb_unet* n, const float* x, float label, float* labels_buf, float* eps_buf, int B, cudaStream_t s) {
+  fill_kernel<<<(B + 127) / 128, 128, 0, s>>>(labels_buf, label, B);
+  n->net->forward(x, labels_buf, eps_buf, B, s, /*allow_graph=*/true);
+}
+
 int mdb_sampler_run(mdb_unet* n, float* x, float* x_mean, const float* mask, const float* labels, const float* betas,
                     const float* stds, int n_steps, int B, unsigned long long seed, float* eps_buf, float* labels_buf,
                     int step0, const mdb_sampler_cond* cond, const float* cond_mean_coefs, const float* cond_stds,
@@ -306,8 +312,7 @@ int mdb_sampler_run(mdb_unet* n, float* x, float* x_mean, const float* mask, con
   if (cond && cond->partial && (!cond_mean_coefs || !cond_stds)) throw std::runtime_error("mdb: conditional run needs the marginal_prob tables");
   if (cond && cond->noise) throw std::runtime_error("mdb: mdb_sampler_run draws its noise in-kernel (cond->noise must be NULL)");
   for (int i = 0; i < n_steps; ++i) {
-    fill_kernel<<<(B + 127) / 128, 128, 0, s>>>(labels_buf, labels[i], B);
-    n->net->forward(x, labels_buf, eps_buf, B, s, /*allow_graph=*/true);
+    forward_at(n, x, labels[i], labels_buf, eps_buf, B, s);
     SamplerUpdateArgs a{};
     a.eps = eps_buf; a.x = x; a.x_mean = x_mean; a.noise = nullptr; a.mask = mask; a.beta = betas[i]; a.stdv = stds[i];
     // curand_normal consumes two 32-bit Philox outputs and `offset` counts single outputs: 4*i gives every step its own
@@ -315,55 +320,6 @@ int mdb_sampler_run(mdb_unet* n, float* x, float* x_mean, const float* mask, con
     a.V = V; a.C = c.num_channels; a.seed = seed; a.offset = 4ull * (unsigned long long)(step0 + i);
     if (cond && step0 + i < cond_until) set_cond(a, cond, cond_mean_coefs[i], cond_stds[i]);
     launch_sampler_update(a, B, s);
-  }
-  MDB_API_END
-}
-
-static SolverUpdateArgs solver_args(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_solver_step& st,
-                                    long long V, int C, const mdb_sampler_cond* c) {
-  SolverUpdateArgs a{};
-  a.eps = eps; a.x = x; a.x0_hist = x0_hist; a.mask = mask;
-  a.sigma = st.sigma; a.inv_alpha = st.inv_alpha; a.c_x = st.c_x; a.c_0 = st.c_0; a.c_1 = st.c_1; a.c_z = st.c_z;
-  a.V = V; a.C = C;
-  if (c && c->partial) {
-    if (!c->partial_mask) throw std::runtime_error("mdb: conditional sampling needs partial_mask");
-    if (c->channel < 0 || c->channel >= C) throw std::runtime_error("mdb: partial_channel out of range");
-    a.cond_partial = c->partial; a.cond_partial_bs = c->partial_bstride;
-    a.cond_pmask = c->partial_mask; a.cond_pmask_bs = c->mask_bstride;
-    a.cond_channel = c->channel; a.cond_coef = st.cond_coef; a.cond_std = st.cond_std; a.cond_noise = c->noise;
-  }
-  return a;
-}
-
-int mdb_solver_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_solver_step* step,
-                      long long V, int C, int B, const float* noise, unsigned long long seed, unsigned long long offset,
-                      const mdb_sampler_cond* cond, void* stream) {
-  MDB_API_BEGIN
-  if (!step) throw std::runtime_error("mdb: mdb_solver_update needs a step");
-  if (V <= 0 || C <= 0 || B <= 0) throw std::runtime_error("mdb: mdb_solver_update needs positive voxels, channels, batch");
-  SolverUpdateArgs a = solver_args(eps, x, x0_hist, mask, *step, V, C, cond);
-  a.noise = noise; a.seed = seed; a.offset = offset;
-  launch_solver_update(a, B, (cudaStream_t)stream);
-  MDB_API_END
-}
-
-int mdb_solver_run(mdb_unet* n, float* x, float* x0_hist, const float* mask, const mdb_solver_step* steps, int n_steps,
-                   int B, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
-                   const mdb_sampler_cond* cond, int cond_until, void* stream) {
-  MDB_API_BEGIN
-  cudaStream_t s = (cudaStream_t)stream;
-  const UNetConfig& c = n->net->cfg();
-  const long long V = (long long)c.image_size * c.image_size * c.image_size;
-  if (n_steps > 0 && !steps) throw std::runtime_error("mdb: mdb_solver_run needs the step table");
-  if (cond && cond->noise) throw std::runtime_error("mdb: mdb_solver_run draws its noise in-kernel (cond->noise must be NULL)");
-  for (int i = 0; i < n_steps; ++i) {
-    fill_kernel<<<(B + 127) / 128, 128, 0, s>>>(labels_buf, steps[i].label, B);
-    n->net->forward(x, labels_buf, eps_buf, B, s, /*allow_graph=*/true);
-    SolverUpdateArgs a = solver_args(eps_buf, x, x0_hist, mask, steps[i], V, c.num_channels,
-                                     step0 + i < cond_until ? cond : nullptr);
-    // the same Philox counter blocks as mdb_sampler_run: 4 outputs per step, the replacement draw at +2
-    a.noise = nullptr; a.seed = seed; a.offset = 4ull * (unsigned long long)(step0 + i);
-    launch_solver_update(a, B, s);
   }
   MDB_API_END
 }
@@ -389,53 +345,51 @@ int mdb_distill_targets(mdb_unet* n, const float* z_s, const int* step_idx, cons
   MDB_API_END
 }
 
-static RepaintArgs repaint_args(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry& e,
-                                long long V, int C, const mdb_repaint_known* k) {
-  if (e.kind != 0 && e.kind != 1) throw std::runtime_error("mdb: repaint entry kind must be 0 (denoise) or 1 (renoise)");
-  RepaintArgs a{};
+static SolverEntryArgs entry_args(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_solver_entry& e,
+                                  long long V, int C, const mdb_solver_known* k) {
+  if (e.kind != 0 && e.kind != 1) throw std::runtime_error("mdb: solver entry kind must be 0 (denoise) or 1 (renoise)");
+  SolverEntryArgs a{};
   a.renoise = e.kind; a.eps = eps; a.x = x; a.x0_hist = x0_hist; a.mask = mask;
   a.sigma = e.sigma; a.inv_alpha = e.inv_alpha; a.c_x = e.c_x; a.c_0 = e.c_0; a.c_1 = e.c_1; a.c_z = e.c_z;
   a.V = V; a.C = C;
   if (k && k->known && k->channels) {
     if (!k->mask) throw std::runtime_error("mdb: the kept region needs its mask");
-    if (C > 32 || (C < 32 && (k->channels >> C) != 0u)) throw std::runtime_error("mdb: repaint channel set outside the channels");
+    if (C > 32 || (C < 32 && (k->channels >> C) != 0u)) throw std::runtime_error("mdb: kept channel set outside the channels");
     a.known = k->known; a.known_bs = k->known_bstride; a.kmask = k->mask; a.kmask_bs = k->mask_bstride;
     a.channels = k->channels; a.coef = e.known_coef; a.std = e.known_std; a.known_noise = k->noise;
   }
   return a;
 }
 
-int mdb_repaint_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry* entry,
-                       long long V, int C, int B, const float* noise, unsigned long long seed, unsigned long long offset,
-                       const mdb_repaint_known* known, void* stream) {
+int mdb_solver_update(const float* eps, float* x, float* x0_hist, const float* mask, const mdb_solver_entry* entry,
+                      long long V, int C, int B, const float* noise, unsigned long long seed, unsigned long long offset,
+                      const mdb_solver_known* known, void* stream) {
   MDB_API_BEGIN
-  if (!entry) throw std::runtime_error("mdb: mdb_repaint_update needs an entry");
-  if (V <= 0 || C <= 0 || B <= 0) throw std::runtime_error("mdb: mdb_repaint_update needs positive voxels, channels, batch");
-  RepaintArgs a = repaint_args(eps, x, x0_hist, mask, *entry, V, C, known);
+  if (!entry) throw std::runtime_error("mdb: mdb_solver_update needs an entry");
+  if (V <= 0 || C <= 0 || B <= 0) throw std::runtime_error("mdb: mdb_solver_update needs positive voxels, channels, batch");
+  SolverEntryArgs a = entry_args(eps, x, x0_hist, mask, *entry, V, C, known);
   if (!a.renoise && !eps) throw std::runtime_error("mdb: a denoise entry needs the network output");
   a.noise = noise; a.seed = seed; a.offset = offset;
-  launch_repaint_update(a, B, (cudaStream_t)stream);
+  launch_solver_entry(a, B, (cudaStream_t)stream);
   MDB_API_END
 }
 
-int mdb_repaint_run(mdb_unet* n, float* x, float* x0_hist, const float* mask, const mdb_repaint_entry* entries,
-                    int n_entries, int B, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
-                    const mdb_repaint_known* known, void* stream) {
+int mdb_solver_run(mdb_unet* n, float* x, float* x0_hist, const float* mask, const mdb_solver_entry* entries,
+                   int n_entries, int B, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
+                   const mdb_solver_known* known, int replace_until, void* stream) {
   MDB_API_BEGIN
   cudaStream_t s = (cudaStream_t)stream;
   const UNetConfig& c = n->net->cfg();
   const long long V = (long long)c.image_size * c.image_size * c.image_size;
-  if (n_entries > 0 && !entries) throw std::runtime_error("mdb: mdb_repaint_run needs the entry table");
-  if (known && known->noise) throw std::runtime_error("mdb: mdb_repaint_run draws its noise in-kernel (known->noise must be NULL)");
+  if (n_entries > 0 && !entries) throw std::runtime_error("mdb: mdb_solver_run needs the entry table");
+  if (known && known->noise) throw std::runtime_error("mdb: mdb_solver_run draws its noise in-kernel (known->noise must be NULL)");
   for (int i = 0; i < n_entries; ++i) {
-    RepaintArgs a = repaint_args(eps_buf, x, x0_hist, mask, entries[i], V, c.num_channels, known);
-    if (!a.renoise) {
-      fill_kernel<<<(B + 127) / 128, 128, 0, s>>>(labels_buf, entries[i].label, B);
-      n->net->forward(x, labels_buf, eps_buf, B, s, /*allow_graph=*/true);
-    }
-    // mdb_solver_run's Philox counter blocks, keyed by the global entry: 4 outputs per entry, the replacement draw at +2
+    SolverEntryArgs a = entry_args(eps_buf, x, x0_hist, mask, entries[i], V, c.num_channels,
+                                   step0 + i < replace_until ? known : nullptr);
+    if (!a.renoise) forward_at(n, x, entries[i].label, labels_buf, eps_buf, B, s);
+    // mdb_sampler_run's Philox counter blocks, keyed by the global entry: 4 outputs per entry, the replacement draw at +2
     a.noise = nullptr; a.seed = seed; a.offset = 4ull * (unsigned long long)(step0 + i);
-    launch_repaint_update(a, B, s);
+    launch_solver_entry(a, B, s);
   }
   MDB_API_END
 }

@@ -520,61 +520,4 @@ void launch_sampler_update(const SamplerUpdateArgs& a, int B, cudaStream_t s) {
   MDB_LAUNCH_CHECK();
 }
 
-// ------------------------------------------------------------------ DPM-Solver++(2M) update
-// Every product and sum is rounded on its own (no FMA contraction), in this order:
-//   x0 = (x - sigma*eps) * inv_alpha
-//   x' = ((c_x*x + c_0*x0) + c_1*x0_prev) + c_z*z       (c_1 term only if c_1 != 0, c_z term only if c_z != 0)
-//   x' = x' * g
-//   channel c: s = coef*partial + std*z';  x' = (x'*(1-pm) + s*pm) * g
-// The eager torch update in diffusion/sampling.py (_solver_update_eager) does the same operations in the same order,
-// so given the same eps and noise the two are bit-identical.
-__global__ void solver_update_kernel(SolverUpdateArgs a, int B) {
-  const long long per = a.V * a.C;
-  const long long total = per * B;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const long long v = i % a.V;
-    const float m = __ldg(a.mask + v);
-    const float xv = a.x[i];
-    const float x0 = __fmul_rn(__fsub_rn(xv, __fmul_rn(a.sigma, a.eps[i])), a.inv_alpha);
-    float xn = __fadd_rn(__fmul_rn(a.c_x, xv), __fmul_rn(a.c_0, x0));
-    if (a.c_1 != 0.f) xn = __fadd_rn(xn, __fmul_rn(a.c_1, a.x0_hist[i]));
-    if (a.c_z != 0.f) {
-      float z;
-      if (a.noise) {
-        z = a.noise[i];
-      } else {
-        curandStatePhilox4_32_10_t st;
-        curand_init(a.seed, (unsigned long long)i, a.offset, &st);
-        z = curand_normal(&st);
-      }
-      xn = __fadd_rn(xn, __fmul_rn(a.c_z, z));
-    }
-    xn = __fmul_rn(xn, m);
-    if (a.cond_partial) {
-      const long long bc = i / a.V;
-      if ((int)(bc % a.C) == a.cond_channel) {
-        const long long b = bc / a.C;
-        const float pm = __ldg(a.cond_pmask + b * a.cond_pmask_bs + v);
-        const float pv = __ldg(a.cond_partial + b * a.cond_partial_bs + v);
-        float z2;
-        if (a.cond_noise) {
-          z2 = a.cond_noise[b * a.V + v];
-        } else {
-          curandStatePhilox4_32_10_t st;
-          curand_init(a.seed, (unsigned long long)i, a.offset + 2, &st);
-          z2 = curand_normal(&st);
-        }
-        const float sampled = __fadd_rn(__fmul_rn(a.cond_coef, pv), __fmul_rn(a.cond_std, z2));
-        xn = __fmul_rn(__fadd_rn(__fmul_rn(xn, __fsub_rn(1.f, pm)), __fmul_rn(sampled, pm)), m);
-      }
-    }
-    a.x[i] = xn;
-    a.x0_hist[i] = x0;
-  }
-}
-void launch_solver_update(const SolverUpdateArgs& a, int B, cudaStream_t s) {
-  solver_update_kernel<<<grid_for(a.V * a.C * B, 256), 256, 0, s>>>(a, B);
-  MDB_LAUNCH_CHECK();
-}
-
 }  // namespace mdb

@@ -84,33 +84,14 @@ struct SamplerUpdateArgs {
 };
 void launch_sampler_update(const SamplerUpdateArgs& a, int B, cudaStream_t s);
 
-// One DPM-Solver++(2M) step (ODE or SDE form), in place, fp32 NCDHW [B][C][V]; mask [V]:
-//   x0 = (x - sigma eps) inv_alpha;  x' = (c_x x + c_0 x0 [+ c_1 x0_prev] [+ c_z z]) g;  x0_hist <- x0
-// then, when cond_partial != nullptr, on channel cond_channel: x_c <- (x_c (1-pm) + (coef partial + std z') pm) g.
-// The c_1 term is skipped when c_1 == 0 (first-order step: x0_hist is not read) and the noise term when c_z == 0.
-struct SolverUpdateArgs {
-  const float* eps;    // network output
-  float* x;            // in/out state
-  float* x0_hist;      // in: x0 of the previous step, out: x0 of this step
-  const float* mask;   // [V]
-  float sigma, inv_alpha, c_x, c_0, c_1, c_z;
-  long long V; int C;
-  const float* noise;               // z ~ N(0,1) [B][C][V] or null (then Philox(seed, element, offset))
-  unsigned long long seed, offset;
-  const float* cond_partial; long long cond_partial_bs;  // channel c of sample 0, sample stride (0 = shared grid)
-  const float* cond_pmask; long long cond_pmask_bs;
-  int cond_channel;
-  float cond_coef, cond_std;        // alpha, sigma of the label the step lands on
-  const float* cond_noise;          // z' [B][V] or null (then Philox(seed, element, offset + 2))
-};
-void launch_solver_update(const SolverUpdateArgs& a, int B, cudaStream_t s);
-
-// One entry of a RePaint resampling schedule (csrc/repaint.cu), in place, fp32 NCDHW [B][C][V]; mask [V]:
-//   denoise: solver_update_kernel's step without its replacement (x0_hist <- x0)
+// One entry of a solver table (csrc/solver.cu), in place, fp32 NCDHW [B][C][V]; mask g [V]:
+//   denoise: x0 = (x - sigma eps) inv_alpha;  x' = (c_x x + c_0 x0 [+ c_1 x0_prev] [+ c_z z]) g;  x0_hist <- x0
+//            (the c_1 term is skipped when c_1 == 0, a first-order step that does not read x0_hist; the noise term when
+//            c_z == 0)
 //   renoise: x' = (c_x x + c_z z) g   (c_x = alpha_hi / alpha_lo, c_z = sqrt(1 - c_x^2); x0_hist untouched)
 // then, when known != nullptr, on every channel c with bit c of `channels` set:
 //   x_c <- (x_c (1 - m) + (coef known_c + std z'_c) m) g
-struct RepaintArgs {
+struct SolverEntryArgs {
   int renoise;
   const float* eps;    // network output (denoise)
   float* x;            // in/out state
@@ -123,9 +104,9 @@ struct RepaintArgs {
   const float* known; long long known_bs;  // [C][V] of sample 0, sample stride (0 = shared)
   const float* kmask; long long kmask_bs;  // m [V] of sample 0, sample stride (0 = shared)
   unsigned channels;
-  float coef, std;                  // alpha, sigma of the label the entry lands on; (1, 0) on the last entry
+  float coef, std;                  // alpha, sigma of the label the entry lands on
   const float* known_noise;         // z' [B][C][V] or null (then Philox(seed, element, offset + 2))
 };
-void launch_repaint_update(const RepaintArgs& a, int B, cudaStream_t s);
+void launch_solver_entry(const SolverEntryArgs& a, int B, cudaStream_t s);
 
 }  // namespace mdb

@@ -12,6 +12,7 @@ sampler at the end of this file; `get_dpm_solver_inverter` runs its ODE form bac
 student (`--mode=distill`), through the same solver code.
 """
 import abc
+import contextlib
 import ctypes
 
 import numpy as np
@@ -218,8 +219,7 @@ def _native_net(model):
 class _Cond:
     """Replacement conditioning of the partial branch (sampling.py:453-467 of the reference) in the form the update kernel
     takes it: channel `c` of `partial` / `partial_mask` (batch 1 = one grid shared by all samples, or one per sample) and
-    the per-step marginal_prob scalars, computed with the reference's torch ops so they are bit-identical. The DPM-Solver
-    sampler passes timesteps=None: its per-step scalars are in the solver's step table."""
+    the per-step marginal_prob scalars, computed with the reference's torch ops so they are bit-identical."""
 
     def __init__(self, sde, partial, partial_mask, c, timesteps, B):
         V = partial[0, 0].numel()
@@ -231,8 +231,6 @@ class _Cond:
                 raise ValueError("partial / partial_mask must have batch 1 or the sampling batch")
         self.pb = V if self.partial.shape[0] == B and B > 1 else 0
         self.mb = V if self.pmask.shape[0] == B and B > 1 else 0
-        if timesteps is None:
-            return
         lmc = -0.25 * timesteps ** 2 * (sde.beta_1 - sde.beta_0) - 0.5 * timesteps * sde.beta_0  # sde_lib.py:211
         self.coefs = torch.exp(lmc).cpu().tolist()
         self.stds = torch.sqrt(1.0 - torch.exp(2.0 * lmc)).cpu().tolist()
@@ -317,15 +315,11 @@ def get_pc_sampler(sde, shape, predictor, corrector, inverse_scaler, snr, n_step
             traj = []
             if use_fused:
                 net._ensure_engine(B, x.device)
-                net.sync_parameters()
-                net._frozen = True  # nobody edits the weights inside the loop: skip per-step change detection
-            try:
+            # nobody edits the weights inside the loop: skip per-step change detection
+            with net.frozen() if use_fused else contextlib.nullcontext():
                 return _run(model, net, x, use_fused, partial, partial_mask, c, freeze_iters, timesteps, B, traj,
                             betas if use_fused else None, stds if use_fused else None,
                             labels_all if use_fused else None, mask_flat if use_fused else None)
-            finally:
-                if use_fused:
-                    net._frozen = False  # also on OOM / NativeError / KeyboardInterrupt inside the loop
 
     def _run(model, net, x, use_fused, partial, partial_mask, c, freeze_iters, timesteps, B, traj, betas, stds,
              labels_all, mask_flat):
@@ -482,8 +476,8 @@ def dpm_solver_schedule(sde, n_steps, stochastic=False, denoise=True):
     With alpha_n = sqrt(alphas_cumprod[n]), sigma_n = sqrt(1 - alphas_cumprod[n]) and lambda_n = log alpha_n - log sigma_n
     (float64), the labels are the ones whose lambda is nearest each of K + 1 equally spaced targets from lambda_{N-1} to
     lambda_0, repeats dropped: labels[0] = N - 1, labels[-1] = 0, K_eff = len(labels) - 1 network evaluations (K_eff < K
-    only when two targets share a label, near label 0). Row k of the table (float64, mdb_solver_step field order: label,
-    sigma, inv_alpha, c_x, c_0, c_1, c_z, cond_coef, cond_std) moves x from labels[k] to labels[k + 1]:
+    only when two targets share a label, near label 0). Row k of the table (float64, the fields of mdb_solver_entry after
+    `kind`: label, sigma, inv_alpha, c_x, c_0, c_1, c_z, known_coef, known_std) moves x from labels[k] to labels[k + 1]:
     x' = c_x x + c_0 x0_k + c_1 x0_{k-1} + c_z z with x0_k = (x - sigma eps) inv_alpha. Step 0 is first order (c_1 = 0);
     with `denoise` the last SDE step adds no noise. Returns (labels, table)."""
     if isinstance(n_steps, bool) or int(n_steps) != n_steps or n_steps < 2:
@@ -557,8 +551,8 @@ def ddim_grid(sde, K):
 
 
 def ddim_table(sde, labels):
-    """float64 first-order ODE rows (mdb_solver_step field order) along `labels`: row k is _solver_table's first-order
-    step labels[k] -> labels[k + 1], i.e. DDIM (c_1 = 0, c_z = 0, cond_coef / cond_std = alpha, sigma of labels[k + 1])."""
+    """float64 first-order ODE rows (dpm_solver_schedule's columns) along `labels`: row k is _solver_table's first-order
+    step labels[k] -> labels[k + 1], i.e. DDIM (c_1 = 0, c_z = 0, known_coef / known_std = alpha, sigma of labels[k + 1])."""
     if len(labels) < 2:
         raise ValueError("ddim_table needs at least two labels")
     alpha, sigma, lam = _vp_arrays(sde)
@@ -584,198 +578,6 @@ def distill_rows(sde, K_T):
     return rows
 
 
-def _solver_steps_c(table):
-    """The step table as the float32 mdb_solver_step array the library takes."""
-    rows = table.astype(np.float32)
-    arr = (_native.SolverStepC * len(rows))()
-    for i, r in enumerate(rows):
-        arr[i] = _native.SolverStepC(*(float(v) for v in r))
-    return arr
-
-
-def _replace_channel(xc, partial, pmask, mask, coef, std, z):
-    """x_c <- (x_c (1 - pm) + (coef partial + std z) pm) g, fp32, in solver_update_kernel's operation order."""
-    sampled = partial * coef + z * std
-    return (xc * (1.0 - pmask) + sampled * pmask) * mask
-
-
-def _solver_update_eager(eps, x, x0_hist, mask, row, noise=None, cond=None, cond_noise=None):
-    """One solver step in torch fp32 ops, in place on x and x0_hist, with the operation order of solver_update_kernel (each
-    product and sum rounded on its own), so it is the kernel's bit-exact oracle. `row`: a float32 table row; `mask`
-    broadcasts over x; `cond`: a _Cond."""
-    label, sg, inv_a, c_x, c_0, c_1, c_z, coef, std = (float(v) for v in row)
-    x0 = (x - eps * sg) * inv_a
-    xn = x * c_x + x0 * c_0
-    if c_1 != 0.0:
-        xn = xn + x0_hist * c_1
-    if c_z != 0.0:
-        xn = xn + noise * c_z
-    xn = xn * mask
-    if cond is not None:
-        xn[:, cond.c] = _replace_channel(xn[:, cond.c], cond.partial, cond.pmask, mask, coef, std, cond_noise)
-    x0_hist.copy_(x0)
-    x.copy_(xn)
-    return x
-
-
-def _solver_update(eps, x, x0_hist, mask_flat, row_c, noise=None, cond=None, cond_noise=None, seed=0, offset=0):
-    """One step through mdb_solver_update, in place on x and x0_hist; noise=None draws it in-kernel."""
-    L = _native.lib()
-    B, C = x.shape[0], x.shape[1]
-    cs = cond.struct(noise=cond_noise) if cond is not None else None
-    _native.check(L.mdb_solver_update(_native.ptr(eps), _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat),
-                                      ctypes.byref(row_c), x[0, 0].numel(), C, B, _native.ptr(noise), int(seed),
-                                      int(offset), ctypes.byref(cs) if cs is not None else None,
-                                      _native.current_stream()))
-    return x
-
-
-def _native_solver_loop(net, x, x0_hist, mask_flat, steps_c, seed, step0=0, n=None, cond=None, cond_until=0):
-    """Steps step0 .. step0+n-1 of the solver loop inside the library (mdb_solver_run), in place on x and x0_hist.
-    `steps_c` is the whole table (_solver_steps_c), indexed by the GLOBAL step."""
-    L = _native.lib()
-    B = x.shape[0]
-    n = len(steps_c) - step0 if n is None else n
-    net._ensure_engine(B, x.device)
-    net.sync_parameters()
-    eps_buf = torch.empty_like(x)
-    labels_buf = torch.empty(B, device=x.device, dtype=torch.float32)
-    part = (_native.SolverStepC * n).from_buffer(steps_c, step0 * ctypes.sizeof(_native.SolverStepC))
-    cs = cond.struct() if cond is not None else None
-    _native.check(L.mdb_solver_run(net._handle, _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat), part, n, B,
-                                   int(seed), _native.ptr(eps_buf), _native.ptr(labels_buf), int(step0),
-                                   ctypes.byref(cs) if cs is not None else None, int(cond_until),
-                                   _native.current_stream()))
-    return x
-
-
-def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=False, denoise=True, device="cuda",
-                           grid_mask=None, native_rng=False, seed=42):
-    """Returns `dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None)`
-    -> (samples, number of network evaluations), the signature of pc_sampler, on dpm_solver_schedule's labels and table.
-
-    The prior is pc_sampler's (sde.prior_sampling(shape) * grid_mask), or x0 * grid_mask when `x0` (shape `shape`) is
-    given: no prior is drawn then. With `partial`, channel c is replaced before step 0
-    (alpha, sigma of label N-1) and after every step k but the last whose label n_k has N-1-n_k < freeze_iters (alpha,
-    sigma of n_{k+1}), with fresh per-sample noise; the x0 history keeps the network's prediction. Paths: on CUDA with
-    `native_rng` and a native ScoreNet the whole loop runs in the library (mdb_solver_run, Philox noise keyed by
-    seed + rank and step); other CUDA states run model + mdb_solver_update per step with torch.randn_like noise; CPU
-    tensors run the eager fp32 update (_solver_update_eager), which is the kernel's oracle."""
-    labels, table = dpm_solver_schedule(sde, n_steps, stochastic, denoise)
-    return _table_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, "dpm_solver")
-
-
-def get_distilled_sampler(sde, shape, inverse_scaler, n_steps=8, device="cuda", grid_mask=None, native_rng=False, seed=42):
-    """The sampler of a progressively distilled student (`sampling.method='distilled'`, `sampling.distill_steps`): the
-    DDIM ODE on `ddim_grid(sde, n_steps)`, through get_dpm_solver_sampler's paths and conditioning with the first-order
-    rows of `ddim_table`. Same signature and return as get_dpm_solver_sampler."""
-    labels = ddim_grid(sde, n_steps)
-    return _table_sampler(sde, shape, inverse_scaler, labels, ddim_table(sde, labels), device, grid_mask, native_rng, seed,
-                          "distilled")
-
-
-def _table_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, name):
-    """The sampler behind get_dpm_solver_sampler and get_distilled_sampler on any solver table along `labels`."""
-    rows32 = table.astype(np.float32)
-    steps_c = _solver_steps_c(table)
-    K_eff = len(labels) - 1
-    N = sde.N
-    abar_T = float(sde.alphas_cumprod[N - 1])
-    a_T, s_T = (float(np.float32(v)) for v in (np.sqrt(abar_T), np.sqrt(1.0 - abar_T)))  # alpha, sigma of label N - 1
-
-    def dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None):
-        with torch.no_grad():
-            if freeze_iters is None:
-                freeze_iters = N + 10
-            c = partial_channel
-            B = shape[0]
-            if x0 is not None and tuple(x0.shape) != tuple(shape):
-                raise ValueError(f"{name}: x0 has shape {tuple(x0.shape)}, the sampler {tuple(shape)}")
-            x = sde.prior_sampling(shape).to(device) if x0 is None else x0.to(device=device, dtype=torch.float32)
-            assert x.dim() == 5
-            x = (x * grid_mask).contiguous()
-            V = x[0, 0].numel()
-            if grid_mask.numel() != V:
-                raise ValueError(f"{name}: grid_mask must hold one value per voxel")
-            mask_v = grid_mask.to(device=x.device, dtype=torch.float32).reshape(x.shape[2:]).contiguous()
-            cond, cond_until = None, 0
-            if partial is not None:
-                assert partial.dim() == 5
-                cond = _Cond(sde, partial.to(x.device), partial_mask.to(x.device), c, None, B)
-                z = torch.randn_like(x[:, c])
-                x[:, c] = _replace_channel(x[:, c], cond.partial, cond.pmask, mask_v, a_T, s_T, z)
-                cond_until = sum(1 for k in range(K_eff - 1) if N - 1 - labels[k] < freeze_iters)
-            x0_hist = torch.empty_like(x)
-            net = _native_net(model)
-            if x.is_cuda and native_rng and net is not None:
-                net._ensure_engine(B, x.device)
-                net.sync_parameters()
-                net._frozen = True  # nobody edits the weights inside the loop: skip per-step change detection
-                try:
-                    _native_solver_loop(net, x, x0_hist, mask_v.reshape(-1), steps_c, seed + _rank(), cond=cond,
-                                        cond_until=cond_until)
-                finally:
-                    net._frozen = False
-                return inverse_scaler(x), K_eff
-            for k in range(K_eff):
-                eps_out = model(x, torch.full((B,), float(labels[k]), device=x.device))
-                z = torch.randn_like(x) if rows32[k, 6] != 0 else None
-                ck = cond if k < cond_until else None
-                z2 = torch.randn_like(x[:, c]).contiguous() if ck is not None else None
-                if x.is_cuda:
-                    _solver_update(eps_out.float().contiguous(), x, x0_hist, mask_v.reshape(-1), steps_c[k], z, ck, z2)
-                else:
-                    _solver_update_eager(eps_out.float(), x, x0_hist, mask_v, rows32[k], z, ck, z2)
-            return inverse_scaler(x), K_eff
-
-    return dpm_solver_sampler
-
-
-def get_dpm_solver_inverter(sde, shape, n_steps=25, grid_mask=None, device="cuda"):
-    """Returns `invert(model, x) -> (z, number of network evaluations)`: the latent at label N - 1 of grids x (shape
-    `shape`), taken as the state at label 0 after the grid mask is applied, by the ODE form of DPM-Solver++(2M) run
-    backwards (dpm_solver_inversion_schedule). The dpm_solver sampler with the same `n_steps`, started from z
-    (x0=z), maps it back to x up to discretisation error. No noise is drawn. Paths: a native ScoreNet on CUDA runs the
-    whole loop in the library (mdb_solver_run); other CUDA models run model + mdb_solver_update per step; CPU tensors run
-    the eager fp32 update."""
-    labels, table = dpm_solver_inversion_schedule(sde, n_steps)
-    rows32 = table.astype(np.float32)
-    steps_c = _solver_steps_c(table)
-    K_eff = len(labels) - 1
-
-    def invert(model, x):
-        with torch.no_grad():
-            if tuple(x.shape) != tuple(shape):
-                raise ValueError(f"dpm_solver inversion: x has shape {tuple(x.shape)}, expected {tuple(shape)}")
-            B = shape[0]
-            x = x.to(device=device, dtype=torch.float32)
-            V = x[0, 0].numel()
-            if grid_mask.numel() != V:
-                raise ValueError("dpm_solver inversion: grid_mask must hold one value per voxel")
-            mask_v = grid_mask.to(device=x.device, dtype=torch.float32).reshape(x.shape[2:]).contiguous()
-            x = (x * mask_v).contiguous()
-            x0_hist = torch.empty_like(x)
-            net = _native_net(model)
-            if x.is_cuda and net is not None:
-                net._ensure_engine(B, x.device)
-                net.sync_parameters()
-                net._frozen = True  # nobody edits the weights inside the loop: skip per-step change detection
-                try:
-                    _native_solver_loop(net, x, x0_hist, mask_v.reshape(-1), steps_c, 0)
-                finally:
-                    net._frozen = False
-                return x, K_eff
-            for k in range(K_eff):
-                eps_out = model(x, torch.full((B,), float(labels[k]), device=x.device))
-                if x.is_cuda:
-                    _solver_update(eps_out.float().contiguous(), x, x0_hist, mask_v.reshape(-1), steps_c[k])
-                else:
-                    _solver_update_eager(eps_out.float(), x, x0_hist, mask_v, rows32[k])
-            return x, K_eff
-
-    return invert
-
-
 # ------------------------------------------------------------------------------------------------------------------
 # RePaint resampling (Lugmayr et al., "RePaint: Inpainting using Denoising Diffusion Probabilistic Models", CVPR 2022) on
 # the DPM-Solver++(2M) label grid, for shape editing: the kept region is replaced on every step, and every block of
@@ -789,7 +591,7 @@ def repaint_schedule(sde, n_steps, jump, resample, stochastic=False, denoise=Tru
 
     The K_eff solver steps are cut into blocks of `jump` steps. Every block but the last runs `resample` times, with a
     renoise entry from the block's last label lo back to its first label hi between two runs; the last block runs once.
-    Rows (float64, mdb_repaint_entry field order, REPAINT_COLUMNS):
+    Rows (float64, mdb_solver_entry field order, REPAINT_COLUMNS):
       denoise (kind 0): the solver step's row (label, sigma, inv_alpha, c_x, c_0, c_1, c_z, alpha, sigma of the label it
         lands on); the first step of a repeated run is first order (c_1 = 0), since the x0 history belongs to the
         abandoned run;
@@ -822,35 +624,58 @@ def repaint_schedule(sde, n_steps, jump, resample, stochastic=False, denoise=Tru
     return out, int((out[:, 0] == 0).sum())
 
 
-def _repaint_entries_c(table):
-    """The entry table as the float32 mdb_repaint_entry array the library takes."""
-    rows = table.astype(np.float32)
-    arr = (_native.RepaintEntryC * len(rows))()
+# ------------------------------------------------------------------------------------------------------------------
+# Every table above -- DPM-Solver++(2M)'s and its inverse's (9 columns, all denoise entries), the distilled student's DDIM
+# rows and RePaint's (REPAINT_COLUMNS) -- runs through one update kernel (mdb_solver_update) and one device loop
+# (mdb_solver_run); _update_eager is the kernel's bit-exact CPU oracle.
+def _rows32(table):
+    """The table as float32 REPAINT_COLUMNS rows: a 9-column solver table gets kind 0 (denoise) on every row."""
+    rows = np.asarray(table, dtype=np.float64)
+    if rows.shape[1] == len(REPAINT_COLUMNS) - 1:
+        rows = np.concatenate([np.zeros((len(rows), 1)), rows], axis=1)
+    return rows.astype(np.float32)
+
+
+def _entries_c(table):
+    """The table (a 9-column solver table or REPAINT_COLUMNS) as the float32 mdb_solver_entry array the library takes."""
+    rows = _rows32(table)
+    arr = (_native.SolverEntryC * len(rows))()
     for i, r in enumerate(rows):
-        arr[i] = _native.RepaintEntryC(int(r[0]), *(float(v) for v in r[1:]))
+        arr[i] = _native.SolverEntryC(int(r[0]), *(float(v) for v in r[1:]))
     return arr
 
 
 class _Known:
     """The kept region in the form the update kernel takes it: `known` fp32 [1 or B, C, R, R, R] (what the output must
     hold there), `mask` fp32 [1 or B, R, R, R] (1 = kept voxel; 1 / B samples = shared / per sample) and the replaced
-    channels."""
+    channels. The per-entry CUDA and CPU paths draw the replacement noise z' with torch.randn_like: one draw the shape
+    of x (`full_noise`, RePaint), or one [B, R, R, R] draw per replaced channel (the conditional sampler's draw order)."""
 
-    def __init__(self, known, mask, channels, B):
+    def __init__(self, known, mask, channels, B, full_noise=True):
         self.known = known.to(torch.float32).contiguous()
         C = self.known.shape[1]
         self.mask = mask.to(torch.float32).reshape(mask.shape[0], *self.known.shape[2:]).contiguous()
         for t in (self.known, self.mask):
             if t.shape[0] not in (1, B):
-                raise ValueError("repaint: known / known_mask must have batch 1 or the sampling batch")
+                raise ValueError("the kept region (known / mask) must have batch 1 or the sampling batch")
         self.channels = sorted({int(c) for c in channels})
         if not self.channels or self.channels[0] < 0 or self.channels[-1] >= C:
-            raise ValueError(f"repaint: channels must be a non-empty subset of 0 .. {C - 1}, got {channels!r}")
+            raise ValueError(f"kept region: channels must be a non-empty subset of 0 .. {C - 1}, got {channels!r}")
         self.kb = self.known[0].numel() if self.known.shape[0] == B and B > 1 else 0
         self.mb = self.mask[0].numel() if self.mask.shape[0] == B and B > 1 else 0
+        self.full_noise = full_noise
+
+    def noise(self, x):
+        """z' shaped like x (zero outside the replaced channels when not `full_noise`)."""
+        if self.full_noise:
+            return torch.randn_like(x)
+        z = torch.zeros_like(x)
+        for c in self.channels:
+            z[:, c] = torch.randn_like(x[:, c])
+        return z
 
     def struct(self, noise=None):
-        s = _native.RepaintKnownC()
+        s = _native.SolverKnownC()
         s.known, s.known_bstride = self.known.data_ptr(), self.kb
         s.mask, s.mask_bstride = self.mask.data_ptr(), self.mb
         s.channels = sum(1 << c for c in self.channels)
@@ -858,10 +683,16 @@ class _Known:
         return s
 
 
-def _repaint_update_eager(eps, x, x0_hist, mask, row, noise=None, known=None, known_noise=None):
-    """One entry in torch fp32 ops, in place on x and x0_hist, with the operation order of repaint_update_kernel (each
-    product and sum rounded on its own), so it is the kernel's bit-exact oracle. `row`: a float32 table row; `mask`
-    broadcasts over x; `known`: a _Known; known_noise: z' shaped like x."""
+def _replace_channel(xc, known, kmask, mask, coef, std, z):
+    """x_c <- (x_c (1 - m) + (coef known + std z) m) g, fp32, in solver_update_kernel's operation order."""
+    sampled = known * coef + z * std
+    return (xc * (1.0 - kmask) + sampled * kmask) * mask
+
+
+def _update_eager(eps, x, x0_hist, mask, row, noise=None, known=None, known_noise=None):
+    """One entry in torch fp32 ops, in place on x and x0_hist, with the operation order of solver_update_kernel (each
+    product and sum rounded on its own), so it is the kernel's bit-exact oracle. `row`: a float32 REPAINT_COLUMNS row
+    (_rows32); `mask` broadcasts over x; `known`: a _Known; known_noise: z' shaped like x."""
     kind, _, sg, inv_a, c_x, c_0, c_1, c_z, coef, std = (float(v) for v in row)
     if kind:
         xn = (x * c_x + noise * c_z) * mask
@@ -881,34 +712,149 @@ def _repaint_update_eager(eps, x, x0_hist, mask, row, noise=None, known=None, kn
     return x
 
 
-def _repaint_update(eps, x, x0_hist, mask_flat, entry_c, noise=None, known=None, known_noise=None, seed=0, offset=0):
-    """One entry through mdb_repaint_update, in place on x and x0_hist; noise=None draws it in-kernel."""
+def _update(eps, x, x0_hist, mask_flat, entry_c, noise=None, known=None, known_noise=None, seed=0, offset=0):
+    """One entry through mdb_solver_update, in place on x and x0_hist; noise=None draws it in-kernel."""
     L = _native.lib()
     B, C = x.shape[0], x.shape[1]
     ks = known.struct(noise=known_noise) if known is not None else None
-    _native.check(L.mdb_repaint_update(_native.ptr(eps), _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat),
-                                       ctypes.byref(entry_c), x[0, 0].numel(), C, B, _native.ptr(noise), int(seed),
-                                       int(offset), ctypes.byref(ks) if ks is not None else None,
-                                       _native.current_stream()))
+    _native.check(L.mdb_solver_update(_native.ptr(eps), _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat),
+                                      ctypes.byref(entry_c), x[0, 0].numel(), C, B, _native.ptr(noise), int(seed),
+                                      int(offset), ctypes.byref(ks) if ks is not None else None,
+                                      _native.current_stream()))
     return x
 
 
-def _native_repaint_loop(net, x, x0_hist, mask_flat, entries_c, seed, step0=0, n=None, known=None):
-    """Entries step0 .. step0+n-1 of the schedule inside the library (mdb_repaint_run), in place on x and x0_hist.
-    `entries_c` is the whole table (_repaint_entries_c), indexed by the GLOBAL entry."""
+def _native_run(net, x, x0_hist, mask_flat, entries_c, seed, step0=0, n=None, known=None, replace_until=None):
+    """Entries step0 .. step0+n-1 of a table inside the library (mdb_solver_run), in place on x and x0_hist. `entries_c`
+    is the whole table (_entries_c), indexed by the GLOBAL entry; `known` is replaced after the global entries below
+    `replace_until` (default: all of them)."""
     L = _native.lib()
     B = x.shape[0]
     n = len(entries_c) - step0 if n is None else n
+    replace_until = len(entries_c) if replace_until is None else replace_until
     net._ensure_engine(B, x.device)
     net.sync_parameters()
     eps_buf = torch.empty_like(x)
     labels_buf = torch.empty(B, device=x.device, dtype=torch.float32)
-    part = (_native.RepaintEntryC * n).from_buffer(entries_c, step0 * ctypes.sizeof(_native.RepaintEntryC))
+    part = (_native.SolverEntryC * n).from_buffer(entries_c, step0 * ctypes.sizeof(_native.SolverEntryC))
     ks = known.struct() if known is not None else None
-    _native.check(L.mdb_repaint_run(net._handle, _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat), part, n,
-                                    B, int(seed), _native.ptr(eps_buf), _native.ptr(labels_buf), int(step0),
-                                    ctypes.byref(ks) if ks is not None else None, _native.current_stream()))
+    _native.check(L.mdb_solver_run(net._handle, _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat), part, n, B,
+                                   int(seed), _native.ptr(eps_buf), _native.ptr(labels_buf), int(step0),
+                                   ctypes.byref(ks) if ks is not None else None, int(replace_until),
+                                   _native.current_stream()))
     return x
+
+
+def _run_table(sde, table, model, x, grid_mask, name, known=None, replace_until=None, native=False, seed=0):
+    """Runs a solver table on x (fp32 [B, C, R, R, R]) and returns the result: the driver behind the four table samplers.
+
+    x is multiplied by the grid mask first. With `known` (a _Known) its kept region is replaced at label N - 1 (alpha,
+    sigma of N - 1, fresh noise), then after every entry below `replace_until` (default: all). Paths: with `native`, a
+    native ScoreNet and x on CUDA the whole table runs in the library (mdb_solver_run, Philox noise keyed by `seed` and
+    the entry); other CUDA states run model + mdb_solver_update per entry with torch.randn_like noise; CPU tensors run the
+    eager fp32 update (_update_eager), which is the kernel's oracle."""
+    B = x.shape[0]
+    if grid_mask.numel() != x[0, 0].numel():
+        raise ValueError(f"{name}: grid_mask must hold one value per voxel")
+    mask_v = grid_mask.to(device=x.device, dtype=torch.float32).reshape(x.shape[2:]).contiguous()
+    x = (x * mask_v).contiguous()
+    rows, entries_c = _rows32(table), _entries_c(table)
+    replace_until = len(rows) if replace_until is None else replace_until
+    if known is not None:
+        abar_T = float(sde.alphas_cumprod[sde.N - 1])
+        a_T, s_T = (float(np.float32(v)) for v in (np.sqrt(abar_T), np.sqrt(1.0 - abar_T)))
+        z = known.noise(x)
+        for c in known.channels:
+            x[:, c] = _replace_channel(x[:, c], known.known[:, c], known.mask, mask_v, a_T, s_T, z[:, c])
+    x0_hist = torch.empty_like(x)
+    net = _native_net(model)
+    if native and x.is_cuda and net is not None:
+        net._ensure_engine(B, x.device)
+        with net.frozen():  # nobody edits the weights inside the loop: skip per-step change detection
+            return _native_run(net, x, x0_hist, mask_v.reshape(-1), entries_c, seed, known=known,
+                               replace_until=replace_until)
+    for e, row in enumerate(rows):
+        renoise = row[0] != 0
+        eps = None if renoise else model(x, torch.full((B,), float(row[1]), device=x.device)).float()
+        noise = torch.randn_like(x) if (renoise or row[7] != 0) else None
+        ke = known if e < replace_until else None
+        z2 = ke.noise(x) if ke is not None else None
+        if x.is_cuda:
+            _update(None if renoise else eps.contiguous(), x, x0_hist, mask_v.reshape(-1), entries_c[e], noise, ke, z2)
+        else:
+            _update_eager(eps, x, x0_hist, mask_v, row, noise, ke, z2)
+    return x
+
+
+def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=False, denoise=True, device="cuda",
+                           grid_mask=None, native_rng=False, seed=42):
+    """Returns `dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None)`
+    -> (samples, number of network evaluations), the signature of pc_sampler, on dpm_solver_schedule's labels and table.
+
+    The prior is pc_sampler's (sde.prior_sampling(shape) * grid_mask), or x0 * grid_mask when `x0` (shape `shape`) is
+    given: no prior is drawn then. With `partial`, channel c is replaced before step 0
+    (alpha, sigma of label N-1) and after every step k but the last whose label n_k has N-1-n_k < freeze_iters (alpha,
+    sigma of n_{k+1}), with fresh per-sample noise; the x0 history keeps the network's prediction. Paths (_run_table): on
+    CUDA with `native_rng` and a native ScoreNet the whole loop runs in the library (mdb_solver_run, Philox noise keyed by
+    seed + rank and step); other CUDA states run model + mdb_solver_update per step with torch.randn_like noise; CPU
+    tensors run the eager fp32 update (_update_eager), which is the kernel's oracle."""
+    labels, table = dpm_solver_schedule(sde, n_steps, stochastic, denoise)
+    return _solver_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, "dpm_solver")
+
+
+def get_distilled_sampler(sde, shape, inverse_scaler, n_steps=8, device="cuda", grid_mask=None, native_rng=False, seed=42):
+    """The sampler of a progressively distilled student (`sampling.method='distilled'`, `sampling.distill_steps`): the
+    DDIM ODE on `ddim_grid(sde, n_steps)`, through get_dpm_solver_sampler's paths and conditioning with the first-order
+    rows of `ddim_table`. Same signature and return as get_dpm_solver_sampler."""
+    labels = ddim_grid(sde, n_steps)
+    return _solver_sampler(sde, shape, inverse_scaler, labels, ddim_table(sde, labels), device, grid_mask, native_rng,
+                           seed, "distilled")
+
+
+def _solver_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, name):
+    """get_dpm_solver_sampler's sampler on any 9-column solver table along `labels`."""
+    K_eff = len(labels) - 1
+
+    def dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None):
+        with torch.no_grad():
+            if freeze_iters is None:
+                freeze_iters = sde.N + 10
+            c = partial_channel
+            if x0 is not None and tuple(x0.shape) != tuple(shape):
+                raise ValueError(f"{name}: x0 has shape {tuple(x0.shape)}, the sampler {tuple(shape)}")
+            x = sde.prior_sampling(shape).to(device) if x0 is None else x0.to(device=device, dtype=torch.float32)
+            assert x.dim() == 5
+            known, until = None, 0
+            if partial is not None:
+                assert partial.dim() == 5
+                # only channel c of partial (cond_gen's has that one channel) and of partial_mask counts
+                kept = torch.zeros(partial.shape[0], *x.shape[1:], device=x.device)
+                kept[:, c] = partial[:, c]
+                known = _Known(kept, partial_mask[:, c].to(x.device), [c], shape[0], full_noise=False)
+                until = sum(1 for k in range(K_eff - 1) if sde.N - 1 - labels[k] < freeze_iters)
+            x = _run_table(sde, table, model, x, grid_mask, name, known, until, native_rng, seed + _rank())
+            return inverse_scaler(x), K_eff
+
+    return dpm_solver_sampler
+
+
+def get_dpm_solver_inverter(sde, shape, n_steps=25, grid_mask=None, device="cuda"):
+    """Returns `invert(model, x) -> (z, number of network evaluations)`: the latent at label N - 1 of grids x (shape
+    `shape`), taken as the state at label 0 after the grid mask is applied, by the ODE form of DPM-Solver++(2M) run
+    backwards (dpm_solver_inversion_schedule). The dpm_solver sampler with the same `n_steps`, started from z
+    (x0=z), maps it back to x up to discretisation error. No noise is drawn. Paths (_run_table): a native ScoreNet on
+    CUDA runs the whole loop in the library (mdb_solver_run); other CUDA models run model + mdb_solver_update per step;
+    CPU tensors run the eager fp32 update."""
+    labels, table = dpm_solver_inversion_schedule(sde, n_steps)
+
+    def invert(model, x):
+        with torch.no_grad():
+            if tuple(x.shape) != tuple(shape):
+                raise ValueError(f"dpm_solver inversion: x has shape {tuple(x.shape)}, expected {tuple(shape)}")
+            x = x.to(device=device, dtype=torch.float32)
+            return _run_table(sde, table, model, x, grid_mask, "dpm_solver inversion", native=True), len(labels) - 1
+
+    return invert
 
 
 def get_repaint_sampler(sde, shape, inverse_scaler, n_steps=25, jump=5, resample=5, stochastic=False, denoise=True,
@@ -918,52 +864,21 @@ def get_repaint_sampler(sde, shape, inverse_scaler, n_steps=25, jump=5, resample
     or shape[0]) exactly on `channels`, the rest regenerated by repaint_schedule's entries.
 
     The prior is sde.prior_sampling(shape) * grid_mask, or x0 * grid_mask; its kept region is replaced at label N - 1
-    (alpha, sigma of N - 1, fresh noise), as the conditional dpm_solver sampler does. Paths: on CUDA with `native_rng`
-    and a native ScoreNet the whole schedule runs in the library (mdb_repaint_run, Philox noise keyed by seed + rank and
-    entry); other CUDA states run model + mdb_repaint_update per entry with torch.randn_like noise; CPU tensors run the
-    eager fp32 update (_repaint_update_eager), which is the kernel's oracle."""
+    (alpha, sigma of N - 1, fresh noise), as the conditional dpm_solver sampler does. Paths (_run_table): on CUDA with
+    `native_rng` and a native ScoreNet the whole schedule runs in the library (mdb_solver_run, Philox noise keyed by
+    seed + rank and entry); other CUDA states run model + mdb_solver_update per entry with torch.randn_like noise; CPU
+    tensors run the eager fp32 update (_update_eager), which is the kernel's oracle."""
     table, nfe = repaint_schedule(sde, n_steps, jump, resample, stochastic, denoise)
-    rows32 = table.astype(np.float32)
-    entries_c = _repaint_entries_c(table)
-    N = sde.N
-    abar_T = float(sde.alphas_cumprod[N - 1])
-    a_T, s_T = (float(np.float32(v)) for v in (np.sqrt(abar_T), np.sqrt(1.0 - abar_T)))  # alpha, sigma of label N - 1
 
     def repaint_sampler(model, known, known_mask, channels, x0=None):
         with torch.no_grad():
-            B = shape[0]
             if x0 is not None and tuple(x0.shape) != tuple(shape):
                 raise ValueError(f"repaint: x0 has shape {tuple(x0.shape)}, the sampler {tuple(shape)}")
             x = sde.prior_sampling(shape).to(device) if x0 is None else x0.to(device=device, dtype=torch.float32)
-            x = (x * grid_mask).contiguous()
             if tuple(known.shape[1:]) != tuple(shape[1:]):
                 raise ValueError(f"repaint: known has shape {tuple(known.shape)}, the sampler {tuple(shape)}")
-            mask_v = grid_mask.to(device=x.device, dtype=torch.float32).reshape(x.shape[2:]).contiguous()
-            kn = _Known(known.to(x.device), known_mask.to(x.device), channels, B)
-            z = torch.randn_like(x)
-            for c in kn.channels:
-                x[:, c] = _replace_channel(x[:, c], kn.known[:, c], kn.mask, mask_v, a_T, s_T, z[:, c])
-            x0_hist = torch.empty_like(x)
-            net = _native_net(model)
-            if x.is_cuda and native_rng and net is not None:
-                net._ensure_engine(B, x.device)
-                net.sync_parameters()
-                net._frozen = True  # nobody edits the weights inside the loop: skip per-step change detection
-                try:
-                    _native_repaint_loop(net, x, x0_hist, mask_v.reshape(-1), entries_c, seed + _rank(), known=kn)
-                finally:
-                    net._frozen = False
-                return inverse_scaler(x), nfe
-            for e in range(len(rows32)):
-                renoise = rows32[e, 0] != 0
-                eps_out = None if renoise else model(x, torch.full((B,), float(rows32[e, 1]), device=x.device)).float()
-                noise = torch.randn_like(x) if (renoise or rows32[e, 7] != 0) else None
-                z2 = torch.randn_like(x)
-                if x.is_cuda:
-                    _repaint_update(None if renoise else eps_out.contiguous(), x, x0_hist, mask_v.reshape(-1),
-                                    entries_c[e], noise, kn, z2)
-                else:
-                    _repaint_update_eager(eps_out, x, x0_hist, mask_v, rows32[e], noise, kn, z2)
+            kn = _Known(known.to(x.device), known_mask.to(x.device), channels, shape[0])
+            x = _run_table(sde, table, model, x, grid_mask, "repaint", kn, None, native_rng, seed + _rank())
             return inverse_scaler(x), nfe
 
     return repaint_sampler

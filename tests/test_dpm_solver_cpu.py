@@ -193,7 +193,7 @@ def test_conditioning_replaces_channel(monkeypatch, stochastic, freeze_iters):
     assert torch.all(out[:, :, mask[0] == 0] == 0)
 
 
-def test_eager_update_keeps_network_x0():
+def test_eager_entry_keeps_network_x0():
     """The x0 history receives the network's prediction, not the replaced channel."""
     sde = _sde()
     R, B, c = 6, 2, 0
@@ -202,15 +202,15 @@ def test_eager_update_keeps_network_x0():
     mask = torch.ones(R, R, R)
     partial = torch.randn(1, 4, R, R, R, generator=g)
     pmask = torch.ones(1, 4, R, R, R)
-    cond = sampling._Cond(sde, partial, pmask, c, None, B)
+    known = sampling._Known(partial, pmask[:, c], [c], B)
     _, table = sampling.dpm_solver_schedule(sde, 10)
-    row = table.astype(np.float32)[3]
+    row = sampling._rows32(table)[3]
     hist = torch.randn(B, 4, R, R, R, generator=g)
-    z2 = torch.randn(B, R, R, R, generator=g)
-    x0 = (x - eps * float(row[1])) * float(row[2])
-    xn = sampling._solver_update_eager(eps, x.clone(), hist, mask, row, cond=cond, cond_noise=z2)
+    z2 = torch.randn(B, 4, R, R, R, generator=g)
+    x0 = (x - eps * float(row[2])) * float(row[3])
+    xn = sampling._update_eager(eps, x.clone(), hist, mask, row, known=known, known_noise=z2)
     assert torch.equal(hist, x0)
-    assert torch.equal(xn[:, c], partial[:, c] * float(row[7]) + z2 * float(row[8]))
+    assert torch.equal(xn[:, c], partial[:, c] * float(row[8]) + z2[:, c] * float(row[9]))
 
 
 def test_get_sampling_fn_dispatches_dpm_solver():

@@ -112,7 +112,7 @@ def _restated(x, eps, hist, g, row, z, known, m, chans, z2):
 
 
 @pytest.mark.parametrize("entry", ["first_order", "second_order_sde", "renoise", "last"])
-def test_eager_update_against_float64_restatement(entry):
+def test_eager_entry_against_float64_restatement(entry):
     sde = _sde()
     table, _ = sampling.repaint_schedule(sde, 10, 3, 3, stochastic=True)
     e = {"first_order": 0, "second_order_sde": 1, "renoise": 3, "last": len(table) - 1}[entry]
@@ -126,7 +126,7 @@ def test_eager_update_against_float64_restatement(entry):
     m = (torch.rand(B, R, R, R, generator=gen) < 0.5).float() * g
     kn = sampling._Known(known, m, [0, 2, 3], B)
     xe, he = x.clone(), hist.clone()
-    sampling._repaint_update_eager(eps, xe, he, g, row, z, kn, z2)
+    sampling._update_eager(eps, xe, he, g, row, z, kn, z2)
     xr, hr = _restated(x, eps, hist, g.numpy(), row, z, known.double().numpy(), m.double().numpy(), [0, 2, 3], z2)
     assert np.array_equal(xe.double().numpy(), xr)
     assert np.array_equal(he.double().numpy(), hr)

@@ -69,19 +69,19 @@ def test_wrappers_refuse_operands_the_kernel_would_misread():
             distill.distill_step(**{**ok, key: bad})
 
 
-def test_phase0_equals_solver_update_with_equal_indices():
+def test_phase0_equals_denoise_entry_with_equal_indices():
     from meshdiffusion_b200.diffusion import distill, sampling
     B, C, R = 3, 4, 9
     z_s, eps_s, _, mask, rows = _case(B, C, R, 2, K_T=16)
     sde = _sde()
     labels = sampling.ddim_grid(sde, 16)
-    steps_c = sampling._solver_steps_c(sampling.ddim_table(sde, labels))
+    entries_c = sampling._entries_c(sampling.ddim_table(sde, labels))
     for i in (0, 5, 7):
         idx = torch.full((B,), i, dtype=torch.int32, device="cuda")
         z_mid, lab = torch.empty_like(z_s), torch.empty(B, device="cuda")
         distill.distill_step(eps_s, z_s, z_mid, None, mask.reshape(-1), idx, rows, 0, lab)
         x, hist = z_s.clone(), torch.empty_like(z_s)
-        sampling._solver_update(eps_s, x, hist, mask.reshape(-1), steps_c[2 * i])
+        sampling._update(eps_s, x, hist, mask.reshape(-1), entries_c[2 * i])
         assert torch.equal(z_mid, x), f"phase 0 differs from mdb_solver_update at row {i}"
         assert torch.all(lab == labels[2 * i + 1])
 

@@ -23,35 +23,36 @@ def _sde(device="cuda"):
 
 @pytest.mark.parametrize("conditional", [False, True])
 @pytest.mark.parametrize("kind", ["first_order", "second_order", "sde"])
-def test_update_kernel_matches_eager(kind, conditional):
+def test_entry_kernel_matches_eager(kind, conditional):
     from meshdiffusion_b200.diffusion import sampling
     sde = _sde("cpu")
     _, table = sampling.dpm_solver_schedule(sde, 20, stochastic=(kind == "sde"))
     k = 0 if kind == "first_order" else 7
-    rows32, steps_c = table.astype(np.float32), sampling._solver_steps_c(table)
+    rows32, entries_c = sampling._rows32(table), sampling._entries_c(table)
     g = torch.Generator().manual_seed(11 + k)
     B, R, c = 3, 16, 2
     x = torch.randn(B, 4, R, R, R, generator=g)
     eps, hist, z = (torch.randn(B, 4, R, R, R, generator=g) for _ in range(3))
-    z2 = torch.randn(B, R, R, R, generator=g)
+    z2 = torch.zeros(B, 4, R, R, R)
+    z2[:, c] = torch.randn(B, R, R, R, generator=g)
     mask = (torch.rand(R, R, R, generator=g) < 0.4).float()
-    cond = None
+    known = known_cpu = None
     if conditional:
         partial = torch.sign(torch.randn(1, 4, R, R, R, generator=g))
         pmask = (torch.rand(B, 4, R, R, R, generator=g) < 0.5).float()
-        cond_cpu = sampling._Cond(sde, partial, pmask, c, None, B)
-        cond = sampling._Cond(sde, partial.cuda(), pmask.cuda(), c, None, B)
+        known_cpu = sampling._Known(partial, pmask[:, c], [c], B)
+        known = sampling._Known(partial.cuda(), pmask[:, c].cuda(), [c], B)
     xe, he = x.clone(), hist.clone()
-    sampling._solver_update_eager(eps, xe, he, mask, rows32[k], z, cond_cpu if conditional else None, z2)
+    sampling._update_eager(eps, xe, he, mask, rows32[k], z, known_cpu, z2)
     xg, hg = x.cuda(), hist.cuda()
-    sampling._solver_update(eps.cuda(), xg, hg, mask.cuda().reshape(-1), steps_c[k], z.cuda(), cond,
-                            z2.cuda() if conditional else None)
+    sampling._update(eps.cuda(), xg, hg, mask.cuda().reshape(-1), entries_c[k], z.cuda(), known,
+                     z2.cuda() if conditional else None)
     assert torch.equal(xg.cpu(), xe), f"{kind}: x differs from the eager update"
     assert torch.equal(hg.cpu(), he), f"{kind}: x0 history differs from the eager update"
     assert torch.all(xe[:, :, mask == 0] == 0)
 
 
-def test_in_kernel_noise():
+def test_entry_in_kernel_noise():
     """noise=NULL: z from Philox(seed, element, offset). A step with c_z = 1 and every other coefficient 0 writes z * g."""
     from meshdiffusion_b200 import _native
     from meshdiffusion_b200.diffusion import sampling
@@ -59,11 +60,11 @@ def test_in_kernel_noise():
     mask = torch.ones(R, R, R, device="cuda")
     mask[:, :, : R // 2] = 0
     zeros = torch.zeros(B, 4, R, R, R, device="cuda")
-    row = _native.SolverStepC(0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0)
+    row = _native.SolverEntryC(0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0)
 
     def draw(seed, step):
         x = zeros.clone()
-        sampling._solver_update(zeros, x, torch.empty_like(x), mask.reshape(-1), row, seed=seed, offset=4 * step)
+        sampling._update(zeros, x, torch.empty_like(x), mask.reshape(-1), row, seed=seed, offset=4 * step)
         assert torch.all(x[..., : R // 2] == 0)
         return x[..., R // 2:]
 
@@ -79,9 +80,9 @@ def test_in_kernel_noise():
 @pytest.mark.parametrize("conditional", [False, True])
 @pytest.mark.parametrize("precision", ["bf16", "tf32", "bf16x3"])
 @pytest.mark.parametrize("size", ["tiny", "res64"])
-def test_native_loop_matches_stepwise(size, precision, conditional, stochastic):
+def test_device_loop_matches_stepwise(size, precision, conditional, stochastic):
     """mdb_solver_run(seed, step0, n) is bitwise equal to n x [model(x, label) + mdb_solver_update(noise=NULL, seed,
-    offset=4*k)] through the public entry points, with and without the replacement conditioning."""
+    offset=4*k)] through the public entry points, with and without the replacement of channel 0 of a partial grid."""
     from meshdiffusion_b200 import _native
     from meshdiffusion_b200.diffusion import sampling
     cfg = tiny_config("res64", precision) if size == "tiny" else full_config("res64", precision)
@@ -91,28 +92,28 @@ def test_native_loop_matches_stepwise(size, precision, conditional, stochastic):
     R = cfg.data.image_size
     sde = _sde()
     labels, table = sampling.dpm_solver_schedule(sde, 12, stochastic=stochastic)
-    steps_c = sampling._solver_steps_c(table)
+    entries_c = sampling._entries_c(table)
     mask = sd["mask"].view(-1).cuda().contiguous()
     g = torch.Generator(device="cuda").manual_seed(seed)
     x0 = (torch.randn(B, 4, R, R, R, device="cuda", generator=g) * mask.view(R, R, R)).contiguous()
     h0 = torch.randn(B, 4, R, R, R, device="cuda", generator=g)
-    cond = None
+    known = None
     if conditional:
         partial = torch.sign(torch.randn(1, 1, R, R, R, device="cuda", generator=g))
         pmask = (torch.rand(1, 1, R, R, R, device="cuda", generator=g) < 0.5).float()
-        cond = sampling._Cond(sde, partial, pmask, 0, None, B)
+        known = sampling._Known(partial, pmask[:, 0], [0], B)
     until = step0 + n - 1  # the last step runs without the replacement
     with torch.no_grad():
         xa, ha = x0.clone(), h0.clone()
-        sampling._native_solver_loop(net, xa, ha, mask, steps_c, seed, step0, n, cond, until)
+        sampling._native_run(net, xa, ha, mask, entries_c, seed, step0, n, known, until)
         xb, hb = x0.clone(), h0.clone()
         L = _native.lib()
         for k in range(step0, step0 + n):
             eps = model(xb, torch.full((B,), float(labels[k]), device="cuda"))
-            cs = cond.struct() if (cond is not None and k < until) else None
+            ks = known.struct() if (known is not None and k < until) else None
             _native.check(L.mdb_solver_update(_native.ptr(eps), _native.ptr(xb), _native.ptr(hb), _native.ptr(mask),
-                                              ctypes.byref(steps_c[k]), R ** 3, 4, B, None, seed, 4 * k,
-                                              ctypes.byref(cs) if cs is not None else None, _native.current_stream()))
+                                              ctypes.byref(entries_c[k]), R ** 3, 4, B, None, seed, 4 * k,
+                                              ctypes.byref(ks) if ks is not None else None, _native.current_stream()))
     assert torch.isfinite(xa).all()
     assert torch.equal(xa, xb) and torch.equal(ha, hb), "mdb_solver_run differs from the step-by-step public path"
     if conditional:

@@ -1,7 +1,7 @@
-"""Shape editing on the GPU: mdb_repaint_update bit-exact against the eager fp32 update (both entry kinds, caller and
-Philox noise, shared and per-sample kept regions), mdb_repaint_run bit-exact against the per-entry public path,
-resample = 1 on one channel against mdb_solver_run, the analytic gate through the kernel path, and `--mode=edit` end
-to end followed by `--mode=export`."""
+"""Shape editing on the GPU: mdb_solver_update bit-exact against the eager fp32 update on RePaint entries (both kinds,
+caller and Philox noise, shared and per-sample kept regions), mdb_solver_run bit-exact against the per-entry public path,
+resample = 1 on one channel against the conditional solver table, the analytic gate through the kernel path, and
+`--mode=edit` end to end followed by `--mode=export`."""
 import ctypes
 import glob
 import json
@@ -28,21 +28,20 @@ def _philox(kind_offset, seed, B, C, R):
     from meshdiffusion_b200 import _native
     from meshdiffusion_b200.diffusion import sampling
     x = torch.zeros(B, C, R, R, R, device="cuda")
-    e = _native.RepaintEntryC(1, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0)
-    sampling._repaint_update(None, x, torch.empty_like(x), torch.ones(R ** 3, device="cuda"), e, seed=seed,
-                             offset=kind_offset)
+    e = _native.SolverEntryC(1, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0)
+    sampling._update(None, x, torch.empty_like(x), torch.ones(R ** 3, device="cuda"), e, seed=seed, offset=kind_offset)
     return x
 
 
 @pytest.mark.parametrize("per_sample", [False, True])
 @pytest.mark.parametrize("philox", [False, True])
 @pytest.mark.parametrize("entry", ["first_order", "second_order_sde", "renoise", "last"])
-def test_update_kernel_matches_eager(entry, philox, per_sample):
+def test_entry_kernel_matches_eager(entry, philox, per_sample):
     from meshdiffusion_b200.diffusion import sampling
     sde = _sde("cpu")
     table, _ = sampling.repaint_schedule(sde, 10, 3, 3, stochastic=True)
     e = {"first_order": 0, "second_order_sde": 1, "renoise": 3, "last": len(table) - 1}[entry]
-    rows32, entries_c = table.astype(np.float32), sampling._repaint_entries_c(table)
+    rows32, entries_c = table.astype(np.float32), sampling._entries_c(table)
     g = torch.Generator().manual_seed(21 + e)
     B, C, R, seed, offset = 3, 4, 16, 99, 4 * e
     x, eps, hist, z, z2 = (torch.randn(B, C, R, R, R, generator=g) for _ in range(5))
@@ -54,11 +53,11 @@ def test_update_kernel_matches_eager(entry, philox, per_sample):
     if philox:
         z, z2 = _philox(offset, seed, B, C, R).cpu(), _philox(offset + 2, seed, B, C, R).cpu()
     xe, he = x.clone(), hist.clone()
-    sampling._repaint_update_eager(eps, xe, he, mask, rows32[e], z, sampling._Known(known, m, chans, B), z2)
+    sampling._update_eager(eps, xe, he, mask, rows32[e], z, sampling._Known(known, m, chans, B), z2)
     xg, hg = x.cuda(), hist.cuda()
     kn = sampling._Known(known.cuda(), m.cuda(), chans, B)
-    sampling._repaint_update(eps.cuda(), xg, hg, mask.cuda().reshape(-1), entries_c[e], None if philox else z.cuda(), kn,
-                             None if philox else z2.cuda(), seed=seed, offset=offset)
+    sampling._update(eps.cuda(), xg, hg, mask.cuda().reshape(-1), entries_c[e], None if philox else z.cuda(), kn,
+                     None if philox else z2.cuda(), seed=seed, offset=offset)
     assert torch.equal(xg.cpu(), xe), f"{entry}: x differs from the eager update"
     assert torch.equal(hg.cpu(), he), f"{entry}: x0 history differs from the eager update"
     assert torch.all(xe[:, :, mask == 0] == 0)
@@ -68,9 +67,9 @@ def test_update_kernel_matches_eager(entry, philox, per_sample):
 
 
 @pytest.mark.parametrize("size,precision", [("tiny", "bf16x3"), ("res64", "bf16")])
-def test_native_loop_matches_per_entry(size, precision):
-    """mdb_repaint_run(seed, step0, n) is bitwise equal to n x [model(x, label) on denoise entries +
-    mdb_repaint_update(noise=NULL, seed, offset=4*e)] through the public entry points."""
+def test_device_loop_matches_per_entry(size, precision):
+    """mdb_solver_run(seed, step0, n) on a RePaint table is bitwise equal to n x [model(x, label) on denoise entries +
+    mdb_solver_update(noise=NULL, seed, offset=4*e)] through the public entry points."""
     from meshdiffusion_b200 import _native
     from meshdiffusion_b200.diffusion import sampling
     cfg = tiny_config("res64", precision) if size == "tiny" else full_config("res64", precision)
@@ -80,7 +79,7 @@ def test_native_loop_matches_per_entry(size, precision):
     R = cfg.data.image_size
     table, _ = sampling.repaint_schedule(_sde(), 8, 2, 3, stochastic=True)
     assert 1 in table[step0:step0 + n, 0]
-    entries_c = sampling._repaint_entries_c(table)
+    entries_c = sampling._entries_c(table)
     mask = sd["mask"].view(-1).cuda().contiguous()
     g = torch.Generator(device="cuda").manual_seed(seed)
     x0 = (torch.randn(B, 4, R, R, R, device="cuda", generator=g) * mask.view(R, R, R)).contiguous()
@@ -90,23 +89,23 @@ def test_native_loop_matches_per_entry(size, precision):
     kn = sampling._Known(known, keep, range(4), B)
     with torch.no_grad():
         xa, ha = x0.clone(), h0.clone()
-        sampling._native_repaint_loop(net, xa, ha, mask, entries_c, seed, step0, n, kn)
+        sampling._native_run(net, xa, ha, mask, entries_c, seed, step0, n, kn)
         xb, hb = x0.clone(), h0.clone()
         L = _native.lib()
         ks = kn.struct()
         for e in range(step0, step0 + n):
             eps = None if table[e, 0] else model(xb, torch.full((B,), float(entries_c[e].label), device="cuda"))
-            _native.check(L.mdb_repaint_update(_native.ptr(eps), _native.ptr(xb), _native.ptr(hb), _native.ptr(mask),
-                                               ctypes.byref(entries_c[e]), R ** 3, 4, B, None, seed, 4 * e,
-                                               ctypes.byref(ks), _native.current_stream()))
+            _native.check(L.mdb_solver_update(_native.ptr(eps), _native.ptr(xb), _native.ptr(hb), _native.ptr(mask),
+                                              ctypes.byref(entries_c[e]), R ** 3, 4, B, None, seed, 4 * e,
+                                              ctypes.byref(ks), _native.current_stream()))
     assert torch.isfinite(xa).all()
-    assert torch.equal(xa, xb) and torch.equal(ha, hb), "mdb_repaint_run differs from the per-entry public path"
+    assert torch.equal(xa, xb) and torch.equal(ha, hb), "mdb_solver_run differs from the per-entry public path"
 
 
 @pytest.mark.parametrize("stochastic", [False, True])
-def test_resample_one_single_channel_is_the_conditional_solver(stochastic):
-    """resample = 1 with channel set {0}: outside the kept region the output is mdb_solver_run's with the equivalent
-    mdb_sampler_cond (same initial x, same seed); inside it, the known grid exactly."""
+def test_resample_one_single_channel_is_the_solver_table(stochastic):
+    """resample = 1 with channel set {0}: outside the kept region the output is the conditional solver table's, which
+    stops replacing before its last step (same loop, initial x and seed); inside it, the known grid exactly."""
     from meshdiffusion_b200.diffusion import sampling
     cfg = tiny_config("res64", "bf16x3")
     model, sd = build_model(cfg, "cuda:0", 21)
@@ -122,12 +121,11 @@ def test_resample_one_single_channel_is_the_conditional_solver(stochastic):
     keep = (torch.rand(B, 1, R, R, R, device="cuda", generator=g) < 0.5).float() * mask.view(1, 1, R, R, R)
     with torch.no_grad():
         xa = x0.clone()
-        sampling._native_repaint_loop(net, xa, torch.empty_like(xa), mask, sampling._repaint_entries_c(table), seed,
-                                      known=sampling._Known(known, keep, [0], B))
+        kn = sampling._Known(known, keep, [0], B)
+        sampling._native_run(net, xa, torch.empty_like(xa), mask, sampling._entries_c(table), seed, known=kn)
         xb = x0.clone()
-        cond = sampling._Cond(sde, known, keep.expand(B, 4, R, R, R), 0, None, B)
-        sampling._native_solver_loop(net, xb, torch.empty_like(xb), mask, sampling._solver_steps_c(dpm), seed, cond=cond,
-                                     cond_until=K - 1)
+        sampling._native_run(net, xb, torch.empty_like(xb), mask, sampling._entries_c(dpm), seed, known=kn,
+                             replace_until=K - 1)
     kept = keep[:, 0] > 0
     assert torch.equal(xa[:, 1:], xb[:, 1:])
     assert torch.equal(xa[:, 0][~kept], xb[:, 0][~kept])

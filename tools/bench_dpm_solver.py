@@ -83,11 +83,11 @@ def bench_mode(precision, B, K, device):
         for stochastic in (False, True):
             key = "sde" if stochastic else "ode"
             lab, table = sampling.dpm_solver_schedule(sde, K, stochastic)
-            steps_c = sampling._solver_steps_c(table)
+            entries_c = sampling._entries_c(table)
             x, hist = x0.clone(), torch.empty_like(x0)
-            sampling._native_solver_loop(net, x, hist, mask_flat, steps_c, 1, 0, 2)
+            sampling._native_run(net, x, hist, mask_flat, entries_c, 1, 0, 2)
             x.copy_(x0)
-            ev, host = _timed(lambda: sampling._native_solver_loop(net, x, hist, mask_flat, steps_c, 1))
+            ev, host = _timed(lambda: sampling._native_run(net, x, hist, mask_flat, entries_c, 1))
             cfg.sampling.method, cfg.sampling.dpm_steps, cfg.sampling.dpm_sde = "dpm_solver", K, stochastic
             cfg.sampling.native_rng = True
             fn = sampling.get_sampling_fn(cfg, sde, (B, 4, R, R, R), lambda t: t, 1e-3, grid_mask=mask.view(1, R, R, R))
@@ -102,12 +102,12 @@ def bench_mode(precision, B, K, device):
             eps = torch.randn_like(x0)
             xk, hk = x0.clone(), torch.randn_like(x0)
             for _ in range(3):
-                sampling._solver_update(eps, xk, hk, mask_flat, steps_c[3], seed=1, offset=12)
+                sampling._update(eps, xk, hk, mask_flat, entries_c[3], seed=1, offset=12)
             reps = 200
 
             def launches():
                 for _ in range(reps):
-                    sampling._solver_update(eps, xk, hk, mask_flat, steps_c[3], seed=1, offset=12)
+                    sampling._update(eps, xk, hk, mask_flat, entries_c[3], seed=1, offset=12)
             ev, _ = _timed(launches)
             V = R ** 3
             nbytes = B * 4 * V * 20 + V * 4

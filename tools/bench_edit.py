@@ -1,10 +1,10 @@
 """Times shape editing (`--mode=edit`: RePaint resampling on the DPM-Solver++(2M) grid) on synthetic weights:
-  * the entry kernel alone (mdb_repaint_update, in-kernel Philox noise, all four channels replaced): time per launch and
+  * the entry kernel alone (mdb_solver_update, in-kernel Philox noise, all four channels replaced): time per launch and
     GB/s over the bytes it must move, against the H100 SXM data-sheet 3.35 TB/s, for a second-order denoise entry
     (x, eps, x0_hist, known read, x and x0_hist written: 24 bytes per element) and a renoise entry (x, known read, x
     written: 12 bytes per element), plus the two masks (8 bytes per voxel);
   * one res64 edit call per operand mode (batch 32, K = 25, jump 5, resample 3 by default): the public sampler call with
-    the whole schedule in mdb_repaint_run, wall time around a device synchronise, and its network evaluations.
+    the whole schedule in mdb_solver_run, wall time around a device synchronise, and its network evaluations.
 The card's name, power limit and SM clock are read with nvidia-smi in the same run.
 
     python tools/bench_edit.py [--batch 32] [--steps 25] [--jump 5] [--resample 3] [--precisions bf16x3,bf16] [--out f]
@@ -35,7 +35,7 @@ def bench_kernel(B, device, R=64, reps=200):
     from meshdiffusion_b200.geometry import dmtet
     sde = sde_lib.VPSDE(0.1, 20.0, 1000, device=device)
     table, _ = sampling.repaint_schedule(sde, 25, 5, 3, stochastic=True)
-    entries_c = sampling._repaint_entries_c(table)
+    entries_c = sampling._entries_c(table)
     mask = dmtet.grid_mask_from_tets(R).to(device)
     mask_flat = mask.reshape(-1).contiguous()
     x0 = torch.randn(B, 4, R, R, R, device=device) * mask
@@ -49,7 +49,7 @@ def bench_kernel(B, device, R=64, reps=200):
 
         def launches(n):
             for _ in range(n):
-                sampling._repaint_update(eps, x, h, mask_flat, entries_c[e], known=kn, seed=1, offset=4 * e)
+                sampling._update(eps, x, h, mask_flat, entries_c[e], known=kn, seed=1, offset=4 * e)
         launches(3)
         ev, _ = _timed(lambda: launches(reps))
         nbytes = B * 4 * V * per_elem + 2 * V * 4
