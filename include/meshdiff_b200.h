@@ -41,6 +41,9 @@ typedef struct mdb_unet_config {
                               meets the 1e-3 parity contract); fp32 accumulation in all three */
   int training;            /* 1 = also build the backward plan and keep what it needs; precision 0 (bf16) or 2 (split bf16:
                               fp32-class gradients at about a third of the tensor rate); tf32 is refused */
+  int num_classes;         /* config.model.num_classes: 0 = unconditional (the reference's network). K > 0 adds
+                              label_embed.weight [K+1][4nf], last in the parameter table; row K is the null class of
+                              classifier-free guidance: act(temb) = silu(Linear1(silu(Linear0(emb(t)))) + E[y]) */
 } mdb_unet_config;
 
 int mdb_unet_create(const mdb_unet_config* cfg, mdb_unet** out);
@@ -87,6 +90,14 @@ int mdb_unet_profile(mdb_unet* net, const float* x, const float* labels, float* 
  * Dropout of the next forward/backward pair (nn.Dropout(p) after GroupNorm_1+SiLU, layers.py:661,682); p = 0 is
  * model.eval(). The same (p, seed) must be in force for a forward and its backward. */
 int mdb_unet_set_dropout(mdb_unet* net, float p, unsigned long long seed);
+/* Class ids (device int32 [batch], each in 0..K with K = num_classes the null class; NULL = the null class for every
+ * sample) of the following forward/backward pairs, which must run at this batch; in force until the next call, like
+ * mdb_unet_set_dropout. The ids are copied on `stream` into a buffer the engine owns and checked there; the check copies
+ * them back to the host and synchronises `stream`. The caller's array may be freed when the call returns. Each forward
+ * copies the ids in force, on its stream, into a second engine buffer at a fixed address, which is what its CUDA graphs
+ * read. An engine with num_classes = 0 refuses a non-NULL pointer; an id outside 0..K is an error (no ids are then in
+ * force: the null class). */
+int mdb_unet_set_classes(mdb_unet* net, const int* classes, int batch, void* stream);
 /* dout = dL/d(out) of the immediately preceding mdb_unet_forward (same x, labels, batch; x and labels must still be
  * alive). grads: ONE flat fp32 buffer of grads_numel = sum of all parameter numels, parameter i at the offset
  * mdb_unet_grad_offset gives (table order); slots of non-trainable tensors (mask, coords, sigmas, pos_layer.weight,
@@ -209,6 +220,24 @@ int mdb_solver_update(const float* eps, float* x, float* x0_hist, const float* m
 int mdb_solver_run(mdb_unet* net, float* x, float* x0_hist, const float* mask, const mdb_solver_entry* entries,
                    int n_entries, int batch, unsigned long long seed, float* eps_buf, float* labels_buf, int step0,
                    const mdb_solver_known* known /* nullable */, int replace_until, void* stream);
+
+/* Classifier-free guidance (Ho & Salimans 2022) of a class-conditional network. A guided denoise entry reads the
+ * conditional output eps_c and the null-class output eps_u and uses, in the same single pass over HBM,
+ *   eps = eps_u + w (eps_c - eps_u)     (each operation rounded on its own)
+ * in place of eps; the rest is mdb_solver_update's arithmetic, unchanged. Renoise entries ignore both outputs. */
+int mdb_solver_update_guided(const float* eps_c, const float* eps_u, float w, float* x, float* x0_hist, const float* mask,
+                             const mdb_solver_entry* entry, long long voxels, int channels, int batch,
+                             const float* noise /* nullable */, unsigned long long seed, unsigned long long offset,
+                             const mdb_solver_known* known /* nullable */, void* stream);
+/* mdb_solver_run with guidance: each denoise entry runs the network twice at `batch`, with `classes` (device int32
+ * [batch], checked as mdb_unet_set_classes checks them) into eps_buf and with the null class into eps_u_buf (device
+ * scratch [B][C][V]), then the guided entry. w == 1 runs the conditional forward and the plain entry only (eps_u_buf may
+ * be NULL): bitwise mdb_unet_set_classes(classes) followed by mdb_solver_run. After the call `classes` are the ids in
+ * force, as after mdb_unet_set_classes. */
+int mdb_solver_run_guided(mdb_unet* net, float* x, float* x0_hist, const float* mask, const mdb_solver_entry* entries,
+                          int n_entries, int batch, unsigned long long seed, const int* classes, float w, float* eps_buf,
+                          float* eps_u_buf, float* labels_buf, int step0, const mdb_solver_known* known /* nullable */,
+                          int replace_until, void* stream);
 
 /* Progressive distillation (Salimans & Ho 2022; `--mode=distill`, diffusion/distill.py, with the rows computed in float64
  * on the host by diffusion/sampling.py: distill_rows). A student step i moves z from label s = l_{2i} to e = l_{2i+2} of

@@ -31,6 +31,7 @@ class UNetConfigC(ctypes.Structure):
         ("max_batch", ctypes.c_int),
         ("precision", ctypes.c_int),
         ("training", ctypes.c_int),
+        ("num_classes", ctypes.c_int),
     ]
 
 
@@ -89,6 +90,7 @@ SIGNATURES = {
                                  ctypes.POINTER(_i)]),
     "mdb_unet_profile": (_i, [_vp, _vp, _vp, _vp, _i, _vp, ctypes.c_char_p, _i, ctypes.POINTER(_f), _i, ctypes.POINTER(_i)]),
     "mdb_unet_set_dropout": (_i, [_vp, _f, _u64]),
+    "mdb_unet_set_classes": (_i, [_vp, _vp, _i, _vp]),
     "mdb_unet_backward": (_i, [_vp, _vp, _vp, _ll, _i, _i, _vp]),
     "mdb_unet_grad_offset": (_i, [_vp, ctypes.c_char_p, ctypes.POINTER(_ll)]),
     "mdb_unet_backward_input": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
@@ -105,6 +107,10 @@ SIGNATURES = {
                                ctypes.POINTER(SolverKnownC), _vp]),
     "mdb_solver_run": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverEntryC), _i, _i, _u64, _vp, _vp, _i,
                             ctypes.POINTER(SolverKnownC), _i, _vp]),
+    "mdb_solver_update_guided": (_i, [_vp, _vp, _f, _vp, _vp, _vp, ctypes.POINTER(SolverEntryC), _ll, _i, _i, _vp, _u64, _u64,
+                                      ctypes.POINTER(SolverKnownC), _vp]),
+    "mdb_solver_run_guided": (_i, [_vp, _vp, _vp, _vp, ctypes.POINTER(SolverEntryC), _i, _i, _u64, _vp, _f, _vp, _vp, _vp, _i,
+                                   ctypes.POINTER(SolverKnownC), _i, _vp]),
     "mdb_distill_step": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _ll, _i, _i, _vp]),
     "mdb_distill_targets": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "mdb_ddpm_loss": (_i, [_vp, _vp, _vp, _d, _vp, _vp, _vp, _i, _i, _ll, _vp]),

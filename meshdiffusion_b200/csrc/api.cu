@@ -45,7 +45,7 @@ static int create_impl(const mdb_unet_config* c, mdb_unet** out, bool dry) {
   u.n_attn = c->n_attn;
   for (int i = 0; i < 4; ++i) u.attn_resolutions[i] = c->attn_resolutions[i];
   u.num_channels = c->num_channels; u.stem_ksize = c->stem_ksize; u.use_pos_bias = c->use_pos_bias;
-  u.max_batch = c->max_batch; u.precision = c->precision; u.training = c->training;
+  u.max_batch = c->max_batch; u.precision = c->precision; u.training = c->training; u.num_classes = c->num_classes;
   auto* h = new mdb_unet;
   h->net = nullptr;
   try { h->net = new UNet(u, dry); } catch (...) { delete h; throw; }
@@ -171,6 +171,12 @@ int mdb_unet_profile(mdb_unet* n, const float* x, const float* labels, float* ou
 int mdb_unet_set_dropout(mdb_unet* n, float p, unsigned long long seed) {
   MDB_API_BEGIN
   n->net->set_dropout(p, seed);
+  MDB_API_END
+}
+
+int mdb_unet_set_classes(mdb_unet* n, const int* classes, int B, void* stream) {
+  MDB_API_BEGIN
+  n->net->set_classes(classes, B, (cudaStream_t)stream);
   MDB_API_END
 }
 
@@ -371,6 +377,60 @@ int mdb_solver_update(const float* eps, float* x, float* x0_hist, const float* m
   if (!a.renoise && !eps) throw std::runtime_error("mdb: a denoise entry needs the network output");
   a.noise = noise; a.seed = seed; a.offset = offset;
   launch_solver_entry(a, B, (cudaStream_t)stream);
+  MDB_API_END
+}
+
+int mdb_solver_update_guided(const float* eps_c, const float* eps_u, float w, float* x, float* x0_hist, const float* mask,
+                             const mdb_solver_entry* entry, long long V, int C, int B, const float* noise,
+                             unsigned long long seed, unsigned long long offset, const mdb_solver_known* known, void* stream) {
+  MDB_API_BEGIN
+  if (!entry) throw std::runtime_error("mdb: mdb_solver_update_guided needs an entry");
+  if (V <= 0 || C <= 0 || B <= 0) throw std::runtime_error("mdb: mdb_solver_update_guided needs positive voxels, channels, batch");
+  SolverEntryArgs a = entry_args(eps_c, x, x0_hist, mask, *entry, V, C, known);
+  if (!a.renoise && (!eps_c || !eps_u)) throw std::runtime_error("mdb: a guided denoise entry needs both network outputs");
+  if (!a.renoise) { a.eps_u = eps_u; a.w = w; }
+  a.noise = noise; a.seed = seed; a.offset = offset;
+  launch_solver_entry(a, B, (cudaStream_t)stream);
+  MDB_API_END
+}
+
+int mdb_solver_run_guided(mdb_unet* n, float* x, float* x0_hist, const float* mask, const mdb_solver_entry* entries,
+                          int n_entries, int B, unsigned long long seed, const int* classes, float w, float* eps_buf,
+                          float* eps_u_buf, float* labels_buf, int step0, const mdb_solver_known* known, int replace_until,
+                          void* stream) {
+  MDB_API_BEGIN
+  cudaStream_t s = (cudaStream_t)stream;
+  UNet& net = *n->net;
+  const UNetConfig& c = net.cfg();
+  const long long V = (long long)c.image_size * c.image_size * c.image_size;
+  if (c.num_classes == 0) throw std::runtime_error("mdb: mdb_solver_run_guided needs a class-conditional network (num_classes > 0)");
+  if (!classes) throw std::runtime_error("mdb: mdb_solver_run_guided needs the class ids");
+  if (w != 1.f && !eps_u_buf) throw std::runtime_error("mdb: mdb_solver_run_guided needs eps_u_buf unless w == 1");
+  if (n_entries > 0 && !entries) throw std::runtime_error("mdb: mdb_solver_run_guided needs the entry table");
+  if (known && known->noise) throw std::runtime_error("mdb: mdb_solver_run_guided draws its noise in-kernel (known->noise must be NULL)");
+  net.set_classes(classes, B, s);  // copies and checks the ids once
+  try {
+    for (int i = 0; i < n_entries; ++i) {
+      SolverEntryArgs a = entry_args(eps_buf, x, x0_hist, mask, entries[i], V, c.num_channels,
+                                     step0 + i < replace_until ? known : nullptr);
+      if (!a.renoise) {
+        net.use_null_class(false);
+        forward_at(n, x, entries[i].label, labels_buf, eps_buf, B, s);
+        if (w != 1.f) {
+          net.use_null_class(true);
+          n->net->forward(x, labels_buf, eps_u_buf, B, s, /*allow_graph=*/true);
+          a.eps_u = eps_u_buf; a.w = w;
+        }
+      }
+      // mdb_solver_run's Philox counter blocks
+      a.noise = nullptr; a.seed = seed; a.offset = 4ull * (unsigned long long)(step0 + i);
+      launch_solver_entry(a, B, s);
+    }
+  } catch (...) {
+    net.use_null_class(false);
+    throw;
+  }
+  net.use_null_class(false);
   MDB_API_END
 }
 

@@ -664,10 +664,11 @@ void launch_dense_bwd_input(const float* dy, long long dy_ld, const float* W, fl
 }
 
 // One block per sample. Recomputes emb -> t1 -> h1 -> t2 (elementwise.cu temb_kernel), then
-// dt2 = dact * silu'(t2), dh1 = W1^T dt2, dt1 = dh1 * silu'(t1).
+// dt2 = dact * silu'(t2), dh1 = W1^T dt2, dt1 = dh1 * silu'(t1). t2 includes the label embedding row when label_w is set.
 __global__ void temb_bwd_kernel(const float* __restrict__ labels, const float* __restrict__ w0, const float* __restrict__ b0,
                                 const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ dact,
-                                float* __restrict__ dt2, float* __restrict__ h1o, float* __restrict__ dt1, float* __restrict__ embo, int nf) {
+                                float* __restrict__ dt2, float* __restrict__ h1o, float* __restrict__ dt1, float* __restrict__ embo, int nf,
+                                const int* __restrict__ classes, const float* __restrict__ label_w) {
   extern __shared__ float sm[];
   const int H = 4 * nf;
   float* emb = sm;          // nf
@@ -698,6 +699,7 @@ __global__ void temb_bwd_kernel(const float* __restrict__ labels, const float* _
   for (int n = threadIdx.x; n < H; n += blockDim.x) {
     float acc = b1[n];
     for (int k = 0; k < H; ++k) acc += w1[(long long)n * H + k] * h1[k];
+    if (label_w) acc += label_w[(long long)classes[b] * H + n];
     const float sg = sigmoid_expf(acc);
     const float d = dact[(long long)b * H + n] * sg * (1.f + acc * (1.f - sg));
     d2[n] = d;
@@ -712,8 +714,26 @@ __global__ void temb_bwd_kernel(const float* __restrict__ labels, const float* _
   }
 }
 void launch_temb_bwd(const float* labels, const float* w0, const float* b0, const float* w1, const float* b1, const float* dact,
-                     float* dt2, float* h1, float* dt1, float* emb, int B, int nf, cudaStream_t s) {
-  temb_bwd_kernel<<<B, 256, (nf + 12 * nf) * sizeof(float), s>>>(labels, w0, b0, w1, b1, dact, dt2, h1, dt1, emb, nf);
+                     float* dt2, float* h1, float* dt1, float* emb, int B, int nf, cudaStream_t s, const int* classes,
+                     const float* label_w) {
+  temb_bwd_kernel<<<B, 256, (nf + 12 * nf) * sizeof(float), s>>>(labels, w0, b0, w1, b1, dact, dt2, h1, dt1, emb, nf, classes,
+                                                                  label_w);
+  MDB_LAUNCH_CHECK();
+}
+
+__global__ void label_embed_grad_kernel(const int* __restrict__ classes, const float* __restrict__ dt2, float* __restrict__ dE,
+                                        int B, int K1, int H, int accumulate) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= (long long)K1 * H) return;
+  const int k = (int)(i / H), n = (int)(i % H);
+  float acc = 0.f;
+  for (int b = 0; b < B; ++b)
+    if (__ldg(classes + b) == k) acc += dt2[(long long)b * H + n];
+  dE[i] = accumulate ? dE[i] + acc : acc;
+}
+void launch_label_embed_grad(const int* classes, const float* dt2, float* dE, int B, int K1, int H, int accumulate, cudaStream_t s) {
+  const long long n = (long long)K1 * H;
+  label_embed_grad_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(classes, dt2, dE, B, K1, H, accumulate);
   MDB_LAUNCH_CHECK();
 }
 

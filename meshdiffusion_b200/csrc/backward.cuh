@@ -87,6 +87,10 @@ void launch_dense_bwd_input(const float* dy, long long dy_ld, const float* W, fl
 // time-embedding MLP backward (recomputes the forward from labels): given d(act(temb)) [B][4nf] produces
 // dt2, h1 [B][4nf] and dt1 [B][4nf], emb [B][nf] for the outer-product weight gradients.
 void launch_temb_bwd(const float* labels, const float* w0, const float* b0, const float* w1, const float* b1, const float* dact,
-                     float* dt2, float* h1, float* dt1, float* emb, int B, int nf, cudaStream_t s);
+                     float* dt2, float* h1, float* dt1, float* emb, int B, int nf, cudaStream_t s, const int* classes = nullptr,
+                     const float* label_w = nullptr);
+// gradient of label_embed.weight [K+1][H]: dE[k][n] (+)= sum over b = 0 .. B-1 in order with classes[b] == k of dt2[b][n]
+// (one thread per (k, n), no atomics: the same bits on every run)
+void launch_label_embed_grad(const int* classes, const float* dt2, float* dE, int B, int K1, int H, int accumulate, cudaStream_t s);
 
 }  // namespace mdb

@@ -298,8 +298,10 @@ void launch_transpose_vc(const void* in, long long ld, int c0, void* out, int B,
 // get_timestep_embedding (layers.py:542-556): half = nf/2, freq_k = exp(-ln(1e4) * k / (half-1)), [sin, cos];
 // then Linear(nf,4nf) -> SiLU -> Linear(4nf,4nf) (ddpm_res64.py:132-136); ResnetBlockDDPM applies act(temb) before
 // Dense_0 (layers.py:680), so act(temb) is what every consumer needs and is what we store.
+// A class-conditional network adds its label embedding row to Linear1's output before the SiLU.
 __global__ void temb_kernel(const float* __restrict__ labels, const float* __restrict__ w0, const float* __restrict__ b0,
-                            const float* __restrict__ w1, const float* __restrict__ b1, float* __restrict__ out, int nf) {
+                            const float* __restrict__ w1, const float* __restrict__ b1, float* __restrict__ out, int nf,
+                            const int* __restrict__ classes, const float* __restrict__ label_w) {
   extern __shared__ float sm[];
   float* emb = sm;            // nf
   float* h1 = sm + nf;        // 4nf
@@ -324,12 +326,13 @@ __global__ void temb_kernel(const float* __restrict__ labels, const float* __res
   for (int n = threadIdx.x; n < H; n += blockDim.x) {
     float acc = b1[n];
     for (int k = 0; k < H; ++k) acc += w1[(long long)n * H + k] * h1[k];
+    if (label_w) acc += label_w[(long long)classes[b] * H + n];
     out[(long long)b * H + n] = silu_ex2(acc);
   }
 }
 void launch_temb(const float* labels, const float* w0, const float* b0, const float* w1, const float* b1, float* out,
-                 int B, int nf, cudaStream_t s) {
-  temb_kernel<<<B, 256, 5 * nf * sizeof(float), s>>>(labels, w0, b0, w1, b1, out, nf);
+                 int B, int nf, cudaStream_t s, const int* classes, const float* label_w) {
+  temb_kernel<<<B, 256, 5 * nf * sizeof(float), s>>>(labels, w0, b0, w1, b1, out, nf, classes, label_w);
   MDB_LAUNCH_CHECK();
 }
 

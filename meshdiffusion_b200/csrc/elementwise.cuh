@@ -35,9 +35,11 @@ void launch_softmax_rows(float* s, long long rows, int L, Precision prec, cudaSt
 void launch_transpose_vc(const void* in, long long ld_in, int c0, void* out, int B, int V, int C, int elem_bytes,
                          cudaStream_t s, long long ld_out = 0);
 
-// temb path (ddpm_res64.py:132-136 + layers.py:542-556,680): act(temb)[B][4nf]
+// temb path (ddpm_res64.py:132-136 + layers.py:542-556,680): act(temb)[B][4nf]. Class-conditional networks also pass
+// label_w = label_embed.weight [K+1][4nf] and classes [B] (ids in 0..K, K = the null class): act(temb) =
+// silu(Linear1(silu(Linear0(emb(t)))) + label_w[classes[b]]). label_w == nullptr: the unconditional network.
 void launch_temb(const float* labels, const float* w0, const float* b0, const float* w1, const float* b1, float* out,
-                 int B, int nf, cudaStream_t s);
+                 int B, int nf, cudaStream_t s, const int* classes = nullptr, const float* label_w = nullptr);
 // out[b][n] = W[n][:] . x[b][:] + bias[n]   (all Dense_0 projections at once)
 void launch_dense(const float* x, const float* w, const float* bias, float* out, int B, int K, int N, cudaStream_t s);
 
@@ -85,6 +87,7 @@ struct SamplerUpdateArgs {
 void launch_sampler_update(const SamplerUpdateArgs& a, int B, cudaStream_t s);
 
 // One entry of a solver table (csrc/solver.cu), in place, fp32 NCDHW [B][C][V]; mask g [V]:
+//   guided denoise (eps_u != nullptr): eps <- eps_u + w (eps - eps_u), each operation rounded on its own, first
 //   denoise: x0 = (x - sigma eps) inv_alpha;  x' = (c_x x + c_0 x0 [+ c_1 x0_prev] [+ c_z z]) g;  x0_hist <- x0
 //            (the c_1 term is skipped when c_1 == 0, a first-order step that does not read x0_hist; the noise term when
 //            c_z == 0)
@@ -106,6 +109,7 @@ struct SolverEntryArgs {
   unsigned channels;
   float coef, std;                  // alpha, sigma of the label the entry lands on
   const float* known_noise;         // z' [B][C][V] or null (then Philox(seed, element, offset + 2))
+  const float* eps_u; float w;      // classifier-free guidance: the null-class output and the guidance scale, or null
 };
 void launch_solver_entry(const SolverEntryArgs& a, int B, cudaStream_t s);
 

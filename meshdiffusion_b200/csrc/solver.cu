@@ -4,6 +4,7 @@
 // their tables through this one kernel. One HBM pass per entry.
 //
 // Every product and sum is rounded on its own (no FMA contraction), in this order:
+//   guided:  eps = eps_u + w*(eps_c - eps_u)   (classifier-free guidance, Ho & Salimans 2022; only when eps_u is given)
 //   denoise: x0 = (x - sigma*eps) * inv_alpha
 //            x' = ((c_x*x + c_0*x0) + c_1*x0_prev) + c_z*z   (c_1 term only if c_1 != 0, c_z term only if c_z != 0)
 //            x' = x' * g;  x0_hist <- x0
@@ -44,7 +45,12 @@ __global__ void __launch_bounds__(256) solver_update_kernel(SolverEntryArgs a) {
       const float z = a.noise ? a.noise[i] : philox_normal(a.seed, (unsigned long long)i, a.offset);
       xn = __fmul_rn(__fadd_rn(__fmul_rn(a.c_x, xv), __fmul_rn(a.c_z, z)), g);
     } else {
-      const float x0 = __fmul_rn(__fsub_rn(xv, __fmul_rn(a.sigma, a.eps[i])), a.inv_alpha);
+      float e = a.eps[i];
+      if (a.eps_u) {
+        const float eu = a.eps_u[i];
+        e = __fadd_rn(eu, __fmul_rn(a.w, __fsub_rn(e, eu)));
+      }
+      const float x0 = __fmul_rn(__fsub_rn(xv, __fmul_rn(a.sigma, e)), a.inv_alpha);
       xn = __fadd_rn(__fmul_rn(a.c_x, xv), __fmul_rn(a.c_0, x0));
       if (a.c_1 != 0.f) xn = __fadd_rn(xn, __fmul_rn(a.c_1, a.x0_hist[i]));
       if (a.c_z != 0.f) {

@@ -397,7 +397,7 @@ void UNet::build() {
   float* tb1 = P("all_modules.1.bias", {tdim});
   m = 2;
   add_step("temb", [=](cudaStream_t s, int B) {
-    launch_temb(rt_labels_, tw0, tb0, tw1, tb1, temb_act_, B, nf, s);
+    launch_temb(rt_labels_, tw0, tb0, tw1, tb1, temb_act_, B, nf, s, classes_buf_, label_w_);
     launch_dense(temb_act_, dense_w_, dense_b_, dense_out_, B, tdim, dense_total_, s);
   });
   if (train_) tape_temb();
@@ -540,6 +540,8 @@ void UNet::build() {
   }
   if (train_) tape_head(head_in, a, head_gn, "all_modules." + std::to_string(m - 1));
   release(a);
+  // registered last, so the K = 0 table is a prefix of every conditional one (the EMA checkpoint is a positional list)
+  if (cfg_.num_classes > 0) label_w_ = P("label_embed.weight", {cfg_.num_classes + 1, tdim});
   dense_total_ = dense_cursor_;
   // every parameter is registered by now: the offsets of their gradients in the flat buffer
   long long off = 0;
@@ -565,6 +567,7 @@ void UNet::build() {
 UNet::UNet(const UNetConfig& cfg, bool dry_only) : cfg_(cfg), prec_(precision_from_int(cfg.precision)) {
   if (cfg_.image_size % (1 << (cfg_.n_levels - 1)) != 0) throw std::runtime_error("mdb: image_size not divisible by 2^(levels-1)");
   if (cfg_.nf % 32 != 0) throw std::runtime_error("mdb: nf must be a multiple of 32 (GroupNorm(32))");
+  if (cfg_.num_classes < 0) throw std::runtime_error("mdb: num_classes must be >= 0");
   train_ = cfg_.training != 0;
   if (const char* e = getenv("MDB_GRAPH_MAX_BATCH")) graph_max_batch_ = atoi(e);  // 0 disables graph replay
   if (train_ && prec_ == kTF32) throw std::runtime_error("mdb: the training plan is built for bf16 or bf16x3 (split bf16) operands");
@@ -584,6 +587,13 @@ UNet::UNet(const UNetConfig& cfg, bool dry_only) : cfg_(cfg), prec_(precision_fr
   dense_b_ = (float*)dmalloc((size_t)dense_total_ * 4);
   dense_out_ = (float*)dmalloc((size_t)cfg_.max_batch * dense_total_ * 4);
   if (train_) d_dense_out_ = (float*)dmalloc((size_t)cfg_.max_batch * dense_total_ * 4);
+  if (cfg_.num_classes > 0) {
+    classes_buf_ = (int*)dmalloc((size_t)cfg_.max_batch * sizeof(int));
+    null_ids_ = (int*)dmalloc((size_t)cfg_.max_batch * sizeof(int));
+    ids_set_ = (int*)dmalloc((size_t)cfg_.max_batch * sizeof(int));
+    std::vector<int> k(cfg_.max_batch, cfg_.num_classes);
+    MDB_CUDA_CHECK(cudaMemcpy(null_ids_, k.data(), k.size() * sizeof(int), cudaMemcpyHostToDevice));
+  }
   for (auto& p : params_)
     if (!p.external) p.d = (float*)dmalloc(p.numel * 4);
   build();
@@ -638,11 +648,42 @@ void UNet::drop_graphs() {
   graphs_.clear();
 }
 
+void UNet::set_classes(const int* classes, int B, cudaStream_t s) {
+  check_runnable();
+  have_ids_ = false;
+  null_forward_ = false;
+  if (!classes) return;
+  if (cfg_.num_classes == 0) throw std::runtime_error("mdb: class ids given to an unconditional network (num_classes = 0)");
+  if (B < 1 || B > cfg_.max_batch) throw std::runtime_error("mdb: class ids: batch out of range");
+  // ordered after whatever wrote the ids on `s`, and after the forwards already enqueued there that read ids_set_
+  MDB_CUDA_CHECK(cudaMemcpyAsync(ids_set_, classes, (size_t)B * sizeof(int), cudaMemcpyDeviceToDevice, s));
+  std::vector<int> h(B);
+  MDB_CUDA_CHECK(cudaMemcpyAsync(h.data(), ids_set_, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, s));
+  MDB_CUDA_CHECK(cudaStreamSynchronize(s));
+  for (int b = 0; b < B; ++b)
+    if (h[b] < 0 || h[b] > cfg_.num_classes)
+      throw std::runtime_error("mdb: class id " + std::to_string(h[b]) + " of sample " + std::to_string(b) + " is outside 0.." +
+                               std::to_string(cfg_.num_classes) + " (" + std::to_string(cfg_.num_classes) + " = the null class)");
+  have_ids_ = true;
+  ids_B_ = B;
+}
+
+void UNet::stage_classes(int B, cudaStream_t s) {
+  if (cfg_.num_classes == 0) return;
+  const bool ids = have_ids_ && !null_forward_;
+  if (ids && ids_B_ != B)
+    throw std::runtime_error("mdb: the class ids were set for batch " + std::to_string(ids_B_) + ", the forward runs batch " +
+                             std::to_string(B));
+  MDB_CUDA_CHECK(cudaMemcpyAsync(classes_buf_, ids ? ids_set_ : null_ids_, (size_t)B * sizeof(int),
+                                 cudaMemcpyDeviceToDevice, s));
+}
+
 void UNet::forward(const float* x, const float* labels, float* out, int B, cudaStream_t s, bool allow_graph) {
   check_runnable();
   if (!committed_) throw std::runtime_error("mdb: parameters changed, call commit() before forward()");
   if (B < 1 || B > cfg_.max_batch) throw std::runtime_error("mdb: batch out of range");
   rt_x_ = x; rt_labels_ = labels; rt_out_ = out;
+  stage_classes(B, s);  // outside any graph: the graphs read classes_buf_, never the caller's ids
   if (allow_graph && !train_ && B <= graph_max_batch_) {
     FwdGraph* fg = nullptr;
     for (auto& g : graphs_) if (g.x == x && g.labels == labels && g.out == out && g.B == B) fg = &g;
@@ -681,6 +722,7 @@ std::vector<std::pair<std::string, float>> UNet::profile(const float* x, const f
   check_runnable();
   if (!committed_) throw std::runtime_error("mdb: commit() first");
   rt_x_ = x; rt_labels_ = labels; rt_out_ = out;
+  stage_classes(B, s);
   std::vector<std::pair<std::string, float>> res;
   std::vector<cudaEvent_t> ev(steps_.size() + 1);
   for (auto& e : ev) MDB_CUDA_CHECK(cudaEventCreate(&e));

@@ -29,6 +29,7 @@ struct UNetConfig {
   int max_batch = 1;
   int precision = 0;    // 0 = bf16 operands, 1 = tf32 operands, 2 = split bf16 (fp32 accumulate in all three)
   int training = 0;     // 1: keep the activations backward needs and build the backward plan (bf16 or split bf16)
+  int num_classes = 0;  // K > 0: class-conditional, label_embed.weight [K+1][4nf] (row K = the null class)
 };
 
 struct ParamInfo {
@@ -95,6 +96,14 @@ class UNet {
   void forward(const float* x, const float* labels, float* out, int B, cudaStream_t s, bool allow_graph = false);
   // training engines only. Dropout of the next forward()/backward() pair (p = 0 disables; same seed in both).
   void set_dropout(float p, unsigned long long seed);
+  // class-conditional engines: the class ids (device int32 [B], each in 0..K; nullptr = the null class K for every sample)
+  // of the following forward()/backward() pairs, which must run at batch B. The ids are copied on `s` into a buffer the
+  // engine owns and checked there (the copy back to the host synchronises `s`), so the caller's array may be freed as
+  // soon as the call returns. Every forward copies the ids in force into a second engine buffer at a fixed address,
+  // on its own stream, which is what the captured forward graphs read. K = 0 refuses a non-null pointer.
+  void set_classes(const int* classes, int B, cudaStream_t s);
+  // the following forwards run the null class (true) or the ids set last (false); mdb_solver_run_guided alternates
+  void use_null_class(bool on) { null_forward_ = on; }
   // dout: fp32 NCDHW dL/d(out) of the preceding forward() (same x, labels, B). grads: flat fp32 buffer holding the
   // gradient of every parameter in table order (params()[i] at the sum of the numels before it); entries of
   // non-trainable tensors (mask, coords, pos_layer.weight) are left untouched. accumulate: += instead of =.
@@ -158,6 +167,14 @@ class UNet {
   float* temb_act_ = nullptr;
   float* dense_w_ = nullptr; float* dense_b_ = nullptr; float* dense_out_ = nullptr;
   int dense_total_ = 0, dense_cursor_ = 0;
+  // class conditioning: label_embed.weight, the ids the forward reads ([max_batch], fixed address), K repeated
+  float* label_w_ = nullptr;
+  int* classes_buf_ = nullptr;
+  int* null_ids_ = nullptr;
+  int* ids_set_ = nullptr;      // copy of the ids given to set_classes
+  bool have_ids_ = false, null_forward_ = false;
+  int ids_B_ = 0;
+  void stage_classes(int B, cudaStream_t s);
 
   void build();
   void check_runnable() const { if (dry_) throw std::runtime_error("mdb: a dry plan cannot run"); }

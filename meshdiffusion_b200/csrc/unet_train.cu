@@ -655,9 +655,14 @@ void UNet::tape_temb() {
     const float* dd = d_dense_out_; const float* dw = dense_w_; const int dt = dense_total_;
     const long long g_w0 = G("all_modules.0.weight"), g_b0 = G("all_modules.0.bias");
     const long long g_w1 = G("all_modules.1.weight"), g_b1 = G("all_modules.1.bias");
+    const int K1 = cfg_.num_classes + 1;
+    const float* lw = cfg_.num_classes > 0 ? P("label_embed.weight", {}) : nullptr;
+    const long long g_e = cfg_.num_classes > 0 ? G("label_embed.weight") : 0;
+    const int* cls = classes_buf_;
     add_bwd("temb.bwd", [=](cudaStream_t s, int B) {
       launch_dense_bwd_input(dd, dt, dw, dact, B, dt, tdim, s);
-      launch_temb_bwd(rt_labels_, tw0, tb0, tw1, tb1, dact, dt2, h1, dt1, emb, B, nf, s);
+      launch_temb_bwd(rt_labels_, tw0, tb0, tw1, tb1, dact, dt2, h1, dt1, emb, B, nf, s, cls, lw);
+      if (lw) launch_label_embed_grad(cls, dt2, rt_grads_ + g_e, B, K1, tdim, rt_accum_ ? 1 : 0, s);
       launch_outer_sum(dt2, tdim, h1, tdim, rt_grads_ + g_w1, rt_grads_ + g_b1, B, tdim, tdim, rt_accum_ ? 1 : 0, s);
       launch_outer_sum(dt1, tdim, emb, nf, rt_grads_ + g_w0, rt_grads_ + g_b0, B, tdim, nf, rt_accum_ ? 1 : 0, s);
     }, kParamGradOnly);

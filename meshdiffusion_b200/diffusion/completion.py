@@ -293,6 +293,8 @@ def _sync(device):
 def eval_completion(config):
     """Writes this rank's completions and its metrics file; returns the report. Every argument is checked (ValueError,
     FileNotFoundError) before a network is built."""
+    from .classes import refuse_conditional
+    refuse_conditional(config, "eval_completion")
     from ..dataset.shapenet_dmtet_dataset import ShapeNetDMTetDataset
     from .trainer import _path_or_none
     ev = config.eval

@@ -237,6 +237,8 @@ def _write_json(path, obj):
 
 def distill(config):
     """Runs (or resumes) every round; returns the paths of the students' checkpoints."""
+    from .classes import refuse_conditional
+    refuse_conditional(config, "distill")
     st = settings(config)
     if config.training.sde.lower() != "vpsde":
         raise NotImplementedError(f"SDE {config.training.sde} unknown.")

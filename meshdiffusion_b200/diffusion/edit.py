@@ -169,6 +169,8 @@ def group_metrics(src_pts, src_empty, var_pts, var_empty, k):
 def edit(config):
     """Writes this rank's variants and its report; returns the report. Every argument is checked (ValueError,
     FileNotFoundError) before a network is built."""
+    from .classes import refuse_conditional
+    refuse_conditional(config, "edit")
     ev = config.eval
     k, jump, resample = edit_settings(ev)
     B = ev.batch_size

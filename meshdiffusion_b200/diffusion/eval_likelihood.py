@@ -24,6 +24,8 @@ TIMING_KEYS = ("seconds",)
 
 def eval_likelihood(config):
     """Writes `<eval_dir>/likelihood.json` and returns its content."""
+    from .classes import refuse_conditional
+    refuse_conditional(config, "eval_likelihood")
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         raise SystemExit("--mode=eval_likelihood runs in one process; start it with python, not torchrun")
     from ..dataset.shapenet_dmtet_dataset import ShapeNetDMTetDataset

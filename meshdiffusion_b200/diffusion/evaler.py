@@ -12,7 +12,7 @@ import os
 import numpy as np
 import torch
 
-from . import sampling, sde_lib
+from . import classes, sampling, sde_lib
 from .models import utils as mutils
 from .models.ema import ExponentialMovingAverage
 from .utils import restore_checkpoint
@@ -58,7 +58,7 @@ def uncond_gen(config, idx=None):
     state = restore_checkpoint(config.eval.ckpt_path, state, device=config.device)
     ema.copy_to(score_model.parameters())
     logging.info("rank %d: sampling %d grids of %d^3", idx, shape[0], R)
-    samples, _ = sampling_fn(score_model)
+    samples, _ = sampling_fn(score_model, **classes.sampling_kwargs(config))
     out = os.path.join(eval_dir, f"{idx}.npy")
     np.save(out, samples.cpu().numpy())
     return out
@@ -100,7 +100,7 @@ def cond_gen(config, save_fname=None):
     partial = torch.load(config.eval.partial_dmtet_path, map_location=device)
     sdf_grid, vis_grid = partial_grids([partial], tet_grid_coords(config.eval.tet_path, device), R, device)
     samples, _ = sampling_fn(score_model, partial=sdf_grid, partial_mask=vis_grid,
-                             freeze_iters=config.eval.freeze_iters)
+                             freeze_iters=config.eval.freeze_iters, **classes.sampling_kwargs(config))
     out = os.path.join(eval_dir, f"{save_fname}.npy")
     np.save(out, samples.cpu().numpy())
     return out

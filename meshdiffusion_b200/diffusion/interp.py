@@ -130,6 +130,8 @@ def _masked_rel_l2(x, ref, mask):
 def uncond_gen_interp(config):
     """Writes the frames of this rank's pairs and its index; returns the index. Every argument is checked (ValueError)
     before a network is built."""
+    from .classes import refuse_conditional
+    refuse_conditional(config, "uncond_gen_interp")
     ev = config.eval
     F = _frames(ev)
     shapes = _shape_pairs(ev.get("interp_shapes", None))

@@ -63,9 +63,10 @@ def get_ddpm_loss_fn(vpsde, train, mask=None, loss_type="l2"):
 
     mask_sum = [None]
 
-    def loss_fn(model, batch):
+    def loss_fn(model, batch, class_labels=None):
         dev = batch.device
-        net = mutils.get_model_fn(model, train=train)
+        model_fn = mutils.get_model_fn(model, train=train)
+        net = lambda x, t: model_fn(x, t, class_labels)  # noqa: E731
         t = torch.randint(0, vpsde.N, (batch.shape[0],), device=dev)
         eps = torch.randn_like(batch)
         if batch.is_cuda and mask is not None and loss_type == "l2" and batch.dtype == torch.float32:
@@ -114,26 +115,28 @@ def get_step_fn(sde, train, optimize_fn=None, mask=None, loss_type="l2"):
     loss_fn = get_ddpm_loss_fn(sde, train, mask=mask, loss_type=loss_type)
     update = get_update_fn(optimize_fn)
 
-    def train_step(state, batch, clear_grad, update_param):
+    def train_step(state, batch, clear_grad, update_param, class_labels=None):
         model, optimizer = state["model"], state["optimizer"]
         if clear_grad:
             optimizer.zero_grad()
-        loss = loss_fn(model, batch)
+        loss = loss_fn(model, batch, class_labels)
         update(state, loss, update_param)
         return loss
 
-    def eval_step(state, batch):
+    def eval_step(state, batch, class_labels=None):
         model, ema = state["model"], state["ema"]
         with torch.no_grad():
             ema.store(model.parameters())
             ema.copy_to(model.parameters())
             try:
-                return loss_fn(model, batch)
+                return loss_fn(model, batch, class_labels)
             finally:
                 ema.restore(model.parameters())
 
-    def step_fn(state, batch, clear_grad=True, update_param=True):
-        loss = train_step(state, batch, clear_grad, update_param) if train else eval_step(state, batch)
+    def step_fn(state, batch, clear_grad=True, update_param=True, class_labels=None):
+        """class_labels: the ids of a class-conditional network's batch (None: unconditional / the null class)."""
+        loss = (train_step(state, batch, clear_grad, update_param, class_labels) if train
+                else eval_step(state, batch, class_labels))
         return {"loss": loss}
 
     return step_fn

@@ -31,6 +31,7 @@ def arch_from_config(config):
         attn_resolutions=tuple(int(r) for r in config.model.attn_resolutions),
         num_channels=int(config.data.num_channels), stem_ksize=5 if is128 else 3, use_pos_bias=not is128,
         level0_blocks=2 if is128 else int(config.model.num_res_blocks),
+        num_classes=int(config.model.get("num_classes", 0) or 0) if hasattr(config.model, "get") else 0,
     )
 
 
@@ -47,6 +48,7 @@ def _config_c(arch, max_batch, precision, training=False):
     c.use_pos_bias = 1 if arch["use_pos_bias"] else 0
     c.max_batch, c.precision = max_batch, PRECISIONS[precision]
     c.training = 1 if training else 0
+    c.num_classes = int(arch.get("num_classes", 0))
     return c
 
 
@@ -103,17 +105,18 @@ class _ScoreNetFn(torch.autograd.Function):
     formed when autograd asks for it; with no parameter asking for one, the engine's input-only backward runs."""
 
     @staticmethod
-    def forward(ctx, net, x, labels, *params):
-        out = net._train_forward(x, labels, net._diff_precision(), net.dropout if net.training else 0.0)
+    def forward(ctx, net, x, labels, class_labels, *params):
+        out = net._train_forward(x, labels, net._diff_precision(), net.dropout if net.training else 0.0, class_labels)
         ctx.net = net
         ctx.save_for_backward(x, labels)
+        ctx.class_labels = class_labels  # the engine copied the ids on the stream; kept alive until backward
         return out
 
     @staticmethod
     def backward(ctx, dout):
         x, labels = ctx.saved_tensors
-        dx = ctx.net._train_backward(x, labels, dout, want_x=ctx.needs_input_grad[1], want_params=any(ctx.needs_input_grad[3:]))
-        return (None, dx, None) + (None,) * len(ctx.net._trainable)
+        dx = ctx.net._train_backward(x, labels, dout, want_x=ctx.needs_input_grad[1], want_params=any(ctx.needs_input_grad[4:]))
+        return (None, dx, None, None) + (None,) * len(ctx.net._trainable)
 
 
 class _Scope(nn.Module):
@@ -124,6 +127,10 @@ class ScoreNet(nn.Module):
     def __init__(self, config):
         super().__init__()
         self.arch = arch_from_config(config)
+        # class-conditional network with classifier-free guidance: K classes plus the null class K (label_embed.weight)
+        self.num_classes = self.arch["num_classes"]
+        if self.num_classes < 0:
+            raise ValueError("config.model.num_classes must be >= 0")
         # inference operand mode; the default is the parity-grade one (results within 1e-3 of the reference's fp32 arithmetic).
         # 'tf32' (1.6e-3, 1.55x faster) and 'bf16' (1.3e-2, 2.7x faster) are opt-in.
         self.precision = str(config.model.get("compute_dtype", "bf16x3")) if hasattr(config.model, "get") else "bf16x3"
@@ -165,6 +172,7 @@ class ScoreNet(nn.Module):
             if n == "mask": return (1, 0)
             if n.startswith("pos_layer."): return (2, 0)
             if n.startswith("mask_layer."): return (3, 0)
+            if n == "label_embed.weight": return (5, 0)  # not in the reference: last, so the K = 0 list is a prefix
             return (4, int(n.split(".")[1]))
         for name, shape in sorted(table, key=ref_order):
             self._register(name, self._initial_value(name, shape, head_idx), trainable=name not in ("mask", "coords"))
@@ -172,12 +180,19 @@ class ScoreNet(nn.Module):
         self._engine_batch = 0
         self._synced = None
         self._trainable = [n for n in self._names if n not in ("mask", "coords")]
+        self._bound_classes = None  # class_labels of every call inside conditioned()
+
+    def _load_from_state_dict(self, state_dict, prefix, *args):
+        # an override, not a registered hook: a bound-method hook would make the module a reference cycle, and its
+        # engines would then wait for the cyclic garbage collector instead of being freed with the last reference
+        check_class_count(state_dict, self.num_classes, prefix + "label_embed.weight")
+        super()._load_from_state_dict(state_dict, prefix, *args)
 
     # ---- parameter plumbing -------------------------------------------------------------------------------------
     def _initial_value(self, name, shape, head_idx):
         leaf = name.split(".")[-1]
-        if name == "mask" or name == "coords":
-            return torch.zeros(shape)
+        if name == "mask" or name == "coords" or name == "label_embed.weight":
+            return torch.zeros(shape)  # a zero label embedding: at initialisation the conditional net is the unconditional one
         if leaf in ("bias", "b"):
             return torch.zeros(shape)
         if "GroupNorm" in name or name == f"all_modules.{head_idx - 1}.weight":
@@ -305,7 +320,15 @@ class ScoreNet(nn.Module):
             _native.check(L.mdb_unet_grad_offset(self._train_handle, n.encode(), ctypes.byref(off)))
             _native.check(L.mdb_unet_grad_ready(self._train_handle, n.encode(), ctypes.byref(rdy)))
             entries.append((off.value, self._param(n).numel(), rdy.value))
-        self._buckets = make_grad_buckets(entries, self._flat_grad.numel(), self.bucket_bytes)
+        total = self._flat_grad.numel()
+        if self.num_classes > 0:
+            # label_embed.weight is the last slot but its gradient is final only after the last launch: a bucket of its
+            # own, so the head's gradients before it are not held back to the end of the backward pass
+            off, numel, rdy = max(entries)
+            self._buckets = sorted(make_grad_buckets([e for e in entries if e[0] != off], off, self.bucket_bytes)
+                                   + [(rdy, off, off + numel)])
+        else:
+            self._buckets = make_grad_buckets(entries, total, self.bucket_bytes)
         return self._buckets
 
     def _backward_with_overlapped_allreduce(self, dout, B, accumulate):
@@ -372,11 +395,45 @@ class ScoreNet(nn.Module):
             if src.is_cuda:
                 src.record_stream(torch.cuda.current_stream())
 
-    def _train_forward(self, x, labels, precision, p):
+    def _class_ids(self, class_labels, B, device):
+        """class_labels as the device int32 [B] the engine takes, or None (the null class). Refuses ids for an
+        unconditional network."""
+        if class_labels is None:
+            return None
+        if self.num_classes == 0:
+            raise ValueError("class_labels given to an unconditional score network (config.model.num_classes = 0)")
+        ids = torch.as_tensor(class_labels, device=device).to(torch.int32).reshape(-1)
+        if ids.numel() == 1 and B > 1:
+            ids = ids.expand(B)
+        if ids.numel() != B:
+            raise ValueError(f"class_labels holds {ids.numel()} ids for a batch of {B}")
+        return ids.contiguous()
+
+    def conditioned(self, class_labels):
+        """Context manager: calls inside that pass no class_labels (and the native sampler loops) use these."""
+        net = self
+
+        class _Bound:
+            def __enter__(self_inner):
+                net._class_ids(class_labels, 1 if class_labels is None else torch.as_tensor(class_labels).numel(), "cpu")
+                net._bound_classes = class_labels
+
+            def __exit__(self_inner, *exc):
+                net._bound_classes = None
+
+        return _Bound()
+
+    def _set_classes(self, handle, ids, B):
+        """Puts the class ids (or the null class, ids None) in force on an engine of a conditional network."""
+        if self.num_classes > 0:
+            _native.check(_native.lib().mdb_unet_set_classes(handle, _native.ptr(ids), B, _native.current_stream()))
+
+    def _train_forward(self, x, labels, precision, p, class_ids=None):
         L = _native.lib()
         B = x.shape[0]
         with torch.cuda.device(x.device):
             h = self._diff_engine(precision, B, x.device)
+            self._set_classes(h, class_ids, B)
             self._drop_calls += 1
             seed = (torch.initial_seed() * 1000003 + self._drop_calls) & 0xFFFFFFFFFFFFFFFF
             _native.check(L.mdb_unet_set_dropout(h, p, seed))
@@ -520,7 +577,9 @@ class ScoreNet(nn.Module):
         out = self._train_forward(x, labels, precision, 0.0)
         return out, self._train_backward(x, labels, v, want_x=True, want_params=False)
 
-    def forward(self, x, labels):
+    def forward(self, x, labels, class_labels=None):
+        """score_model(x, labels); a class-conditional network (num_classes K > 0) also takes `class_labels` (ids in
+        0..K-1, one per sample or one for the batch; K or None = the null class of classifier-free guidance)."""
         # input gradients through model.eval(): autograd enabled and x requiring grad runs the training-plan engine in the
         # inference operand mode with dropout 0. Its output equals the inference engine's only within the mode's tolerance
         # (the training plan materialises the nearest upsample; the inference plan folds it into eight parity
@@ -534,17 +593,19 @@ class ScoreNet(nn.Module):
         x = x.float().contiguous()
         labels = labels.to(device=x.device, dtype=torch.float32).contiguous()
         B = x.shape[0]
+        ids = self._class_ids(class_labels if class_labels is not None else self._bound_classes, B, x.device)
         # training path: model.train() + autograd enabled (what step_fn(train=True) sets up, losses.py:104-139 with
         # get_model_fn(train=True)); the input-gradient path above; everything else -- model.eval() or no_grad -- is the
         # inference engine
         if input_grad or (self.training and torch.is_grad_enabled() and any(self._param(n).requires_grad for n in self._trainable)):
-            out = _ScoreNetFn.apply(self, x, labels, *[self._param(n) for n in self._trainable])
+            out = _ScoreNetFn.apply(self, x, labels, ids, *[self._param(n) for n in self._trainable])
             if self.scale_by_sigma:
                 out = out / self.sigmas.to(out.device)[labels.long(), None, None, None, None].float()
             return out
         with torch.cuda.device(x.device):
             self._ensure_engine(B, x.device)
             self.sync_parameters()
+            self._set_classes(self._handle, ids, B)
             out = torch.empty_like(x)
             _native.check(L.mdb_unet_forward(self._handle, _native.ptr(x), _native.ptr(labels), _native.ptr(out), B,
                                              _native.current_stream()))
@@ -604,6 +665,14 @@ class ScoreNet(nn.Module):
         _native.check(L.mdb_unet_profile(self._handle, _native.ptr(x), _native.ptr(labels), _native.ptr(out), B,
                                          _native.current_stream(), names, len(names), ms, 1024, ctypes.byref(n)))
         return list(zip(names.value.decode().strip().split("\n"), [ms[i] for i in range(n.value)]))
+
+
+def check_class_count(state_dict, num_classes, key):
+    """Refuses a state dict whose label embedding (or its absence) does not match a network of `num_classes`."""
+    w = state_dict.get(key)
+    have = 0 if w is None else int(w.shape[0]) - 1
+    if have != num_classes:
+        raise ValueError(f"the checkpoint's score network has {have} classes, the config's (model.num_classes) {num_classes}")
 
 
 @utils.register_model(name="ddpm_res64")

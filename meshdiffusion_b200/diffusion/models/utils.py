@@ -57,9 +57,11 @@ def create_model(config, use_parallel=True):
 
 
 def get_model_fn(model, train=False):
-    def model_fn(x, labels):
+    def model_fn(x, labels, class_labels=None):
         model.train() if train else model.eval()
-        return model(x, labels)
+        if class_labels is None:
+            return model(x, labels)
+        return model(x, labels, class_labels=class_labels)
 
     return model_fn
 
@@ -76,9 +78,9 @@ def get_score_fn(sde, model, train=False, continuous=False, std_scale=True):
         raise NotImplementedError(f"SDE class {sde.__class__.__name__} not yet supported.")
     model_fn = get_model_fn(model, train=train)
 
-    def score_fn(x, t):
+    def score_fn(x, t, class_labels=None):
         labels = t * (sde.N - 1)
-        eps = model_fn(x, labels)
+        eps = model_fn(x, labels, class_labels)
         if not std_scale:
             return eps
         if continuous:

@@ -14,6 +14,7 @@ student (`--mode=distill`), through the same solver code.
 import abc
 import contextlib
 import ctypes
+import functools
 
 import numpy as np
 import torch
@@ -66,22 +67,24 @@ def get_sampling_fn(config, sde, shape, inverse_scaler, eps, grid_mask=None, ret
             denoise=config.sampling.noise_removal, eps=eps, device=config.device, grid_mask=grid_mask,
             return_traj=return_traj,
             max_iters=config.sampling.get("max_iters", None), native_rng=config.sampling.get("native_rng", False),
-            seed=config.get("seed", 42))
+            seed=config.get("seed", 42), guidance_scale=config.sampling.get("guidance_scale", 1.0))
     if method == "ddim":
         return get_ddim_sampler(sde=sde, shape=shape, predictor=get_predictor("ddim"), inverse_scaler=inverse_scaler,
                                 n_steps=config.sampling.n_steps_each, denoise=config.sampling.noise_removal, eps=eps,
-                                device=config.device, grid_mask=grid_mask)
+                                device=config.device, grid_mask=grid_mask,
+                                guidance_scale=config.sampling.get("guidance_scale", 1.0))
     if method == "dpm_solver":
         return get_dpm_solver_sampler(sde=sde, shape=shape, inverse_scaler=inverse_scaler,
                                       n_steps=config.sampling.get("dpm_steps", 25),
                                       stochastic=config.sampling.get("dpm_sde", False),
                                       denoise=config.sampling.noise_removal, device=config.device, grid_mask=grid_mask,
-                                      native_rng=config.sampling.get("native_rng", False), seed=config.get("seed", 42))
+                                      native_rng=config.sampling.get("native_rng", False), seed=config.get("seed", 42),
+                                      guidance_scale=config.sampling.get("guidance_scale", 1.0))
     if method == "distilled":
         return get_distilled_sampler(sde=sde, shape=shape, inverse_scaler=inverse_scaler,
                                      n_steps=config.sampling.get("distill_steps", 8), device=config.device,
                                      grid_mask=grid_mask, native_rng=config.sampling.get("native_rng", False),
-                                     seed=config.get("seed", 42))
+                                     seed=config.get("seed", 42), guidance_scale=config.sampling.get("guidance_scale", 1.0))
     raise ValueError(f"Sampler name {method} unknown.")
 
 
@@ -265,7 +268,7 @@ def _rank():
 
 def get_pc_sampler(sde, shape, predictor, corrector, inverse_scaler, snr, n_steps=1, probability_flow=False,
                    continuous=False, denoise=True, eps=1e-3, device="cuda", grid_mask=None, return_traj=False,
-                   max_iters=None, native_rng=False, seed=42):
+                   max_iters=None, native_rng=False, seed=42, guidance_scale=1.0):
     """Returns `pc_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None)`.
 
     `max_iters` truncates the loop to its first iterations of the N-step schedule (used by the plumbing config;
@@ -290,8 +293,9 @@ def get_pc_sampler(sde, shape, predictor, corrector, inverse_scaler, snr, n_step
         eps_pred = model(x, t * torch.ones(shape[0], device=x.device))
         return ((x - a2 * eps_pred) / a1).clamp(-1, 1) * mask
 
-    def pc_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None):
-        with torch.no_grad():
+    def pc_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, class_labels=None,
+                   guidance_scale=guidance_scale):
+        with _conditioned(model, class_labels, guidance_scale, "pc") as model, torch.no_grad():
             if freeze_iters is None:
                 freeze_iters = sde.N + 10
             c = partial_channel
@@ -382,6 +386,23 @@ def get_pc_sampler(sde, shape, predictor, corrector, inverse_scaler, snr, n_step
     return pc_sampler
 
 
+@contextlib.contextmanager
+def _conditioned(model, class_labels, guidance_scale, name):
+    """The pc and ddim samplers condition on class_labels without guidance: yields the model to call."""
+    if float(guidance_scale) != 1.0:
+        raise ValueError(f"the {name} sampler supports class conditioning without guidance only (guidance_scale = 1, "
+                         f"got {guidance_scale}); use sampling.method='dpm_solver' or 'distilled' for guidance")
+    if class_labels is None:
+        yield model
+        return
+    net = _native_net(model)
+    if net is None:
+        yield functools.partial(model, class_labels=class_labels)
+        return
+    with net.conditioned(class_labels):
+        yield model
+
+
 def _native_loop(net, x, mask_flat, labels, betas, stds, total, seed, step0=0, cond=None, cond_until=0):
     """Steps step0 .. step0+total-1 of the loop inside the library (mdb_sampler_run): no Python between steps. The
     schedule lists are indexed by the GLOBAL step; `cond` (a _Cond) switches on the partial branch's replacement
@@ -390,6 +411,7 @@ def _native_loop(net, x, mask_flat, labels, betas, stds, total, seed, step0=0, c
     B = x.shape[0]
     net._ensure_engine(B, x.device)
     net.sync_parameters()
+    net._set_classes(net._handle, net._class_ids(net._bound_classes, B, x.device), B)
     x_mean = torch.empty_like(x)
     eps_buf = torch.empty_like(x)
     labels_buf = torch.empty(B, device=x.device, dtype=torch.float32)
@@ -428,9 +450,10 @@ class DDIMPredictor(Predictor):
 
 
 def get_ddim_sampler(sde, shape, predictor, inverse_scaler, n_steps=1, denoise=False, eps=1e-3, device="cuda",
-                     grid_mask=None):
-    def ddim_sampler(model, schedule="quad", num_steps=100, x0=None, partial=None, partial_mask=None, partial_channel=0):
-        with torch.no_grad():
+                     grid_mask=None, guidance_scale=1.0):
+    def ddim_sampler(model, schedule="quad", num_steps=100, x0=None, partial=None, partial_mask=None, partial_channel=0,
+                     class_labels=None, guidance_scale=guidance_scale):
+        with _conditioned(model, class_labels, guidance_scale, "ddim") as model, torch.no_grad():
             x = (x0 if x0 is not None else sde.prior_sampling(shape).to(device)) * grid_mask
             c = partial_channel
             if partial is not None:
@@ -689,14 +712,17 @@ def _replace_channel(xc, known, kmask, mask, coef, std, z):
     return (xc * (1.0 - kmask) + sampled * kmask) * mask
 
 
-def _update_eager(eps, x, x0_hist, mask, row, noise=None, known=None, known_noise=None):
+def _update_eager(eps, x, x0_hist, mask, row, noise=None, known=None, known_noise=None, eps_u=None, w=1.0):
     """One entry in torch fp32 ops, in place on x and x0_hist, with the operation order of solver_update_kernel (each
     product and sum rounded on its own), so it is the kernel's bit-exact oracle. `row`: a float32 REPAINT_COLUMNS row
-    (_rows32); `mask` broadcasts over x; `known`: a _Known; known_noise: z' shaped like x."""
+    (_rows32); `mask` broadcasts over x; `known`: a _Known; known_noise: z' shaped like x. With `eps_u` (the null-class
+    output) a denoise entry uses the guided eps_u + w (eps - eps_u) in place of eps."""
     kind, _, sg, inv_a, c_x, c_0, c_1, c_z, coef, std = (float(v) for v in row)
     if kind:
         xn = (x * c_x + noise * c_z) * mask
     else:
+        if eps_u is not None:
+            eps = eps_u + (eps - eps_u) * float(np.float32(w))
         x0 = (x - eps * sg) * inv_a
         xn = x * c_x + x0 * c_0
         if c_1 != 0.0:
@@ -712,11 +738,19 @@ def _update_eager(eps, x, x0_hist, mask, row, noise=None, known=None, known_nois
     return x
 
 
-def _update(eps, x, x0_hist, mask_flat, entry_c, noise=None, known=None, known_noise=None, seed=0, offset=0):
-    """One entry through mdb_solver_update, in place on x and x0_hist; noise=None draws it in-kernel."""
+def _update(eps, x, x0_hist, mask_flat, entry_c, noise=None, known=None, known_noise=None, seed=0, offset=0, eps_u=None,
+            w=1.0):
+    """One entry through mdb_solver_update (mdb_solver_update_guided with `eps_u`), in place on x and x0_hist;
+    noise=None draws it in-kernel."""
     L = _native.lib()
     B, C = x.shape[0], x.shape[1]
     ks = known.struct(noise=known_noise) if known is not None else None
+    if eps_u is not None:
+        _native.check(L.mdb_solver_update_guided(_native.ptr(eps), _native.ptr(eps_u), float(w), _native.ptr(x),
+                                                 _native.ptr(x0_hist), _native.ptr(mask_flat), ctypes.byref(entry_c),
+                                                 x[0, 0].numel(), C, B, _native.ptr(noise), int(seed), int(offset),
+                                                 ctypes.byref(ks) if ks is not None else None, _native.current_stream()))
+        return x
     _native.check(L.mdb_solver_update(_native.ptr(eps), _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat),
                                       ctypes.byref(entry_c), x[0, 0].numel(), C, B, _native.ptr(noise), int(seed),
                                       int(offset), ctypes.byref(ks) if ks is not None else None,
@@ -724,10 +758,12 @@ def _update(eps, x, x0_hist, mask_flat, entry_c, noise=None, known=None, known_n
     return x
 
 
-def _native_run(net, x, x0_hist, mask_flat, entries_c, seed, step0=0, n=None, known=None, replace_until=None):
+def _native_run(net, x, x0_hist, mask_flat, entries_c, seed, step0=0, n=None, known=None, replace_until=None,
+                class_ids=None, w=1.0):
     """Entries step0 .. step0+n-1 of a table inside the library (mdb_solver_run), in place on x and x0_hist. `entries_c`
     is the whole table (_entries_c), indexed by the GLOBAL entry; `known` is replaced after the global entries below
-    `replace_until` (default: all of them)."""
+    `replace_until` (default: all of them). With `class_ids` (device int32 [B]) the table runs through
+    mdb_solver_run_guided at guidance scale w."""
     L = _native.lib()
     B = x.shape[0]
     n = len(entries_c) - step0 if n is None else n
@@ -738,6 +774,15 @@ def _native_run(net, x, x0_hist, mask_flat, entries_c, seed, step0=0, n=None, kn
     labels_buf = torch.empty(B, device=x.device, dtype=torch.float32)
     part = (_native.SolverEntryC * n).from_buffer(entries_c, step0 * ctypes.sizeof(_native.SolverEntryC))
     ks = known.struct() if known is not None else None
+    if class_ids is not None:
+        eps_u_buf = torch.empty_like(x) if w != 1.0 else None
+        _native.check(L.mdb_solver_run_guided(net._handle, _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat), part,
+                                              n, B, int(seed), _native.ptr(class_ids), float(w), _native.ptr(eps_buf),
+                                              _native.ptr(eps_u_buf), _native.ptr(labels_buf), int(step0),
+                                              ctypes.byref(ks) if ks is not None else None, int(replace_until),
+                                              _native.current_stream()))
+        return x
+    net._set_classes(net._handle, None, B)
     _native.check(L.mdb_solver_run(net._handle, _native.ptr(x), _native.ptr(x0_hist), _native.ptr(mask_flat), part, n, B,
                                    int(seed), _native.ptr(eps_buf), _native.ptr(labels_buf), int(step0),
                                    ctypes.byref(ks) if ks is not None else None, int(replace_until),
@@ -745,15 +790,23 @@ def _native_run(net, x, x0_hist, mask_flat, entries_c, seed, step0=0, n=None, kn
     return x
 
 
-def _run_table(sde, table, model, x, grid_mask, name, known=None, replace_until=None, native=False, seed=0):
+def _run_table(sde, table, model, x, grid_mask, name, known=None, replace_until=None, native=False, seed=0,
+               class_labels=None, w=1.0):
     """Runs a solver table on x (fp32 [B, C, R, R, R]) and returns the result: the driver behind the four table samplers.
 
     x is multiplied by the grid mask first. With `known` (a _Known) its kept region is replaced at label N - 1 (alpha,
     sigma of N - 1, fresh noise), then after every entry below `replace_until` (default: all). Paths: with `native`, a
     native ScoreNet and x on CUDA the whole table runs in the library (mdb_solver_run, Philox noise keyed by `seed` and
     the entry); other CUDA states run model + mdb_solver_update per entry with torch.randn_like noise; CPU tensors run the
-    eager fp32 update (_update_eager), which is the kernel's oracle."""
+    eager fp32 update (_update_eager), which is the kernel's oracle.
+
+    `class_labels` (ids of a class-conditional model, one per sample or one for the batch) conditions every network
+    call; with w != 1 each denoise entry also calls the model without them (the null class) and uses the classifier-free
+    guided eps_u + w (eps_c - eps_u)."""
     B = x.shape[0]
+    w = float(w)
+    if w != 1.0 and class_labels is None:
+        raise ValueError(f"{name}: guidance_scale {w} needs class_labels")
     if grid_mask.numel() != x[0, 0].numel():
         raise ValueError(f"{name}: grid_mask must hold one value per voxel")
     mask_v = grid_mask.to(device=x.device, dtype=torch.float32).reshape(x.shape[2:]).contiguous()
@@ -770,24 +823,31 @@ def _run_table(sde, table, model, x, grid_mask, name, known=None, replace_until=
     net = _native_net(model)
     if native and x.is_cuda and net is not None:
         net._ensure_engine(B, x.device)
+        ids = net._class_ids(class_labels, B, x.device)
         with net.frozen():  # nobody edits the weights inside the loop: skip per-step change detection
             return _native_run(net, x, x0_hist, mask_v.reshape(-1), entries_c, seed, known=known,
-                               replace_until=replace_until)
+                               replace_until=replace_until, class_ids=ids, w=w)
     for e, row in enumerate(rows):
         renoise = row[0] != 0
-        eps = None if renoise else model(x, torch.full((B,), float(row[1]), device=x.device)).float()
+        eps = eps_u = None
+        if not renoise:
+            lab = torch.full((B,), float(row[1]), device=x.device)
+            eps = (model(x, lab) if class_labels is None else model(x, lab, class_labels=class_labels)).float()
+            if w != 1.0:
+                eps_u = model(x, lab).float().contiguous()
         noise = torch.randn_like(x) if (renoise or row[7] != 0) else None
         ke = known if e < replace_until else None
         z2 = ke.noise(x) if ke is not None else None
         if x.is_cuda:
-            _update(None if renoise else eps.contiguous(), x, x0_hist, mask_v.reshape(-1), entries_c[e], noise, ke, z2)
+            _update(None if renoise else eps.contiguous(), x, x0_hist, mask_v.reshape(-1), entries_c[e], noise, ke, z2,
+                    eps_u=eps_u, w=w)
         else:
-            _update_eager(eps, x, x0_hist, mask_v, row, noise, ke, z2)
+            _update_eager(eps, x, x0_hist, mask_v, row, noise, ke, z2, eps_u=eps_u, w=w)
     return x
 
 
 def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=False, denoise=True, device="cuda",
-                           grid_mask=None, native_rng=False, seed=42):
+                           grid_mask=None, native_rng=False, seed=42, guidance_scale=1.0):
     """Returns `dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None)`
     -> (samples, number of network evaluations), the signature of pc_sampler, on dpm_solver_schedule's labels and table.
 
@@ -797,25 +857,32 @@ def get_dpm_solver_sampler(sde, shape, inverse_scaler, n_steps=25, stochastic=Fa
     sigma of n_{k+1}), with fresh per-sample noise; the x0 history keeps the network's prediction. Paths (_run_table): on
     CUDA with `native_rng` and a native ScoreNet the whole loop runs in the library (mdb_solver_run, Philox noise keyed by
     seed + rank and step); other CUDA states run model + mdb_solver_update per step with torch.randn_like noise; CPU
-    tensors run the eager fp32 update (_update_eager), which is the kernel's oracle."""
+    tensors run the eager fp32 update (_update_eager), which is the kernel's oracle.
+
+    The sampler also takes `class_labels` (a class-conditional model's ids) and `guidance_scale` (w, default the one
+    given here): w != 1 is classifier-free guidance, two network evaluations per step (_run_table)."""
     labels, table = dpm_solver_schedule(sde, n_steps, stochastic, denoise)
-    return _solver_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, "dpm_solver")
+    return _solver_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, "dpm_solver",
+                           guidance_scale)
 
 
-def get_distilled_sampler(sde, shape, inverse_scaler, n_steps=8, device="cuda", grid_mask=None, native_rng=False, seed=42):
+def get_distilled_sampler(sde, shape, inverse_scaler, n_steps=8, device="cuda", grid_mask=None, native_rng=False, seed=42,
+                          guidance_scale=1.0):
     """The sampler of a progressively distilled student (`sampling.method='distilled'`, `sampling.distill_steps`): the
     DDIM ODE on `ddim_grid(sde, n_steps)`, through get_dpm_solver_sampler's paths and conditioning with the first-order
     rows of `ddim_table`. Same signature and return as get_dpm_solver_sampler."""
     labels = ddim_grid(sde, n_steps)
     return _solver_sampler(sde, shape, inverse_scaler, labels, ddim_table(sde, labels), device, grid_mask, native_rng,
-                           seed, "distilled")
+                           seed, "distilled", guidance_scale)
 
 
-def _solver_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, name):
+def _solver_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask, native_rng, seed, name, guidance_scale=1.0):
     """get_dpm_solver_sampler's sampler on any 9-column solver table along `labels`."""
     K_eff = len(labels) - 1
 
-    def dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None):
+    def dpm_solver_sampler(model, partial=None, partial_mask=None, partial_channel=0, freeze_iters=None, x0=None,
+                           class_labels=None, guidance_scale=guidance_scale):
+        w = float(guidance_scale)
         with torch.no_grad():
             if freeze_iters is None:
                 freeze_iters = sde.N + 10
@@ -832,8 +899,8 @@ def _solver_sampler(sde, shape, inverse_scaler, labels, table, device, grid_mask
                 kept[:, c] = partial[:, c]
                 known = _Known(kept, partial_mask[:, c].to(x.device), [c], shape[0], full_noise=False)
                 until = sum(1 for k in range(K_eff - 1) if sde.N - 1 - labels[k] < freeze_iters)
-            x = _run_table(sde, table, model, x, grid_mask, name, known, until, native_rng, seed + _rank())
-            return inverse_scaler(x), K_eff
+            x = _run_table(sde, table, model, x, grid_mask, name, known, until, native_rng, seed + _rank(), class_labels, w)
+            return inverse_scaler(x), K_eff * (2 if w != 1.0 else 1)
 
     return dpm_solver_sampler
 

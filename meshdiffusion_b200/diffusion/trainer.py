@@ -103,22 +103,39 @@ def make_train_step(config, state, sde, mask):
     step_fn = losses.get_step_fn(sde, train=True, optimize_fn=data_parallel_optimize_fn(config, net), mask=mask,
                                  loss_type=config.training.loss_type)
 
-    def train_step_fn(state, batch, clear_grad=True, update_param=True):
+    def train_step_fn(state, batch, clear_grad=True, update_param=True, class_labels=None):
         net.reduce_in_backward = bool(update_param)  # gradients are exchanged once per optimiser step
-        return step_fn(state, batch, clear_grad=clear_grad, update_param=update_param)
+        return step_fn(state, batch, clear_grad=clear_grad, update_param=update_param, class_labels=class_labels)
 
     return train_step_fn
 
 
 def batch_source(config, mask, local_batch, rank=0, world=1):
     """`next_batch(generator)` -> this rank's next training batch [local_batch, C, R, R, R] on config.device: on-device
-    synthetic grids (`data.synthetic`) or the dataset (trainer.py:64-75 of the reference)."""
+    synthetic grids (`data.synthetic`) or the dataset (trainer.py:64-75 of the reference). A class-conditional network
+    (model.num_classes K > 0) gets (batch, class ids int64 [local_batch]) instead: one dataset per
+    `data.class_meta_paths` entry, or synthetic grids whose sphere radius follows a class drawn from `generator`."""
+    from . import classes
     device = config.device
     R = config.data.image_size
     synthetic = bool(config.data.get("synthetic", False))
+    K = classes.validate(config)
     data_iter = train_loader = sampler = None
     epoch = 0
-    if not synthetic:
+    if not synthetic and K > 0:
+        from ..dataset.shapenet_dmtet_dataset import ShapeNetDMTetDataset
+        metas = config.data.get("class_meta_paths", None)
+        if classes._unset(metas):
+            raise ValueError("training a class-conditional network (model.num_classes > 0) needs data.class_meta_paths "
+                             "or data.synthetic")
+        filters = config.data.get("class_filter_meta_paths", None)
+        filters = [None] * K if classes._unset(filters) else [_path_or_none(f) for f in filters]
+        dataset = classes.class_dataset([
+            ShapeNetDMTetDataset(m, deform_scale=config.model.get("deform_scale", 1.0), aug=True, grid_mask=mask.cpu(),
+                                 filter_meta_path=f, normalize_sdf=config.data.get("normalize_sdf", True),
+                                 extension=config.data.get("extension", "pt"))
+            for m, f in zip(metas, filters)])
+    elif not synthetic:
         # trainer.py:64-75 of the reference: JSON list of per-shape grids, shuffled DataLoader; under torchrun every rank
         # reads its own shard (DistributedSampler) instead of nn.DataParallel scattering one batch
         from ..dataset.shapenet_dmtet_dataset import ShapeNetDMTetDataset
@@ -126,6 +143,7 @@ def batch_source(config, mask, local_batch, rank=0, world=1):
                                        grid_mask=mask.cpu(), filter_meta_path=_path_or_none(config.data.get("filter_meta_path", None)),
                                        normalize_sdf=config.data.get("normalize_sdf", True),
                                        extension=config.data.get("extension", "pt"))
+    if not synthetic:
         if world > 1:
             sampler = torch.utils.data.distributed.DistributedSampler(dataset, num_replicas=world, rank=rank, shuffle=True,
                                                                       seed=int(config.get("seed", 42)))
@@ -135,6 +153,9 @@ def batch_source(config, mask, local_batch, rank=0, world=1):
 
     def next_batch(gen):
         nonlocal data_iter, epoch
+        if synthetic and K > 0:
+            y = torch.randint(0, K, (local_batch,), device=device, generator=gen)
+            return classes.synthetic_class_grids(y, R, device, gen) * mask, y
         if synthetic:
             return synthetic_grids(local_batch, R, device, gen) * mask
         try:
@@ -145,6 +166,8 @@ def batch_source(config, mask, local_batch, rank=0, world=1):
                 sampler.set_epoch(epoch)  # a new shuffle every epoch
             data_iter = iter(train_loader)
             batch = next(data_iter)
+        if K > 0:
+            return batch[0].to(device, non_blocking=True), batch[1].to(device, non_blocking=True)
         return batch.to(device, non_blocking=True)
 
     return next_batch
@@ -187,14 +210,18 @@ def train(config):
     iter_size = config.training.iter_size
     num_train_steps = config.training.n_iters
     gen = torch.Generator(device=device).manual_seed(int(config.get("seed", 42)) + rank)
+    from . import classes
+    K, class_dropout = classes.num_classes(config), float(config.training.get("class_dropout", 0.1))
     if rank == 0:
         logging.info("Training operand mode: %s (training.compute_dtype).", score_model.module.train_precision)
     logging.info("Starting training loop at step %d.", initial_step // iter_size)
     for step in range(initial_step // iter_size, num_train_steps + 1):
         tmp_loss = 0.0
         for inner in range(iter_size):
-            batch = next_batch(gen)
-            loss = train_step_fn(state, batch, clear_grad=(inner == 0), update_param=(inner == iter_size - 1))["loss"]
+            batch, kw = next_batch(gen), {}
+            if K > 0:  # (grids, class ids); labels dropped to the null class from this rank's generator
+                batch, kw = batch[0], {"class_labels": classes.drop_labels(batch[1], K, class_dropout, gen)}
+            loss = train_step_fn(state, batch, clear_grad=(inner == 0), update_param=(inner == iter_size - 1), **kw)["loss"]
             tmp_loss += loss.item()
         tmp_loss /= iter_size
         if step % config.training.log_freq == 0 and rank == 0:

@@ -38,6 +38,10 @@ def restore_checkpoint(ckpt_dir, state, device, strict=False):
         logging.warning("No checkpoint found at %s. Returned the same state as input", ckpt_dir)
         return state
     blob = torch.load(ckpt_dir, map_location=device, weights_only=False)
+    net = getattr(state["model"], "module", None)
+    if hasattr(net, "num_classes"):  # before the optimiser's positional state is matched against the parameters
+        from .models.ddpm import check_class_count
+        check_class_count(blob["model"], net.num_classes, "module.label_embed.weight")
     for key in CKPT_FIELDS:
         if key == "step":
             state[key] = blob[key]
