@@ -350,6 +350,90 @@ int mdb_groupnorm_act_backward_prec(const void* x, const long long* stats, const
                                     int precision, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Implicit-GEMM test entry points: one GemmOp (or one of the engine's multi-launch composites) built from a description
+ * with the builder calls the engine uses, so a test can compare a single variant with a reference of that operation.
+ * Activations are NDHWC rows in the operand format of `precision` (split bf16: the hi parts of a row's channels, then
+ * their lo parts, `lo_off` logical elements further on). All of them synchronise the stream.
+ */
+/* One A source: [batch_plan][z][y][x] voxels of `channels` channels, `ld` logical elements apart (0 = channels). */
+typedef struct mdb_gemm_src {
+  const void* ptr;
+  int channels, x, y, z;
+  long long ld;
+} mdb_gemm_src;
+enum { MDB_PROBE_CONV = 0, MDB_PROBE_CONV_UP2 = 1, MDB_PROBE_CONV_DGRAD = 2, MDB_PROBE_POINTWISE = 3, MDB_PROBE_ACT_B = 4 };
+typedef struct mdb_gemm_probe_desc {
+  int precision;          /* 0 bf16, 1 tf32, 2 split bf16 */
+  int kind;               /* MDB_PROBE_*: add_conv, add_conv_up2, add_conv_dgrad, add_pointwise, add_pointwise_w(NULL) */
+  int ksize, stride;      /* conv: k in {1,3,5}, stride 1 | 2; dgrad: k */
+  int parity;             /* conv_up2: px | py << 1 | pz << 2 */
+  int n_src;              /* 1 or 2 (the channel concatenation) */
+  mdb_gemm_src src[2];
+  /* conv: OIDHW [n][sum C][k^3]; conv_up2: the 3^3 OIDHW weight [n][C][27], folded by launch_upconv_weights;
+   * dgrad: the forward conv's OIDHW [C of src 0][n][k^3]; pointwise: [in][out] (w_in_out) or [out][in]. fp32. */
+  const float* w;
+  int w_in_out;
+  /* activation B (MDB_PROBE_ACT_B): B[batch][n][k], rows b_row_stride and samples b_batch_stride logical elements apart */
+  const void* b_ptr;
+  int b_k, b_n;
+  long long b_row_stride, b_batch_stride;
+  /* extra pointwise k-steps in the same accumulator (the NIN shortcut of a resblock's Conv_1): W_extra [in][out] */
+  int n_extra;
+  mdb_gemm_src extra[2];
+  const float* w_extra;
+  /* output (set_output_strided): grid x, y, z of the planned batch, n columns, logical strides */
+  int x, y, z, n;
+  void* out;
+  long long osx, osy, osz, osb, lo_off;  /* lo_off < 0: osx */
+  int out_fp32;
+  /* epilogue */
+  const float* bias;
+  const float* rowbias;
+  long long rowbias_ld;
+  const void* residual;   /* in the operand format */
+  long long res_ld, res_batch_stride;
+  long long* stats;
+  float alpha;            /* 0 = 1 */
+  int splits;             /* 0 = none, -1 = plan_splits as the engine calls it, > 1 = forced (clamped to the k-groups) */
+  int batch_plan, batch;  /* built for batch_plan samples, launched at batch (<= batch_plan; <= 0: batch_plan) */
+  int dry;                /* 1: describe only (no CUDA call; pointers may be NULL) and fill the report */
+  /* GroupNorm(32, eps 1e-6) backward (bf16 / split bf16; the training plan's data-gradient GEMMs): the GEMM result `out`
+   * (dense, n = gn_c0 + gn_c1 channels) is dL/da of a = dropout(act(GroupNorm(x))) over the concatenation x = {gn_x0,
+   * gn_x1} (dense rows, forward statistics as mdb_conv3d writes them). gnb = 1: the fused epilogue (set_gn_backward,
+   * after launch_gn_consts; then launch_gnb_tile_reduce and launch_gn_bwd_apply), as the training plan builds it;
+   * gnb = 2: the same GEMM without it, then launch_gn_bwd_reduce and launch_gn_bwd_apply (the two-pass path). Both
+   * overwrite `out` with dL/dy and write gn_dx [batch][voxels][n] and gn_dgamma / gn_dbeta [n] (fp32). */
+  int gnb;
+  const void* gn_x0; int gn_c0;
+  const void* gn_x1; int gn_c1;
+  const long long* gn_stats0; const long long* gn_stats1;
+  const float* gn_gamma; const float* gn_beta;
+  int gn_silu;
+  float gn_dropout;                /* p of the dropout after the activation (0 = none) */
+  unsigned long long gn_seed;      /* the layer's dropout seed */
+  void* gn_dx; float* gn_dgamma; float* gn_dbeta;
+} mdb_gemm_probe_desc;
+/* What mdb_unet_gemm_tiles and mdb_unet_gemm_ops report for a launch at its planned batch. */
+typedef struct mdb_gemm_probe_report {
+  int work_items, splits, ksteps, entry_ksteps, block_n;
+  double flops, fill_bytes;
+} mdb_gemm_probe_report;
+int mdb_gemm_probe(const mdb_gemm_probe_desc* desc, mdb_gemm_probe_report* report, void* stream);
+/* The inference plan's sub-pixel Upsample + conv3^3 (the engine's own construction): x [batch_plan][r^3][C] -> out
+ * [batch_plan][(2r)^3][C]; w fp32 OIDHW [C][C][27], bias [C], stats as in mdb_conv3d (nullable). w8: caller scratch of
+ * 64 C^2 floats that receives the fold [8 parities][C][C][2][2][2]. parity_mask: bit p launches parity class p.
+ * reports (nullable): the 8 parity ops. dry: describe only. */
+int mdb_upsample_conv(const void* x, const float* w, const float* bias, float* w8, void* out, long long* stats, int r,
+                      int C, int batch_plan, int batch, int parity_mask, int precision, int dry,
+                      mdb_gemm_probe_report* reports, void* stream);
+/* The attention core of the engine's AttnBlock over qkv rows [batch_plan][V][3C] (q | k | v): stage bit 0 = v^T into
+ * vT [batch_plan][C][V], bit 1 = logits S = q k^T / sqrt(C) (fp32 [batch_plan][V][V]), bit 2 = softmax of the rows of S
+ * in place (probabilities in the operand format at the start of each fp32 row), bit 3 = O = P v ([batch_plan][V][C]).
+ * reports (nullable): the qk and pv ops. */
+int mdb_attention_core(const void* qkv, void* vT, float* S, void* O, int V, int C, int batch_plan, int batch, int stages,
+                       int precision, int dry, mdb_gemm_probe_report* reports, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Marching tetrahedra. Replaces DMTet.__call__ (nvdiffrec/lib/geometry/dmtet.py:105-163; tables :34-54, map_uv
  * :70-99) for a batch of samples over one static tet grid. Integer outputs (faces, uv_idx, face_to_tet,
  * valid_vert_idx; all int64 like the reference's torch.long) are bit-exact with the reference ordering.

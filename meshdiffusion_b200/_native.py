@@ -68,6 +68,46 @@ class SolverKnownC(ctypes.Structure):
     ]
 
 
+class GemmSrcC(ctypes.Structure):
+    """mdb_gemm_src (include/meshdiff_b200.h)."""
+    _fields_ = [("ptr", ctypes.c_void_p), ("channels", ctypes.c_int), ("x", ctypes.c_int), ("y", ctypes.c_int),
+                ("z", ctypes.c_int), ("ld", ctypes.c_longlong)]
+
+
+PROBE_CONV, PROBE_CONV_UP2, PROBE_CONV_DGRAD, PROBE_POINTWISE, PROBE_ACT_B = range(5)
+
+
+class GemmProbeDescC(ctypes.Structure):
+    """mdb_gemm_probe_desc (include/meshdiff_b200.h)."""
+    _fields_ = [
+        ("precision", ctypes.c_int), ("kind", ctypes.c_int), ("ksize", ctypes.c_int), ("stride", ctypes.c_int),
+        ("parity", ctypes.c_int), ("n_src", ctypes.c_int), ("src", GemmSrcC * 2),
+        ("w", ctypes.c_void_p), ("w_in_out", ctypes.c_int),
+        ("b_ptr", ctypes.c_void_p), ("b_k", ctypes.c_int), ("b_n", ctypes.c_int),
+        ("b_row_stride", ctypes.c_longlong), ("b_batch_stride", ctypes.c_longlong),
+        ("n_extra", ctypes.c_int), ("extra", GemmSrcC * 2), ("w_extra", ctypes.c_void_p),
+        ("x", ctypes.c_int), ("y", ctypes.c_int), ("z", ctypes.c_int), ("n", ctypes.c_int), ("out", ctypes.c_void_p),
+        ("osx", ctypes.c_longlong), ("osy", ctypes.c_longlong), ("osz", ctypes.c_longlong), ("osb", ctypes.c_longlong),
+        ("lo_off", ctypes.c_longlong), ("out_fp32", ctypes.c_int),
+        ("bias", ctypes.c_void_p), ("rowbias", ctypes.c_void_p), ("rowbias_ld", ctypes.c_longlong),
+        ("residual", ctypes.c_void_p), ("res_ld", ctypes.c_longlong), ("res_batch_stride", ctypes.c_longlong),
+        ("stats", ctypes.c_void_p), ("alpha", ctypes.c_float), ("splits", ctypes.c_int),
+        ("batch_plan", ctypes.c_int), ("batch", ctypes.c_int), ("dry", ctypes.c_int),
+        ("gnb", ctypes.c_int), ("gn_x0", ctypes.c_void_p), ("gn_c0", ctypes.c_int), ("gn_x1", ctypes.c_void_p),
+        ("gn_c1", ctypes.c_int), ("gn_stats0", ctypes.c_void_p), ("gn_stats1", ctypes.c_void_p),
+        ("gn_gamma", ctypes.c_void_p), ("gn_beta", ctypes.c_void_p), ("gn_silu", ctypes.c_int),
+        ("gn_dropout", ctypes.c_float), ("gn_seed", ctypes.c_ulonglong),
+        ("gn_dx", ctypes.c_void_p), ("gn_dgamma", ctypes.c_void_p), ("gn_dbeta", ctypes.c_void_p),
+    ]
+
+
+class GemmProbeReportC(ctypes.Structure):
+    """mdb_gemm_probe_report (include/meshdiff_b200.h)."""
+    _fields_ = [("work_items", ctypes.c_int), ("splits", ctypes.c_int), ("ksteps", ctypes.c_int),
+                ("entry_ksteps", ctypes.c_int), ("block_n", ctypes.c_int), ("flops", ctypes.c_double),
+                ("fill_bytes", ctypes.c_double)]
+
+
 # name -> (restype, argtypes); the symbol list is checked against the header by tests/test_abi.py
 _vp, _i, _ll, _f, _u64, _d = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float, ctypes.c_ulonglong, ctypes.c_double
 SIGNATURES = {
@@ -126,6 +166,9 @@ SIGNATURES = {
     "mdb_groupnorm_act_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _i, _i, _f, _u64, _vp]),
     "mdb_conv3d_backward_prec": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "mdb_groupnorm_act_backward_prec": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _i, _i, _f, _u64, _i, _vp]),
+    "mdb_gemm_probe": (_i, [ctypes.POINTER(GemmProbeDescC), ctypes.POINTER(GemmProbeReportC), _vp]),
+    "mdb_upsample_conv": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(GemmProbeReportC), _vp]),
+    "mdb_attention_core": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(GemmProbeReportC), _vp]),
     "mdb_marching_tets_prepare": (_i, [_vp, _i, _i, _i, ctypes.POINTER(_vp)]),
     "mdb_marching_tets_destroy": (None, [_vp]),
     "mdb_marching_tets_info": (_i, [_vp, ctypes.POINTER(_i), ctypes.POINTER(_i)]),

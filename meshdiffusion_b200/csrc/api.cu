@@ -533,6 +533,199 @@ int mdb_conv3d_backward_prec(const void* dy, const void* x, const float* w, int 
   MDB_API_END
 }
 
+// ------------------------------------------------------------------ implicit-GEMM test entry points
+static Act probe_act(const mdb_gemm_src& s, int B) {
+  if (!s.channels || s.x <= 0 || s.y <= 0 || s.z <= 0) throw std::runtime_error("mdb: probe source needs channels and extents");
+  Act a; a.ptr = const_cast<void*>(s.ptr); a.C = s.channels; a.X = s.x; a.Y = s.y; a.Z = s.z; a.B = B; a.ld = s.ld;
+  return a;
+}
+
+static void probe_report(const GemmOp& g, mdb_gemm_probe_report* r) {
+  if (!r) return;
+  const int s = g.p.splits > 1 ? g.p.splits : 1;
+  int nk = 0;
+  for (const LoadEntry& e : g.loads) nk = e.nk > nk ? e.nk : nk;
+  r->work_items = g.p.tx * g.p.ty * g.p.tz * g.p.tb * g.p.n_tiles_n * s;
+  r->splits = s; r->ksteps = g.ksteps; r->entry_ksteps = nk; r->block_n = g.block_n;
+  r->flops = g.flops; r->fill_bytes = g.fill_bytes();
+}
+
+// Device buffers of one probe call, freed on every exit path.
+struct ProbeAllocs {
+  std::vector<void*> ptrs;
+  void* get(size_t bytes) {
+    void* p = nullptr;
+    MDB_CUDA_CHECK(cudaMalloc(&p, bytes ? bytes : 16));
+    ptrs.push_back(p);
+    return p;
+  }
+  ~ProbeAllocs() { for (void* p : ptrs) cudaFree(p); }
+};
+
+static void probe_run(GemmOp& g, int batch, cudaStream_t s) {
+  g.upload(s);
+  g.repack(s);
+  g.launch(s, batch);
+}
+
+int mdb_gemm_probe(const mdb_gemm_probe_desc* d, mdb_gemm_probe_report* report, void* stream) {
+  MDB_API_BEGIN
+  if (!d) throw std::runtime_error("mdb: null probe description");
+  cudaStream_t s = (cudaStream_t)stream;
+  const Precision pr = precision_from_int(d->precision);
+  const int Bp = d->batch_plan;
+  if (Bp < 1 || d->batch > Bp) throw std::runtime_error("mdb: probe needs 1 <= batch <= batch_plan");
+  if (d->n_src < 1 || d->n_src > 2 || d->n_extra < 0 || d->n_extra > 2) throw std::runtime_error("mdb: probe takes 1-2 sources");
+  const bool dry = d->dry != 0;
+  ProbeAllocs mem;
+  GemmOp g;
+  g.name = "probe";
+  g.set_output_strided(pr, d->x, d->y, d->z, Bp, d->n, d->out, d->osx, d->osy, d->osz, d->osb, d->out_fp32 != 0, d->lo_off);
+  std::vector<Act> srcs;
+  int ctot = 0;
+  for (int i = 0; i < d->n_src; ++i) { srcs.push_back(probe_act(d->src[i], Bp)); ctot += d->src[i].channels; }
+  int taps = 1;
+  switch (d->kind) {
+    case MDB_PROBE_CONV:
+      if (d->ksize == 1) throw std::runtime_error("mdb: probe: a 1^3 convolution is MDB_PROBE_POINTWISE");
+      g.add_conv(srcs, d->w, d->ksize, d->stride);
+      taps = d->ksize * d->ksize * d->ksize;
+      break;
+    case MDB_PROBE_CONV_UP2: {
+      if (d->n_src != 1) throw std::runtime_error("mdb: probe: the sub-pixel convolution takes one source");
+      float* w8 = nullptr;
+      if (!dry) {
+        w8 = (float*)mem.get((size_t)64 * d->n * ctot * sizeof(float));
+        launch_upconv_weights(d->w, w8, d->n, ctot, s);
+      }
+      const int par = d->parity;
+      g.add_conv_up2(srcs[0], dry ? nullptr : w8 + (size_t)par * d->n * ctot * 8, par & 1, (par >> 1) & 1, par >> 2);
+      taps = 8;
+      break;
+    }
+    case MDB_PROBE_CONV_DGRAD:
+      if (d->n_src != 1) throw std::runtime_error("mdb: probe: the data gradient takes one source");
+      g.add_conv_dgrad(srcs[0], d->w, d->n, d->ksize);
+      taps = d->ksize * d->ksize * d->ksize;
+      break;
+    case MDB_PROBE_POINTWISE:
+      g.add_pointwise(srcs, d->w, d->w_in_out != 0);
+      break;
+    case MDB_PROBE_ACT_B:
+      g.add_pointwise_w(srcs, nullptr);
+      g.set_b_activation(const_cast<void*>(d->b_ptr), d->b_k, d->b_n, Bp, d->b_row_stride, d->b_batch_stride);
+      break;
+    default:
+      throw std::runtime_error("mdb: unknown probe kind");
+  }
+  if (d->n_extra) {
+    std::vector<Act> extra;
+    for (int i = 0; i < d->n_extra; ++i) extra.push_back(probe_act(d->extra[i], Bp));
+    g.add_pointwise(extra, d->w_extra, true);
+  }
+  if (d->bias) g.set_bias(d->bias);
+  if (d->rowbias) g.set_rowbias(d->rowbias, d->rowbias_ld);
+  if (d->residual) g.set_residual(d->residual, d->res_ld, d->res_batch_stride, false);
+  if (d->stats) g.set_stats(d->stats);
+  if (d->alpha != 0.f) g.set_alpha(d->alpha);
+  // split-K sized as UNet::split_begin sizes it: from the output grid, the planned batch and the main operand's K
+  const int S = d->splits < 0 ? plan_splits(d->x, d->y, d->z, Bp, d->n, ctot, taps, pr) : d->splits;
+  g.enable_splits(S, nullptr);
+  // GroupNorm backward: the epilogue attached as UNet::gn_fuse_attach attaches it (consts [B][N] float4, per-tile partials)
+  const long long V = (long long)d->x * d->y * d->z;
+  float *consts = nullptr, *tile_part = nullptr;
+  if (d->gnb) {
+    if (d->gnb != 1 && d->gnb != 2) throw std::runtime_error("mdb: probe gnb is 0, 1 (fused) or 2 (two-pass)");
+    if (pr == kTF32) throw std::runtime_error("mdb: GroupNorm backward takes bf16 or split-bf16 operands");
+    if (d->gn_c0 + d->gn_c1 != d->n || d->osx != d->n || d->out_fp32)
+      throw std::runtime_error("mdb: GroupNorm backward needs a dense upstream gradient over the concatenation");
+  }
+  if (d->gnb == 1) {
+    if (!dry) {
+      consts = (float*)mem.get((size_t)Bp * d->n * 4 * sizeof(float));
+      tile_part = (float*)mem.get((size_t)g.gnb_rows() * d->n * 2 * sizeof(float));
+    }
+    g.set_gn_backward(d->gn_x0, d->gn_c0, d->gn_c0, d->gn_x1, d->gn_x1 ? d->gn_c1 : 0, consts, d->gn_silu, tile_part);
+  }
+  g.finalize();
+  probe_report(g, report);
+  if (dry) return 0;
+  // the scratch for the factor finalize settled on (a forced factor above the k-groups is clamped to them)
+  if (g.splits > 1) g.p.partial = (float*)mem.get((size_t)g.splits * g.p.split_stride * sizeof(float));
+  const int B = d->batch > 0 ? d->batch : Bp;
+  if (!d->gnb) {
+    probe_run(g, B, s);
+  } else {
+    GnBwdArgs a{};
+    a.x0 = d->gn_x0; a.C0 = d->gn_c0; a.ld0 = d->gn_c0;
+    a.x1 = d->gn_x1; a.C1 = d->gn_x1 ? d->gn_c1 : 0; a.ld1 = a.C1;
+    a.stats0 = d->gn_stats0; a.stats1 = d->gn_stats1; a.gamma = d->gn_gamma; a.beta = d->gn_beta;
+    a.da = d->out; a.voxels = V; a.silu = d->gn_silu; a.groups = 32; a.eps = 1e-6f;
+    const DropoutParams dp = dropout_params(d->gn_dropout);
+    a.drop_thresh = dp.thresh; a.drop_scale = dp.scale; a.seed = d->gn_seed;
+    a.sums = (float*)mem.get((size_t)Bp * d->n * 2 * sizeof(float));
+    a.dgamma = d->gn_dgamma; a.dbeta = d->gn_dbeta; a.accumulate = 0;
+    a.dx = d->gn_dx;
+    a.prec = pr;
+    if (d->gnb == 1) {
+      launch_gn_consts(a, consts, B, s);
+      g.rt_drop_thresh = dp.thresh; g.rt_drop_scale = dp.scale; g.rt_seed = d->gn_seed;
+      probe_run(g, B, s);
+      launch_gnb_tile_reduce(a, tile_part, g.gnb_tiles_per_batch_tile(), g.gnb_bb(), B, s);
+    } else {
+      probe_run(g, B, s);
+      a.part = (float*)mem.get((size_t)kBwdPartRows(Bp) * d->n * 2 * sizeof(float));
+      launch_gn_bwd_reduce(a, B, s);
+    }
+    launch_gn_bwd_apply(a, B, s);
+  }
+  MDB_CUDA_CHECK(cudaStreamSynchronize(s));
+  MDB_API_END
+}
+
+int mdb_upsample_conv(const void* x, const float* w, const float* bias, float* w8, void* out, long long* stats, int r, int C,
+                      int batch_plan, int batch, int parity_mask, int precision, int dry, mdb_gemm_probe_report* reports,
+                      void* stream) {
+  MDB_API_BEGIN
+  cudaStream_t s = (cudaStream_t)stream;
+  const Precision pr = precision_from_int(precision);
+  if (batch_plan < 1 || batch > batch_plan) throw std::runtime_error("mdb: upsample needs 1 <= batch <= batch_plan");
+  Act a; a.ptr = const_cast<void*>(x); a.C = C; a.X = a.Y = a.Z = r; a.B = batch_plan;
+  if (!dry) launch_upconv_weights(w, w8, C, C, s);
+  for (int par = 0; par < 8; ++par) {
+    GemmOp g;
+    build_upconv_parity(g, pr, a, out, w8, bias, stats, par);
+    g.finalize();
+    probe_report(g, reports ? reports + par : nullptr);
+    if (!dry && ((parity_mask >> par) & 1)) probe_run(g, batch > 0 ? batch : batch_plan, s);
+    if (!dry) MDB_CUDA_CHECK(cudaStreamSynchronize(s));  // g's device tables are freed with it
+  }
+  MDB_API_END
+}
+
+int mdb_attention_core(const void* qkv, void* vT, float* S, void* O, int V, int C, int batch_plan, int batch, int stages,
+                       int precision, int dry, mdb_gemm_probe_report* reports, void* stream) {
+  MDB_API_BEGIN
+  cudaStream_t s = (cudaStream_t)stream;
+  const Precision pr = precision_from_int(precision);
+  if (batch_plan < 1 || batch > batch_plan) throw std::runtime_error("mdb: attention needs 1 <= batch <= batch_plan");
+  const int B = batch > 0 ? batch : batch_plan;
+  GemmOp qk, pv;
+  build_attn_qk(qk, pr, V, C, batch_plan, const_cast<void*>(qkv), S);
+  build_attn_pv(pv, pr, V, C, batch_plan, S, vT, O);
+  qk.finalize();
+  pv.finalize();
+  probe_report(qk, reports);
+  probe_report(pv, reports ? reports + 1 : nullptr);
+  if (dry) return 0;
+  if (stages & 1) launch_attn_vT(pr, qkv, vT, B, V, C, s);
+  if (stages & 2) probe_run(qk, B, s);
+  if (stages & 4) launch_attn_softmax(pr, S, B, V, s);
+  if (stages & 8) probe_run(pv, B, s);
+  MDB_CUDA_CHECK(cudaStreamSynchronize(s));
+  MDB_API_END
+}
+
 int mdb_groupnorm_act_backward(const void* x, const long long* stats, const float* gamma, const float* beta, void* da,
                                const void* add, void* dx, float* dgamma, float* dbeta, int B, long long V, int C, int silu,
                                float dropout_p, unsigned long long seed, void* stream) {

@@ -57,6 +57,50 @@ void Arena::release(size_t off) {
   throw std::runtime_error("mdb: arena release of unknown block");
 }
 
+// ------------------------------------------------------------------ multi-launch composites (unet.h)
+void build_upconv_parity(GemmOp& g, Precision prec, const Act& x, void* out, const float* w8, const float* bias,
+                         long long* stats, int par) {
+  const int C = x.C, r = x.X, R = 2 * r;
+  const int px = par & 1, py = (par >> 1) & 1, pz = par >> 2;
+  const long long es = esize(prec) * parts(prec);
+  char* base = (char*)out + (((long long)pz * R + py) * R + px) * C * es;
+  g.set_output_strided(prec, r, r, r, x.B, C, base, 2LL * C, 2LL * R * C, 2LL * R * R * C, (long long)R * R * R * C, false, C);
+  g.add_conv_up2(x, w8 + (size_t)par * C * C * 8, px, py, pz);
+  g.set_bias(bias);
+  g.set_stats(stats);
+}
+
+void launch_attn_vT(Precision prec, const void* qkv, void* vT, int B, int V, int C, cudaStream_t s) {
+  const int es = esize(prec);
+  if (prec == kBF16X3) {
+    // qkv rows are [3C hi | 3C lo]; v^T rows become [V hi | V lo]
+    launch_transpose_vc(qkv, 6 * C, 2 * C, vT, B, V, C, es, s, 2 * V);
+    launch_transpose_vc(qkv, 6 * C, 5 * C, (__nv_bfloat16*)vT + V, B, V, C, es, s, 2 * V);
+  } else {
+    launch_transpose_vc(qkv, 3 * C, 2 * C, vT, B, V, C, es, s);
+  }
+}
+
+void build_attn_qk(GemmOp& g, Precision prec, int V, int C, int mb, void* qkv, float* S) {
+  const int es = esize(prec);
+  g.set_output_strided(prec, V, 1, 1, mb, V, S, V, 0, 0, (long long)V * V, true);
+  Act q; q.ptr = qkv; q.C = C; q.ld = 3 * C; q.X = V; q.Y = 1; q.Z = 1; q.B = mb;
+  g.add_pointwise_w({q}, nullptr);
+  g.set_b_activation((char*)qkv + (size_t)C * es, C, V, mb, 3 * C, (long long)V * 3 * C);
+  g.set_alpha(1.0f / std::sqrt((float)C));
+}
+
+void launch_attn_softmax(Precision prec, float* S, int B, int V, cudaStream_t s) {
+  launch_softmax_rows(S, (long long)B * V, V, prec, s);
+}
+
+void build_attn_pv(GemmOp& g, Precision prec, int V, int C, int mb, float* S, void* vT, void* O) {
+  g.set_output_strided(prec, V, 1, 1, mb, C, O, C, 0, 0, (long long)V * C, false);
+  Act pa; pa.ptr = S; pa.C = V; pa.ld = (prec == kBF16) ? 2 * V : V; pa.X = V; pa.Y = 1; pa.Z = 1; pa.B = mb;
+  g.add_pointwise_w({pa}, nullptr);
+  g.set_b_activation(vT, V, C, mb, V, (long long)C * V);
+}
+
 // ------------------------------------------------------------------ UNet plumbing
 void* UNet::dmalloc(size_t bytes, bool zero) {
   if (dry_) return nullptr;
@@ -262,15 +306,8 @@ TensP UNet::attn(const TensP& x, int midx) {
   // v^T [B][C][V] so that P.V has a K-major B operand
   TensP vT = new_act(C, R, false);
   {
-    const void* src = qkv->ptr; void* dst = vT->ptr;
-    if (prec_ == kBF16X3) {
-      // qkv rows are [3C hi | 3C lo]; v^T rows become [V hi | V lo]
-      add_step("attn" + std::to_string(midx) + ".vT", [=](cudaStream_t s, int B) {
-        launch_transpose_vc(src, 6 * C, 2 * C, dst, B, V, C, es, s, 2 * V);
-        launch_transpose_vc(src, 6 * C, 5 * C, (__nv_bfloat16*)dst + V, B, V, C, es, s, 2 * V);
-      });
-    } else
-    add_step("attn" + std::to_string(midx) + ".vT", [=](cudaStream_t s, int B) { launch_transpose_vc(src, 3 * C, 2 * C, dst, B, V, C, es, s); });
+    const void* src = qkv->ptr; void* dst = vT->ptr; const Precision pr = prec_;
+    add_step("attn" + std::to_string(midx) + ".vT", [=](cudaStream_t s, int B) { launch_attn_vT(pr, src, dst, B, V, C, s); });
   }
   // logits S[b][q][k] in fp32
   auto S = std::make_shared<Tens>();
@@ -279,19 +316,12 @@ TensP UNet::attn(const TensP& x, int midx) {
   S->ptr = at(S->off);
   TensP O = new_act(C, R, false);
   GemmOp* gqk = new_gemm("attn" + std::to_string(midx) + ".qk");
-  gqk->set_output_strided(prec_, V, 1, 1, mb, V, S->ptr, V, 0, 0, (long long)V * V, true);
-  Act q; q.ptr = qkv->ptr; q.C = C; q.ld = 3 * C; q.X = V; q.Y = 1; q.Z = 1; q.B = mb;
-  gqk->add_pointwise_w({q}, nullptr);
-  gqk->set_b_activation((char*)qkv->ptr + (size_t)C * es, C, V, mb, 3 * C, (long long)V * 3 * C);
-  gqk->set_alpha(1.0f / std::sqrt((float)C));
+  build_attn_qk(*gqk, prec_, V, C, mb, qkv->ptr, (float*)S->ptr);
   gemm_step(steps_, gqk);
   float* sp = (float*)S->ptr; const Precision pr = prec_;
-  add_step("attn" + std::to_string(midx) + ".softmax", [=](cudaStream_t s, int B) { launch_softmax_rows(sp, (long long)B * V, V, pr, s); });
+  add_step("attn" + std::to_string(midx) + ".softmax", [=](cudaStream_t s, int B) { launch_attn_softmax(pr, sp, B, V, s); });
   GemmOp* gpv = new_gemm("attn" + std::to_string(midx) + ".pv");
-  gpv->set_output_strided(prec_, V, 1, 1, mb, C, O->ptr, C, 0, 0, (long long)V * C, false);
-  Act pa; pa.ptr = S->ptr; pa.C = V; pa.ld = (prec_ == kBF16) ? 2 * V : V; pa.X = V; pa.Y = 1; pa.Z = 1; pa.B = mb;
-  gpv->add_pointwise_w({pa}, nullptr);
-  gpv->set_b_activation(vT->ptr, V, C, mb, V, (long long)C * V);
+  build_attn_pv(*gpv, prec_, V, C, mb, (float*)S->ptr, vT->ptr, O->ptr);
   gemm_step(steps_, gpv);
   if (!train_) arena_.release(S->off);
   { arena_.release(vT->off); vT->live = false; }  // backward multiplies by v itself (K-major there), not by v^T
@@ -338,18 +368,11 @@ TensP UNet::upsample(const TensP& x, int midx) {
     // (8/27 of the FLOPs) writing its strided share of the output; the upsampled tensor never exists. The training plan
     // keeps the materialised form below (its backward differentiates exactly that graph).
     TensP out = new_act(C, R, true);
-    const int r = x->R, mb = cfg_.max_batch;
     float* w8 = (float*)dmalloc((size_t)64 * C * C * sizeof(float));
     commit_steps_.push_back({"upw:" + pre, [=](cudaStream_t s, int) { launch_upconv_weights(w, w8, C, C, s); }});
-    const long long es = esize(prec_) * parts(prec_);
     for (int par = 0; par < 8; ++par) {
-      const int px = par & 1, py = (par >> 1) & 1, pz = par >> 2;
       GemmOp* g = new_gemm("up" + std::to_string(midx) + ".conv.p" + std::to_string(par));
-      char* base = (char*)out->ptr + (((long long)pz * R + py) * R + px) * C * es;
-      g->set_output_strided(prec_, r, r, r, mb, C, base, 2LL * C, 2LL * R * C, 2LL * R * R * C, (long long)R * R * R * C, false, C);
-      g->add_conv_up2(act_of(x), w8 + (size_t)par * C * C * 8, px, py, pz);
-      g->set_bias(b);
-      g->set_stats(out->stats);
+      build_upconv_parity(*g, prec_, act_of(x), out->ptr, w8, b, out->stats, par);
       gemm_step(steps_, g);
     }
     return out;

@@ -76,6 +76,20 @@ struct Tens {
 };
 typedef std::shared_ptr<Tens> TensP;
 
+// Multi-launch composites of the forward plan. The engine and the test entry points (api.cu) both build them here, so a
+// test of one runs the engine's construction.
+// Sub-pixel Upsample + conv3^3, output-parity class par = px | py << 1 | pz << 2: a 2^3 convolution over the
+// low-resolution x ([x.B][r^3][C]) with that class's share of the folded weights w8 (launch_upconv_weights), writing its
+// strided sites of out, the high-resolution [x.B][(2r)^3][C] tensor; stats summed over the 8 classes.
+void build_upconv_parity(GemmOp& g, Precision prec, const Act& x, void* out, const float* w8, const float* bias,
+                         long long* stats, int par);
+// AttnBlock core over qkv rows [mb][V][3C] (q | k | v): v^T [mb][C][V] (the K-major B operand of P.v), the fp32 logits
+// S = q.k^T / sqrt(C) [mb][V][V], their row softmax in place, O = P.v [mb][V][C].
+void launch_attn_vT(Precision prec, const void* qkv, void* vT, int B, int V, int C, cudaStream_t s);
+void build_attn_qk(GemmOp& g, Precision prec, int V, int C, int mb, void* qkv, float* S);
+void launch_attn_softmax(Precision prec, float* S, int B, int V, cudaStream_t s);
+void build_attn_pv(GemmOp& g, Precision prec, int V, int C, int mb, float* S, void* vT, void* O);
+
 class UNet {
  public:
   // The plan is built twice by the same code: a dry pass without the GPU (it sizes the arena; the pointers it records

@@ -5,8 +5,8 @@ bf16 and bf16x3 128-column tiles store each 64-column round as one TMA box from 
 residual the same way; TMA clips the box at the grid, the batch and N. tf32 keeps the per-thread stores. Every case
 compares against an fp64 reference at the gates of test_gpu_conv.py, and checks that nothing outside the output tensor
 was written: the output sits between two guard regions of a larger buffer, filled with a sentinel. Channel-offset
-outputs (the attention's qkv rows) and the sub-pixel upsample's parity-strided outputs run inside the full network
-(test_gpu_unet.py).
+outputs (the attention's qkv rows) and the sub-pixel upsample's parity-strided outputs have their own cases in
+test_gpu_gemm_variants.py.
 """
 import pytest
 import torch
